@@ -187,6 +187,7 @@ struct NvbMapper {
   unsigned char* xslab = nullptr;  // exchange-slab wavefront (esdf_persistent == 3): 2 x capacity ESDF blocks
   int* xrec = nullptr;             // ... 2 x CTAs x xseg candidate records of 32 ints ...
   int xseg = 0;
+  int xseg_grid = 0;               // CTAs of the exchange-slab launch the segments were sized for
   int* xcounts = nullptr;          // ... and 2 x CTAs count pairs
   int* cand_stamp = nullptr;
   // decay integrators
@@ -340,6 +341,21 @@ int growLayer(NvbMapper* m, DevLayer* L, int new_capacity) {
   return NVB_OK;
 }
 
+// Candidate records of the exchange-slab wavefront: one segment per CTA of the launch, by ring parity. In a ring a CTA
+// processes at most ceil(cap / CTAs) members (seeds or candidates, dealt round-robin) and registers at most 6 face neighbours
+// for each; the single-CTA tail registers at most 6 per group. So the segment is sized for the grid the launch really uses,
+// which shrinks as SMs are reserved.
+int allocWaveXRecords(NvbMapper* m, int cap) {
+  const int grid = esdfWaveXGrid(m->num_sms, m->esdf_reserved_sms);
+  NVB_CUDA(syncAll(m));
+  if (m->xrec) cudaFree(m->xrec);
+  m->xrec = nullptr;
+  m->xseg = 6 * ((cap + grid - 1) / grid) + 64;
+  m->xseg_grid = grid;
+  NVB_CUDA(cudaMalloc(&m->xrec, 2 * (size_t)grid * m->xseg * 32 * sizeof(int)));
+  return NVB_OK;
+}
+
 int allocEsdfScratch(NvbMapper* m, int old_cap, int cap) {
   int rc;
   if ((rc = reallocCopy(&m->work, 0, (size_t)cap, false, m->stream))) return rc;
@@ -389,13 +405,10 @@ int allocEsdfScratch(NvbMapper* m, int old_cap, int cap) {
     // exchange-slab wavefront: two slabs by ring parity + the candidate records (contents only live inside one launch)
     NVB_CUDA(syncAll(m));
     if (m->xslab) cudaFree(m->xslab);
-    if (m->xrec) cudaFree(m->xrec);
-    m->xslab = nullptr, m->xrec = nullptr;
+    m->xslab = nullptr;
     NVB_CUDA(cudaMalloc(&m->xslab, 2 * (size_t)cap * kEsdfBlockBytes));
-    // A CTA registers at most 6 candidates per candidate it owns, i.e. <= 6 * ceil(cap / CTAs) < cap / 16 + 64 per ring.
-    const int ctas = std::min(m->num_sms, esdfWaveXMaxCtas());
-    m->xseg = cap / 16 + 64;
-    NVB_CUDA(cudaMalloc(&m->xrec, 2 * (size_t)ctas * m->xseg * 32 * sizeof(int)));
+    int rc;
+    if ((rc = allocWaveXRecords(m, cap))) return rc;
     if (!m->xcounts) {
       NVB_CUDA(cudaMalloc(&m->xcounts, esdfWaveXFlagBytes()));
       NVB_CUDA(cudaMemsetAsync(m->xcounts, 0, esdfWaveXFlagBytes(), m->stream));
@@ -686,6 +699,7 @@ int checkDeviceError(NvbMapper* m) {
     cudaStreamSynchronize(m->stream);
     if (err & 2) return fail(NVB_ERR_INDEX_RANGE, "a block index does not fit the 21-bit hash key");
     if (err & 4) return fail(NVB_ERR_CAPACITY, "a block-list segment of the multi-GPU merge overflowed (nvb_mapper_append_frame_blocks)");
+    if (err & 8) return fail(NVB_ERR_CAPACITY, "a candidate-record segment of the exchange-slab ESDF wavefront overflowed");
     // Roll the overflow back: find-or-insert left the keys it could not serve in the hash (value -1) and the fill level
     // above the capacity. Clamp the level and rebuild the hashes from the live slots, so that the same indices can be
     // allocated again once the caller has made room (or after the next growth).
@@ -2468,6 +2482,7 @@ int32_t nvb_mapper_set_esdf_reserved_sms(NvbMapper* m, int32_t reserved_sms) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
   if (reserved_sms < 0 || reserved_sms > 64) return fail(NVB_ERR_INVALID_ARGUMENT, "reserved_sms must be in [0, 64]");
   m->esdf_reserved_sms = reserved_sms;
+  if (m->xrec && esdfWaveXGrid(m->num_sms, reserved_sms) != m->xseg_grid) return allocWaveXRecords(m, m->esdf.capacity);
   return NVB_OK;
 }
 int32_t nvb_mapper_get_esdf_reserved_sms(const NvbMapper* m) { return m ? m->esdf_reserved_sms : 0; }

@@ -112,6 +112,7 @@ struct XCtx {
   unsigned char* X[2];    // exchange slabs by ring parity
   int* recs[2];           // candidate records by ring parity: one segment of `seg` records per CTA
   int seg;
+  int* error;             // bit 8: a registration did not fit its CTA's segment (dropped, the launch's result is invalid)
   float max_sq;
   __device__ __forceinline__ int* segment(int p, int cta) const { return recs[p] + (size_t)cta * seg * kRecInts; }
 };
@@ -511,7 +512,7 @@ __device__ __forceinline__ RegState registerBegin(const XCtx& c, XShared& xs, in
   }
   return s;
 }
-__device__ __forceinline__ void registerClaim(XShared& xs, RegState& s, int group, int lane64, int target) {
+__device__ __forceinline__ void registerClaim(const XCtx& c, XShared& xs, RegState& s, int group, int lane64, int target) {
   if (lane64 < 32) {  // the group's first warp
     const bool win = lane64 < 6 && xs.nb[group][lane64] >= 0 && s.old != target;
     const unsigned int ballot = __ballot_sync(0xffffffffu, win);
@@ -520,6 +521,11 @@ __device__ __forceinline__ void registerClaim(XShared& xs, RegState& s, int grou
       if (lane64 == 0) base = atomicAdd(&xs.ncand, __popc(ballot));
       base = __shfl_sync(0xffffffffu, base, 0);
       if (win) s.pos = base + __popc(ballot & ((1u << lane64) - 1u));
+      // Never write past the segment (the next CTA's records follow it): the registration is dropped and reported.
+      if (s.pos >= c.seg) {
+        s.pos = -1;
+        atomicOr(c.error, 8);
+      }
     }
   }
 }
@@ -583,7 +589,7 @@ __device__ __noinline__ void processCandidate(const XCtx& c, const XTables& tab,
     groupSync(group);
     RegState rs = registerBegin(c, xs, group, lane64, ring + 1);
     sweepBlockX(R, group, lane64, c.max_sq);
-    registerClaim(xs, rs, group, lane64, ring + 1);
+    registerClaim(c, xs, rs, group, lane64, ring + 1);
     groupSync(group);
     X_PROF(4)
     ownStore(c.blocks + (size_t)slot * kEsdfBlockBytes, true, c.X[ni] + (size_t)slot * kEsdfBlockBytes, R, c.psum + 2 * (size_t)slot, lane64);
@@ -611,7 +617,7 @@ __device__ __noinline__ void processSeed(const XCtx& c, XShared& xs, unsigned in
   ownToShared(R, own, lane64);
   groupSync(group);
   const bool ch = sweepBlockX(R, group, lane64, c.max_sq);
-  registerClaim(xs, rs, group, lane64, ring);
+  registerClaim(c, xs, rs, group, lane64, ring);
   if (ch) xs.changed[group] = 1;
   groupSync(group);
   // (an unchanged block keeps its parent box)
@@ -625,10 +631,10 @@ __device__ __noinline__ void processSeed(const XCtx& c, XShared& xs, unsigned in
 // arrival counter polled by thread 0, fence, then one read of the per-CTA slots. (The alternative -- one flag per CTA, every
 // CTA polling every other CTA's flag -- needs no read-modify-write on a shared word but grows with the square of the grid.)
 __device__ __forceinline__ void counterBarrierScan(XShared& xs, unsigned int* bar, unsigned int& generation, int2* counts, int nctas,
-                                                   int cta, int tid, int* K, int* M) {
+                                                   int cta, int tid, int seg, int* K, int* M) {
   __syncthreads();
   if (tid == 0) {
-    __stcg(counts + cta, make_int2(xs.ncand, xs.nchanged));
+    __stcg(counts + cta, make_int2(min(xs.ncand, seg), xs.nchanged));  // (registrations past the segment were dropped)
     xs.ncand = 0, xs.nchanged = 0;
   }
   gridBarrier(bar, generation, nctas);
@@ -676,7 +682,7 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
     xc.stamp[0] = c.stamp_a, xc.stamp[1] = c.stamp_b;
     xc.X[0] = c.xslab, xc.X[1] = c.xslab + (size_t)c.esdf.capacity * kEsdfBlockBytes;
     xc.recs[0] = c.xrec, xc.recs[1] = c.xrec + (size_t)nctas * c.xseg * kRecInts;
-    xc.seg = c.xseg, xc.max_sq = c.max_sq;
+    xc.seg = c.xseg, xc.error = c.error, xc.max_sq = c.max_sq;
   }
   __syncthreads();
   XState st;
@@ -716,7 +722,7 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
   unsigned int generation = 0;
 #define X_BARRIER(Kout, Mout)                                                                                                    \
   X_TIME_WORK()                                                                                                                  \
-  counterBarrierScan(xs, c.barrier, generation, count_base + (n_bar & 1) * kMaxCtas, nctas, cta, tid, &(Kout), &(Mout));             \
+  counterBarrierScan(xs, c.barrier, generation, count_base + (n_bar & 1) * kMaxCtas, nctas, cta, tid, c.xseg, &(Kout), &(Mout));             \
   X_TIME_BARRIER()                                                                                                               \
   n_bar++;
   for (int pass = 0; pass < 2; pass++) {
@@ -752,7 +758,7 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
           while (true) {
             if (group < K) processCandidate(xc, tab, xs, R, st.ring, xs.seg[group][0], xs.seg[group][1], 0, group, lane64, prof);
             __syncthreads();
-            const int K2 = xs.ncand, M2 = xs.nchanged;
+            const int K2 = min(xs.ncand, c.xseg), M2 = xs.nchanged;
             __syncthreads();
             if (tid == 0) xs.ncand = 0, xs.nchanged = 0;
             if (tid < kXG) xs.seg[tid][0] = 0, xs.seg[tid][1] = tid;  // the next ring's entries: segment 0, in order
@@ -826,7 +832,11 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
 
 }  // namespace
 
-int esdfWaveXMaxCtas() { return kMaxCtas; }
+int esdfWaveXGrid(int num_sms, int reserved_sms) {
+  int grid = num_sms < kMaxCtas ? num_sms : kMaxCtas;
+  if (reserved_sms > 0 && grid - reserved_sms >= 8) grid -= reserved_sms;
+  return grid;
+}
 size_t esdfWaveXFlagBytes() { return 2 * (size_t)kMaxCtas * sizeof(int2); }
 
 cudaError_t launchEsdfComputeX(const EsdfCtx& c, int num_sms, int reserved_sms, cudaStream_t stream, int* launches) {
@@ -846,8 +856,7 @@ cudaError_t launchEsdfComputeX(const EsdfCtx& c, int num_sms, int reserved_sms, 
   // limit, NVB_WAVEX_RESERVED_SMS = 0 / 2 / 4 / 8, two runs each: 2367, 2339 / 2404, 2407 / 2399, 2378 / 2379, 2336 frames/s),
   // and a multi-GPU rank's NCCL all-gather can start -- and wait for its peers -- while a wavefront is in flight (a
   // cooperative grid that fills every SM serialises the two).
-  int grid = num_sms < kMaxCtas ? num_sms : kMaxCtas;
-  if (reserved_sms > 0 && grid - reserved_sms >= 8) grid -= reserved_sms;
+  const int grid = esdfWaveXGrid(num_sms, reserved_sms);
   return cudaLaunchCooperativeKernel((const void*)esdfWaveXKernel, dim3(grid), dim3(kXT), args, kXSmemBytes, stream);
 }
 

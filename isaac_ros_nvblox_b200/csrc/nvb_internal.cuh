@@ -426,7 +426,7 @@ int launchEsdfClear(const EsdfCtx& c, int esdf_count_upper, int num_sms, cudaStr
 cudaError_t launchEsdfComputeGes(const EsdfCtx& c, int num_sms, cudaStream_t stream, int* launches);
 cudaError_t launchEsdfComputePersistent(const EsdfCtx& c, int num_sms, cudaStream_t stream, int* launches);
 cudaError_t launchEsdfComputeX(const EsdfCtx& c, int num_sms, int reserved_sms, cudaStream_t stream, int* launches);  // nvb_esdf_wavex.cu
-int esdfWaveXMaxCtas();
+int esdfWaveXGrid(int num_sms, int reserved_sms);  // CTAs of an exchange-slab launch
 size_t esdfWaveXFlagBytes();
 // Reference-like driver: one launch per phase, host reads the ring counter.
 cudaError_t runEsdfComputeHostLoop(const EsdfCtx& c, int num_sms, cudaStream_t stream, int* launches);

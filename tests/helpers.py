@@ -238,6 +238,97 @@ def assert_color_equal(gpu_layer, cpu_layer):
             raise AssertionError(("weight", k, len(bad), bad[:3], g["weight"][tuple(bad[0])], c["weight"][tuple(bad[0])]))
 
 
+def _remove_distortion(x_in, y_in, radial, tangential):
+    """removeDistortion (nvb_internal.cuh): Newton-Raphson in double, at most 6 iterations."""
+    k1, k2, k3, k4, k5, k6 = (float(np.float32(k)) for k in radial)
+    p1, p2 = (float(np.float32(p)) for p in tangential)
+    x, y = float(x_in), float(y_in)
+    for _ in range(6):
+        r2 = x * x + y * y
+        q, q2, q3 = r2, r2 * r2, r2 * r2 * r2
+        R = (1.0 + k1 * r2 + k2 * q2 + k3 * q3) / (1.0 + k4 * r2 + k5 * q2 + k6 * q3)
+        ex = x * R + 2.0 * p1 * x * y + p2 * (r2 + 2.0 * x * x) - x_in
+        ey = y * R + 2.0 * p2 * x * y + p1 * (r2 + 2.0 * y * y) - y_in
+        ja, jc = k1 + 2. * k2 * q + 3. * k3 * q2, k4 + 2. * k5 * q + 3. * k6 * q2
+        jb, jd = k4 * q + k5 * q2 + k6 * q3 + 1., k1 * q + k2 * q2 + k3 * q3 + 1.
+        dR = (ja * jb - jc * jd) / (jb * jb)
+        a = R + x * 2.0 * x * dR + 2 * p1 * y + 6 * p2 * x
+        b = x * 2.0 * y * dR + 2 * p1 * x + 2 * p2 * y
+        c = y * 2.0 * x * dR + 2 * p2 * y + 2 * p1 * x
+        d = R + y * 2.0 * y * dR + 2 * p2 * x + 6 * p1 * y
+        det = a * d - b * c
+        dx, dy = (d * ex - b * ey) / det, (-c * ex + a * ey) / det
+        if np.isfinite(dx) and np.isfinite(dy):
+            x, y = x - dx, y - dy
+        if dx * dx + dy * dy < 1e-20:
+            break
+    return np.float32(x), np.float32(y)
+
+
+def view_grid(fu, fv, cu, cv, width, height, T_L_C, block_size, max_dist, radial=None, tangential=None, workspace=None):
+    """computeViewGrid (nvb_api.cu) in binary32: Camera::getViewAABB (the four corner rays of the image plane at depth 0
+    and max_dist, transformed into the layer frame, min / max), the workspace clip (None, ("height", zmin, zmax) or
+    ("box", lo3, hi3)) and the floor(p / block_size) block-index AABB.
+    -> (min block index (3,) int64, size (3,) int64, cells) or None when the clipped AABB is empty."""
+    f32 = np.float32
+    T = np.asarray(T_L_C, f32)
+    R, t = T[:3, :3], T[:3, 3]
+    corners = []
+    for u, v in ((0.0, 0.0), (width, 0.0), (width, height), (0.0, height)):
+        nx, ny = (f32(u) - f32(cu)) / f32(fu), (f32(v) - f32(cv)) / f32(fv)
+        if radial is not None or tangential is not None:
+            nx, ny = _remove_distortion(nx, ny, radial or (0,) * 6, tangential or (0, 0))
+        for d in (f32(0.0), f32(max_dist)):
+            p = np.array([d * nx, d * ny, d * f32(1.0)], f32)
+            # translation + linear * p, the row sums in Eigen's a0 + (a1 + a2) order
+            corners.append([t[i] + (R[i, 0] * p[0] + (R[i, 1] * p[1] + R[i, 2] * p[2])) for i in range(3)])
+    P = np.array(corners, f32)
+    lo, hi = P.min(axis=0), P.max(axis=0)
+    if workspace is not None:
+        if workspace[0] == "height":
+            lo[2], hi[2] = max(lo[2], f32(workspace[1])), min(hi[2], f32(workspace[2]))
+        else:
+            lo = np.maximum(np.asarray(workspace[1], f32), lo)
+            hi = np.minimum(np.asarray(workspace[2], f32), hi)
+    if np.any(lo > hi):
+        return None
+    bs = f32(block_size)
+    mn = np.floor(lo / bs).astype(np.int64)
+    mx = np.floor(hi / bs).astype(np.int64)
+    size = mx - mn + 1
+    return mn, size, int(np.prod(size))
+
+
+def validate_esdf(layer, max_sq):
+    """validateEsdf (tests/test_esdf_integrator.cpp:340-460) on a {block index: ESDF block} layer: sites have distance 0 and
+    no parent; a parent direction's squared length is the distance and it points at a site; voxels without a parent sit at
+    the maximum distance. -> (observed voxels, sites)."""
+    keys = np.array(list(layer))
+    lo, hi = keys.min(0), keys.max(0)
+    shape = tuple((hi - lo + 1) * 8)
+    fields = ("squared_distance_vox", "parent_direction", "is_site", "observed")
+    d = {f: np.zeros(shape + ((3,) if f == "parent_direction" else ()), layer[tuple(keys[0])][f].dtype) for f in fields}
+    have = np.zeros(shape, bool)
+    for k, blk in layer.items():
+        o = (np.asarray(k) - lo) * 8
+        sl = (slice(o[0], o[0] + 8), slice(o[1], o[1] + 8), slice(o[2], o[2] + 8))
+        have[sl] = True
+        for f in fields:
+            d[f][sl] = blk[f]
+    obs, site = d["observed"].astype(bool), d["is_site"].astype(bool)
+    sq, p = d["squared_distance_vox"], d["parent_direction"].astype(np.int64)
+    has_parent = p.any(axis=-1)
+    assert np.all(sq[site & obs] == 0.0) and not has_parent[site & obs].any()
+    w = obs & ~site & has_parent
+    assert np.all(sq[w] == (p[w] ** 2).sum(-1).astype(np.float32))
+    pos = np.argwhere(w) + p[w]
+    assert (pos >= 0).all() and (pos < np.array(have.shape)).all()
+    assert site[pos[:, 0], pos[:, 1], pos[:, 2]].all(), "parent must be a site"
+    n = obs & ~site & ~has_parent
+    assert np.all(sq[n] >= max_sq - 1e-3)
+    return int(obs.sum()), int(site.sum())
+
+
 def textured_image(rows, cols, seed=0):
     """A smooth-plus-noise RGB test image."""
     rng = np.random.default_rng(seed)

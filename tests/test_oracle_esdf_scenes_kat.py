@@ -4,7 +4,7 @@ with its compareEsdfToGt / compareEsdfToEsdf / validateEsdf checks (:238-460) ve
 import numpy as np
 import pytest
 
-from helpers import tsdf_layer_from_distance
+from helpers import tsdf_layer_from_distance, validate_esdf
 from oracle import oracle as orc
 
 VOXEL, MAX_DIST = 0.1, 4.0
@@ -77,24 +77,6 @@ def _signed(d):
     return np.where(d["is_inside"].astype(bool), -dist, dist)
 
 
-def _validate(layer, max_sq):
-    """validateEsdf (:340-460): sites have distance 0 and no parent; a parent direction's squared length is the distance and it
-    points at a site; voxels without a parent sit at the maximum distance."""
-    lo, have, d = _dense(layer, ("squared_distance_vox", "parent_direction", "is_inside", "observed", "is_site"))
-    obs, site = d["observed"].astype(bool), d["is_site"].astype(bool)
-    sq, p = d["squared_distance_vox"], d["parent_direction"].astype(np.int64)
-    has_parent = p.any(axis=-1)
-    assert np.all(sq[site & obs] == 0.0) and not has_parent[site & obs].any()
-    w = obs & ~site & has_parent
-    assert np.all(sq[w] == (p[w] ** 2).sum(-1).astype(np.float32))
-    pos = np.argwhere(w) + p[w]
-    assert (pos >= 0).all() and (pos < np.array(have.shape)).all()
-    assert site[pos[:, 0], pos[:, 1], pos[:, 2]].all(), "parent must be a site"
-    n = obs & ~site & ~has_parent
-    assert np.all(sq[n] >= max_sq - 1e-3)
-    return int(obs.sum()), int(site.sum())
-
-
 @pytest.mark.parametrize("name", list(OBSTACLES))
 def test_single_esdf_against_ground_truth(name):
     """SingleEsdfTestGPU (:511-552): ESDF of the ground-truth TSDF vs the ground-truth SDF up to the maximum distance: at most
@@ -106,7 +88,7 @@ def test_single_esdf_against_ground_truth(name):
     ep = orc.default_esdf_params(max_esdf_distance_m=MAX_DIST, min_weight=1.0)
     m.integrate_esdf(idx, ep)
     layer = m.esdf_layer()
-    n_obs, n_site = _validate(layer, (MAX_DIST / VOXEL) ** 2)
+    n_obs, n_site = validate_esdf(layer, (MAX_DIST / VOXEL) ** 2)
     assert n_obs > 100000 and n_site > 1000
     gt_layer = {tuple(int(c) for c in k): v for k, v in zip(idx, gt)}
     over = total = 0
@@ -136,7 +118,7 @@ def test_all_freespace(name):
         else:
             m.integrate_esdf_with_freespace(idx, ep)
         layer = m.esdf_layer()
-        n_obs, n_site = _validate(layer, (MAX_DIST / VOXEL) ** 2)
+        n_obs, n_site = validate_esdf(layer, (MAX_DIST / VOXEL) ** 2)
         assert n_obs > 1000 and n_site == 0
         for blk in layer.values():
             obs = blk["observed"].astype(bool)
@@ -160,7 +142,7 @@ def test_actual_freespace(name):
             plain.integrate_esdf(idx, ep)
             withfs.integrate_esdf_with_freespace(idx, ep)
         a, b = withfs.esdf_layer(), plain.esdf_layer()
-        _validate(a, (MAX_DIST / VOXEL) ** 2)
+        validate_esdf(a, (MAX_DIST / VOXEL) ** 2)
         over = total = 0
         for k, blk in a.items():
             if k not in b:
@@ -215,7 +197,7 @@ def test_incremental_esdf_with_object_removal(name, thin):
     inc = m.esdf_layer()
     frac, total = _compare_esdf(inc, batch.esdf_layer(), VOXEL)
     assert total > 5000 and frac <= SMALL_CUTOFF, (frac, total)
-    _validate(inc, (MAX_DIST / VOXEL) ** 2)
+    validate_esdf(inc, (MAX_DIST / VOXEL) ** 2)
     if name != "box":  # the obstacle's sites are really gone
         obstacle_only = fn(np.array([[0.0, 0.0, 2.0]], np.float32))[0] < 0
         assert obstacle_only
@@ -250,8 +232,8 @@ def test_incremental_esdf_slice_with_object_removal(name):
     assert total > 5000 and frac <= SMALL_CUTOFF, (frac, total)
     frac, total = _compare_esdf(mo.esdf_layer(), b, 1.5 * VOXEL, negative=False)
     assert total > 5000 and frac <= SMALL_CUTOFF, (frac, total)
-    _validate(mt.esdf_layer(), (MAX_DIST / VOXEL) ** 2)
-    _validate(mo.esdf_layer(), (MAX_DIST / VOXEL) ** 2)
+    validate_esdf(mt.esdf_layer(), (MAX_DIST / VOXEL) ** 2)
+    validate_esdf(mo.esdf_layer(), (MAX_DIST / VOXEL) ** 2)
 
 
 def test_slice_image_of_an_empty_layer():
@@ -288,7 +270,7 @@ def test_complex_scene_with_tsdf(name):
     ep = orc.default_esdf_params(max_esdf_distance_m=MAX_DIST, min_weight=1.0)
     m.integrate_esdf(m.tsdf_block_indices(), ep)
     layer = m.esdf_layer()
-    _validate(layer, (MAX_DIST / VOXEL) ** 2)
+    validate_esdf(layer, (MAX_DIST / VOXEL) ** 2)
     idx, gt = tsdf_layer_from_distance(fn, aabb[0], aabb[1], VOXEL, MAX_DIST)
     gt_layer = {tuple(int(c) for c in k): v for k, v in zip(idx, gt)}
     over = total = 0
@@ -322,4 +304,4 @@ def test_incremental_tsdf_and_esdf_with_object_removal(name):
     batch.integrate_esdf(m.tsdf_block_indices(), ep)
     frac, total = _compare_esdf(m.esdf_layer(), batch.esdf_layer(), VOXEL)
     assert total > 1000 and frac <= SMALL_CUTOFF, (frac, total)  # (min_weight = 1 leaves only the voxels near the camera)
-    _validate(m.esdf_layer(), (MAX_DIST / VOXEL) ** 2)
+    validate_esdf(m.esdf_layer(), (MAX_DIST / VOXEL) ** 2)

@@ -1,0 +1,128 @@
+"""Preconditions of tests/test_gpu_scale_edges.py, checkable without a GPU: every configuration there sits at least 20 %
+beyond the threshold whose branch it is meant to run (tests/scale_edge_cases.py), the numpy restatement of the view AABB
+contains every block the oracle's raycast returns, and the far-from-origin tolerances hold on the oracle."""
+import numpy as np
+import pytest
+
+import scale_edge_cases as sec
+from helpers import cameras, validate_esdf
+from isaac_ros_nvblox_b200 import synthetic as syn
+
+
+def _on_side(cells, path):
+    if path == "smem":
+        assert cells * sec.MARGIN <= sec.SMEM_CELLS, (cells, sec.SMEM_CELLS)
+    elif path == "global":
+        assert cells >= sec.MARGIN * sec.SMEM_CELLS, (cells, sec.SMEM_CELLS)
+        assert cells * sec.MARGIN <= sec.CHAINED_CELLS, (cells, sec.CHAINED_CELLS)
+    else:
+        assert cells >= sec.MARGIN * sec.CHAINED_CELLS, (cells, sec.CHAINED_CELLS)
+
+
+@pytest.mark.parametrize("name", [c["name"] for c in sec.VIEW_CASES])
+def test_view_case_crosses_its_threshold_and_contains_the_oracle_blocks(name):
+    from oracle import oracle as orc
+    case = sec.VIEW[name]
+    mn, size, cells = sec.case_cells(case)
+    _on_side(cells, case["path"])
+    _, _, ocam = cameras(case["width"], case["height"], radial=case.get("radial"), tangential=case.get("tangential"))
+    p = orc.default_tsdf_params(max_integration_distance_m=case["max_dist"])
+    got = orc.view_raycast(sec.random_depth(case, 0), case["pose"], ocam, 8 * case["voxel"], 4 * case["voxel"], p, cap=cells)
+    assert len(got) > cells // 20  # the marks spread over the AABB
+    assert np.all(got >= mn) and np.all(got < mn + size)
+
+
+def test_small_view_and_integrate_cases_cross_their_thresholds():
+    _on_side(sec.case_cells(sec.SMALL_VIEW)[2], "smem")
+    for case in sec.INTEGRATE_2CM:
+        _on_side(sec.case_cells(case)[2], "global")
+    cells = sec.case_cells(sec.INTEGRATE_CHAINED)[2]
+    _on_side(cells, "chained")
+    # one frame of this many cells grows the TSDF slab to 2^22 blocks (16 GiB), not 2^23
+    assert cells < sec.TSDF_SLAB_LIMIT_CELLS
+    assert sec.union_cells() >= sec.MARGIN * sec.CHAINED_CELLS
+    a, b = sec.union_lists()
+    u = np.unique(np.concatenate([a, b]), axis=0)
+    assert np.array_equal(u.min(0), sec.UNION_BOX[0]) and np.array_equal(u.max(0), sec.UNION_BOX[1])
+
+
+def _observed_voxels(layer):
+    """-> (global voxel indices (n, 3) int64, distances (n,)) of the voxels with weight > 0."""
+    keys, dist = [], []
+    for k, b in layer.items():
+        v = np.argwhere(b["weight"] > 0)
+        keys.append(np.asarray(k, np.int64) * 8 + v)
+        dist.append(b["distance"][v[:, 0], v[:, 1], v[:, 2]])
+    return np.concatenate(keys), np.concatenate(dist)
+
+
+def far_origin_differences(far_layer, origin_layer, offset, voxel):
+    """|TSDF distance differences| of the voxels observed in both maps, matched by the voxel-index shift offset / voxel,
+    and the fraction of the origin map's observed voxels that were matched."""
+    shift = np.round(np.asarray(offset, np.float64) / voxel).astype(np.int64)
+    kf, df = _observed_voxels(far_layer)
+    ko, do = _observed_voxels(origin_layer)
+    kf = kf - shift
+    base = np.minimum(kf.min(0), ko.min(0))
+    ext = np.maximum(kf.max(0), ko.max(0)) - base + 1
+
+    def lin(k):
+        k = k - base
+        return (k[:, 2] * ext[1] + k[:, 1]) * ext[0] + k[:, 0]
+
+    lf, lo = lin(kf), lin(ko)
+    common, i_f, i_o = np.intersect1d(lf, lo, assume_unique=True, return_indices=True)
+    return np.abs(df[i_f].astype(np.float64) - do[i_o].astype(np.float64)), len(common) / len(lo)
+
+
+def far_origin_bounds(offset):
+    """Median and 99th-percentile bounds on those differences: the float32 spacing at the offset is the rounding step of a
+    voxel centre and of the camera's position there."""
+    spacing = float(np.spacing(np.float32(np.max(np.abs(offset)))))
+    return 0.5 * spacing, 2.0 * spacing
+
+
+FAR_SEQ = dict(width=320, height=240, voxel=0.05, frames=3)
+
+
+def far_frames():
+    cs, cam, ocam = cameras(FAR_SEQ["width"], FAR_SEQ["height"])
+    return syn.make_sequence(syn.sphere_in_box(), cs, syn.circle_trajectory(40)[:FAR_SEQ["frames"]]), cam, ocam
+
+
+@pytest.mark.parametrize("offset", sec.FAR_OFFSETS)
+def test_far_origin_map_matches_the_origin_map_on_the_oracle(offset):
+    """The oracle's map integrated kilometres from the origin equals its map at the origin up to float32 rounding at the
+    offset (same depth images, poses shifted by a whole number of voxels)."""
+    from oracle import oracle as orc
+    frames, _, ocam = far_frames()
+    near, far = orc.OracleMap(FAR_SEQ["voxel"]), orc.OracleMap(FAR_SEQ["voxel"])
+    for d, T in frames:
+        near.integrate_depth(d, T, ocam)
+        far.integrate_depth(d, sec.shifted(T, offset), ocam)
+    diff, matched = far_origin_differences(far.tsdf_layer(), near.tsdf_layer(), offset, FAR_SEQ["voxel"])
+    med, p99 = far_origin_bounds(offset)
+    assert matched > 0.995
+    assert np.median(diff) <= med and np.percentile(diff, 99) <= p99, (np.median(diff), np.percentile(diff, 99), med, p99)
+    assert np.any(np.abs(far.tsdf_block_indices()) > 5000)  # large block indices
+
+
+def test_key_limit_blocks_are_at_the_limit():
+    for idx in sec.key_limit_block_sets():
+        assert np.all(idx >= -sec.KEY_LIMIT) and np.all(idx < sec.KEY_LIMIT)
+        assert np.any(idx == sec.KEY_LIMIT - 1) or np.any(idx == -sec.KEY_LIMIT)
+
+
+def test_long_range_scene_has_parents_beyond_15_blocks_on_the_oracle():
+    from oracle import oracle as orc
+    o = orc.OracleMap(sec.LR_VOXEL)
+    ep = orc.default_esdf_params(max_esdf_distance_m=sec.LR_MAX_DIST)
+    for i, ((idx, vox), upd) in enumerate(sec.lr_steps()):
+        for k, v in zip(idx, vox):
+            o.set_tsdf_block(k, v)
+        o.integrate_esdf(upd, ep)
+        layer = o.esdf_layer()
+        assert min(sec.far_parent_voxels(layer)) > 10000, i
+        validate_esdf(layer, (sec.LR_MAX_DIST / sec.LR_VOXEL) ** 2)
+        if i == 1:  # removing a cluster clears voxels (the clear pass runs on blocks with "unknown" parent boxes)
+            assert o.esdf_stats()["cleared"] > 1000
