@@ -534,6 +534,9 @@ NVB_API void* nvb_mapper_stream(NvbMapper* m);
 NVB_API int32_t nvb_layer_num_blocks(NvbMapper* m, int32_t layer, int32_t* out_count);      /* numBlocks        */
 NVB_API int32_t nvb_layer_block_indices(NvbMapper* m, int32_t layer, int32_t* out_xyz_host,
                                         int32_t cap, int32_t* out_count);                    /* getAllBlockIndices */
+/* Storage of a layer's block slab: out = {capacity in blocks, high-water mark (slots handed out so far), free-stack size
+ * (deallocated slots below the high-water mark, reused before fresh ones), hash-table size}. */
+NVB_API int32_t nvb_layer_slab_stats(NvbMapper* m, int32_t layer, int64_t out[4]);
 /* getBlockAtIndex(...)->voxels copied to host: out_host receives n blocks of
  * block_bytes (4096 TSDF / 10240 ESDF); found[i] = 0 for unallocated indices
  * (their output bytes are zero). block_bytes: 4096 TSDF / 10240 ESDF / 2048 occupancy. */

@@ -39,7 +39,7 @@ EXPORTED_SYMBOLS = [
     "nvb_mapper_update_esdf", "nvb_mapper_update_esdf_async", "nvb_esdf_integrate_blocks",
     "nvb_mapper_synchronize", "nvb_mapper_last_frame_block_count", "nvb_mapper_last_frame_blocks",
     "nvb_mapper_stream", "nvb_mapper_join_streams", "nvb_blocks_union",
-    "nvb_layer_num_blocks", "nvb_layer_block_indices", "nvb_layer_get_blocks",
+    "nvb_layer_num_blocks", "nvb_layer_block_indices", "nvb_layer_slab_stats", "nvb_layer_get_blocks",
     "nvb_layer_set_blocks", "nvb_layer_block_device_ptr", "nvb_layer_block_bytes",
     "nvb_mapper_last_esdf_stats", "nvb_mapper_set_cache_last_viewpoint", "nvb_mapper_get_cache_last_viewpoint", "nvb_mapper_set_depth_preprocessing", "nvb_mapper_get_depth_preprocessing", "nvb_depth_dilate_invalid", "nvb_esdf_slice_aabb", "nvb_esdf_slice_distance_image_in_aabb", "nvb_mapper_set_esdf_reserved_sms", "nvb_mapper_get_esdf_reserved_sms", "nvb_default_mesh_params", "nvb_mapper_set_mesh_params", "nvb_mapper_get_mesh_params", "nvb_mapper_update_mesh", "nvb_mesh_integrate_blocks", "nvb_mesh_update_color", "nvb_mesh_block_sizes", "nvb_mesh_get_blocks", "nvb_mesh_arena_stats", "nvb_mapper_append_frame_blocks", "nvb_blocks_union_segments", "nvb_blocks_union_status", "nvb_mapper_esdf_time_split", "nvb_mapper_esdf_clear_blocks_read", "nvb_mapper_debug_phase_max", "nvb_mapper_enable_profiling", "nvb_mapper_stage_times",
     "nvb_mapper_kernel_launches",
@@ -220,6 +220,7 @@ def load():
     L.nvb_mapper_stream.restype = vp
     L.nvb_layer_num_blocks.argtypes = [vp, i32, ip]
     L.nvb_layer_block_indices.argtypes = [vp, i32, ip, i32, ip]
+    L.nvb_layer_slab_stats.argtypes = [vp, i32, C.POINTER(C.c_int64)]
     L.nvb_layer_get_blocks.argtypes = [vp, i32, ip, i32, vp, u8p]
     L.nvb_layer_set_blocks.argtypes = [vp, i32, ip, i32, vp]
     L.nvb_layer_block_device_ptr.argtypes = [vp, i32, ip, C.POINTER(vp)]

@@ -2561,6 +2561,19 @@ int32_t nvb_layer_num_blocks(NvbMapper* m, int32_t layer, int32_t* out_count) {
   return NVB_OK;
 }
 
+int32_t nvb_layer_slab_stats(NvbMapper* m, int32_t layer, int64_t out[4]) {
+  if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  DevLayer* L = layerOf(m, layer);
+  if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "unknown layer");
+  NVB_CUDA(cudaSetDevice(m->device));
+  NVB_CUDA(syncAll(m));
+  int count = 0, nfree = 0;
+  NVB_CUDA(cudaMemcpy(&count, L->count, sizeof(int), cudaMemcpyDeviceToHost));
+  NVB_CUDA(cudaMemcpy(&nfree, L->free_count, sizeof(int), cudaMemcpyDeviceToHost));
+  out[0] = L->capacity, out[1] = std::min(count, L->capacity), out[2] = nfree, out[3] = (int64_t)L->hash.mask + 1;
+  return NVB_OK;
+}
+
 int32_t nvb_layer_block_indices(NvbMapper* m, int32_t layer, int32_t* out_xyz_host, int32_t cap, int32_t* out_count) {
   int n = 0;
   int rc = nvb_layer_num_blocks(m, layer, &n);

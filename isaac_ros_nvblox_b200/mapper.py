@@ -93,6 +93,12 @@ class _Layer:
         check(self._m._L.nvb_layer_block_indices(self._m._h, self._id, _ip(out), n, C.byref(cnt)))
         return out[:n].copy()
 
+    def slab_stats(self):
+        """Storage of the layer: slab capacity, high-water mark and free-stack size in blocks, and the hash-table size."""
+        out = (C.c_int64 * 4)()
+        check(self._m._L.nvb_layer_slab_stats(self._m._h, self._id, out))
+        return {"capacity": out[0], "high_water": out[1], "free": out[2], "hash_size": out[3]}
+
     def get_blocks(self, indices):
         """(n,3) int32 -> ((n,8,8,8) voxel array, (n,) found mask)."""
         idx = np.ascontiguousarray(indices, dtype=np.int32).reshape(-1, 3)

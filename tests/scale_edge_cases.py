@@ -166,3 +166,139 @@ def far_parent_voxels(esdf_layer):
         low += int((has & np.any(off < -16, axis=-1)).sum())
         high += int((has & np.any(off > 15, axis=-1)).sum())
     return low, high
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Deallocation, slot reuse and slab growth (nvb_api.cu nvb_mapper_decay / ensureTsdfCapacity / growLayer, nvb_util.cu
+# removeBlocksKernel, nvb_esdf.cu esdfRemoveBlocksKernel, nvb_internal.cuh hashFindOrInsert):
+#   * REMOVE_GRID: the remove kernels launch at most 1184 CTAs, one dead block per CTA and round; more dead blocks than
+#     that take several rounds;
+#   * a frame that allocates more new blocks than the free stack holds empties the stack inside one allocation launch
+#     (atomicSub below zero, atomicAdd back) and continues with fresh slots;
+#   * a frame whose view AABB does not fit behind the slab's high-water mark doubles the slab (growLayer copies the free
+#     stack and rehashes up to the high-water mark), here while the stack is not empty.
+# The churn sequence: 2 cm voxels, three frames at a 4 m range, a decay that removes everything outside a sphere, then one
+# frame at a 7 m range (its view AABB is ~5x larger than the 4 m frames').
+# ---------------------------------------------------------------------------------------------------------------------
+REMOVE_GRID = 1184
+CHURN = dict(voxel=0.02, width=320, height=240, near_m=4.0, far_m=7.0, capacity=4096, radius_m=2.5, frames=3)
+
+
+def churn_frames():
+    """-> (frames [(depth, T)] * 4, product camera, oracle camera): three frames to build the map, one after the decay."""
+    cs, cam, ocam = cameras(CHURN["width"], CHURN["height"])
+    return syn.make_sequence(syn.sphere_in_box(), cs, syn.circle_trajectory(40)[:CHURN["frames"] + 1]), cam, ocam
+
+
+def churn_exclusion_center(frames):
+    """2.5 m in front of the first camera: the decay keeps the blocks within CHURN['radius_m'] of it."""
+    T = frames[0][1]
+    return tuple(float(c) for c in T[:3, 3] + np.float32(2.5) * T[:3, 2])
+
+
+def churn_cells(T, max_dist):
+    cs, _, _ = cameras(CHURN["width"], CHURN["height"])
+    return view_grid(cs.fu, cs.fv, cs.cu, cs.cv, cs.width, cs.height, T, 8 * CHURN["voxel"], max_dist)[2]
+
+
+def grown_capacity(capacity, high_water, cells):
+    """ensureTsdfCapacity: the slab doubles until the frame's view cells fit behind the high-water mark."""
+    while capacity < high_water + cells:
+        capacity *= 2
+    return capacity
+
+
+# Occupancy decay parameters that take every observed voxel to 0.5 in one step (free +4.6, occupied -4.6 log odds).
+OCC_WIPE = dict(free_region_decay_probability=0.99, occupied_region_decay_probability=0.01)
+TSDF_WIPE = dict(decay_factor=1e-6, decayed_weight_threshold=1e-3)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Mesh arena (nvb_api.cu repackMeshArena): at least 2^20 entries, and after a repack at least twice the live data plus the
+# update. MESH_ARENA_TARGET: a 2 cm full-layer update grows it past 2^22 entries.
+# Freespace (nvb_api.cu updateFreespaceImpl): freespaceUpdateKernel runs on 4 CTAs per SM; H100 SXM has 132 SMs.
+# ---------------------------------------------------------------------------------------------------------------------
+MESH_ARENA_MIN = 1 << 20
+MESH_ARENA_TARGET = 1 << 22
+FREESPACE_GRID_H100 = 4 * 132
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The long-range scene restated as an occupancy layer: a voxel is occupied (log odds +6.9) where its TSDF distance is at or
+# below zero, free (-6.9) elsewhere; the occupancy ESDF marks the same sites as the TSDF one.
+# ---------------------------------------------------------------------------------------------------------------------
+def occupancy_from_tsdf(vox):
+    """(n, 8, 8, 8) TSDF voxels -> (n, 8, 8, 8) float32 log odds."""
+    return np.where(vox["distance"] <= 0.0, np.float32(6.9), np.float32(-6.9)).astype(np.float32)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 2-D slices. SLICER_AABB: an EsdfSlicer image box of SLICER_PIXELS at 2 cm voxels (one thread per pixel, a 2-D grid of
+# 16 x 16 tiles). The far-origin slice heights follow the z offsets of FAR_OFFSETS (+345.6 m and -300.2 m).
+# ---------------------------------------------------------------------------------------------------------------------
+SLICER_AABB = (-30.0, -25.0, 0.0, 30.0, 25.0, 0.0)  # min x, min y, min z, max x, max y, max z (m)
+SLICE_Z = dict(slice_min_height_m=0.25, slice_max_height_m=1.45, slice_height_m=0.9)
+
+
+def slicer_pixels(voxel=0.02):
+    """Image size of EsdfSlicer::sliceLayerToDistanceImage over SLICER_AABB: ceil(extent / voxel) per axis."""
+    x0, y0, _, x1, y1, _ = SLICER_AABB
+    return int(np.ceil((x1 - x0) / voxel)) * int(np.ceil((y1 - y0) / voxel))
+
+
+def gyroid_layer(lo=(-2.4, -2.4, 0.0), hi=(2.39, 2.39, 1.91), voxel=0.02, period=0.24, trunc=0.08):
+    """A gyroid-like periodic surface (sin x cos y + sin y cos z + sin z cos x = 0, scaled to a distance) filling a box:
+    every block of the box crosses the surface, so a full-layer mesh update emits ~250 vertices per block.
+    -> (block indices (n, 3), TSDF voxels (n, 8, 8, 8))."""
+    from helpers import tsdf_layer_from_distance
+    k = 2.0 * np.pi / period
+
+    def fn(P):
+        x, y, z = (k * P[..., i].astype(np.float64) for i in range(3))
+        return (np.sin(x) * np.cos(y) + np.sin(y) * np.cos(z) + np.sin(z) * np.cos(x)) / k
+
+    return tsdf_layer_from_distance(fn, lo, hi, voxel, trunc)
+
+
+def smooth_image(rows, cols):
+    """RGB ramps without texture: a colour sample moved by a fraction of a pixel changes by at most a few levels."""
+    y, x = np.mgrid[0:rows, 0:cols]
+    return np.stack([x * 255 // (cols - 1), y * 255 // (rows - 1), (x + y) * 255 // (rows + cols - 2)], -1).astype(np.uint8)
+
+
+def far_colour_differences(far_layer, near_layer, offset, voxel):
+    """Largest colour-channel difference of each voxel coloured (weight > 0) in both maps, matched by the voxel-index shift
+    offset / voxel, and the fraction of the origin map's coloured voxels that were matched."""
+    shift = np.round(np.asarray(offset, np.float64) / voxel).astype(np.int64)
+
+    def coloured(layer):
+        out = {}
+        for k, b in layer.items():
+            for v in np.argwhere(b["weight"] > 0):
+                out[tuple(np.asarray(k, np.int64) * 8 + v)] = b["color"][tuple(v)].astype(np.int64)
+        return out
+
+    f, n = coloured(far_layer), coloured(near_layer)
+    diff = [int(np.max(np.abs(f[tuple(np.asarray(k) + shift)] - c))) for k, c in n.items() if tuple(np.asarray(k) + shift) in f]
+    return np.asarray(diff), len(diff) / max(len(n), 1)
+
+
+def far_vertex_distances(far_mesh, near_mesh, offset):
+    """Distance of every origin-map mesh vertex to the nearest far-map vertex shifted back by offset (float64)."""
+    from scipy.spatial import cKDTree
+    fv = np.concatenate([b["vertices"] for b in far_mesh.values()]).astype(np.float64) - np.asarray(offset, np.float64)
+    nv = np.concatenate([b["vertices"] for b in near_mesh.values()]).astype(np.float64)
+    return cKDTree(fv).query(nv)[0]
+
+
+def far_colour_bounds(offset):
+    """Bounds on far_colour_differences, calibrated on the oracle with smooth_image: matched fraction, median and 99th
+    percentile (colour levels; the 99th percentile scales with the float32 spacing at the offset)."""
+    spacing = float(np.spacing(np.float32(np.max(np.abs(offset)))))
+    return 0.97, 0, 4096.0 * spacing
+
+
+def far_vertex_bounds(offset, voxel):
+    """Bounds on far_vertex_distances: median within one float32 spacing at the offset, 99th percentile within half a
+    voxel (a voxel distance that rounds differently moves a surface crossing along its edge)."""
+    return float(np.spacing(np.float32(np.max(np.abs(offset))))), 0.5 * voxel

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 import scale_edge_cases as sec
-from helpers import cameras, validate_esdf
+from helpers import cameras, textured_image, validate_esdf
 from isaac_ros_nvblox_b200 import synthetic as syn
 
 
@@ -126,3 +126,92 @@ def test_long_range_scene_has_parents_beyond_15_blocks_on_the_oracle():
         validate_esdf(layer, (sec.LR_MAX_DIST / sec.LR_VOXEL) ** 2)
         if i == 1:  # removing a cluster clears voxels (the clear pass runs on blocks with "unknown" parent boxes)
             assert o.esdf_stats()["cleared"] > 1000
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Preconditions of tests/test_gpu_scale_edges_f.py
+# ---------------------------------------------------------------------------------------------------------------------
+def churn_on_the_oracle(occupancy=False):
+    """The churn sequence (scale_edge_cases.CHURN) on the oracle, with the TSDF slab's capacity restated from
+    ensureTsdfCapacity. -> dict of block counts and capacities."""
+    from oracle import oracle as orc
+    C = sec.CHURN
+    frames, _, ocam = sec.churn_frames()
+    o = orc.OracleMap(C["voxel"])
+    blocks = o.occupancy_block_indices if occupancy else o.tsdf_block_indices
+    cap, hw = C["capacity"], 0
+    for i, (d, T) in enumerate(frames[:C["frames"]]):
+        cap = sec.grown_capacity(cap, hw, sec.churn_cells(T, C["near_m"]))
+        p = orc.default_tsdf_params(max_integration_distance_m=C["near_m"])
+        o.integrate_occupancy(d, T, ocam, p) if occupancy else o.integrate_depth(d, T, ocam, p)
+        if not occupancy:
+            o.integrate_color(textured_image(C["height"], C["width"], seed=i), T, ocam)
+        hw = len(blocks())
+    colour_built = len(o.color_block_indices())
+    center = sec.churn_exclusion_center(frames)
+    if occupancy:
+        removed = o.decay_occupancy(orc.default_occupancy_decay_params(**sec.OCC_WIPE), exclusion_center=center,
+                                    exclusion_radius_m=C["radius_m"])
+    else:
+        removed = o.decay_tsdf(orc.default_tsdf_decay_params(**sec.TSDF_WIPE), exclusion_center=center,
+                               exclusion_radius_m=C["radius_m"])
+    left = len(blocks())
+    colour_removed = colour_built - len(o.color_block_indices())
+    d, T = frames[C["frames"]]
+    far_cells = sec.churn_cells(T, C["far_m"])
+    p = orc.default_tsdf_params(max_integration_distance_m=C["far_m"])
+    o.integrate_occupancy(d, T, ocam, p) if occupancy else o.integrate_depth(d, T, ocam, p)
+    return dict(built=hw, capacity=cap, removed=len(removed), colour_removed=colour_removed, left=left, new=len(blocks()) - left, far_cells=far_cells,
+                grown=sec.grown_capacity(cap, hw, far_cells))
+
+
+@pytest.mark.parametrize("occupancy", [False, True])
+def test_churn_crosses_the_remove_grid_the_free_stack_and_the_capacity(occupancy):
+    r = churn_on_the_oracle(occupancy)
+    assert r["removed"] >= sec.MARGIN * sec.REMOVE_GRID, r  # several rounds of the remove kernels
+    assert occupancy or r["colour_removed"] >= sec.MARGIN * sec.REMOVE_GRID, r
+    assert r["left"] >= 0.2 * r["built"], r                  # a partial removal
+    assert r["new"] >= sec.MARGIN * r["removed"], r          # the free stack runs dry in the frame after the decay
+    assert r["built"] + r["far_cells"] >= sec.MARGIN * r["capacity"] and r["grown"] > r["capacity"], r  # ... which grows it
+    assert 20000 <= r["built"] + r["new"] and r["grown"] <= 1 << 22, r
+
+
+def test_gyroid_mesh_needs_an_arena_past_2_22_entries():
+    from oracle import oracle as orc
+    idx, vox = sec.gyroid_layer()
+    o = orc.OracleMap(0.02)
+    for k, v in zip(idx, vox):
+        o.set_tsdf_block(k, v)
+    o.integrate_mesh()
+    verts = sum(len(b["vertices"]) for b in o.mesh_layer().values())
+    # a repack makes room for twice the live data plus the update: one full-layer update on top of half the layer
+    assert 2 * (verts // 2 + verts) >= sec.MARGIN * sec.MESH_ARENA_TARGET, verts
+    assert len(idx) >= 10000
+
+
+@pytest.mark.parametrize("offset", sec.FAR_OFFSETS)
+def test_far_origin_colour_and_mesh_match_the_origin_on_the_oracle(offset):
+    from oracle import oracle as orc
+    frames, _, ocam = far_frames()
+    img = sec.smooth_image(FAR_SEQ["height"], FAR_SEQ["width"])
+    near, far = orc.OracleMap(FAR_SEQ["voxel"]), orc.OracleMap(FAR_SEQ["voxel"])
+    for d, T in frames:
+        near.integrate_depth(d, T, ocam), near.integrate_color(img, T, ocam)
+        far.integrate_depth(d, sec.shifted(T, offset), ocam), far.integrate_color(img, sec.shifted(T, offset), ocam)
+    diff, matched = sec.far_colour_differences(far.color_layer(), near.color_layer(), offset, FAR_SEQ["voxel"])
+    frac, med, p99 = sec.far_colour_bounds(offset)
+    assert matched >= frac and np.median(diff) <= med and np.percentile(diff, 99) <= p99, (matched, np.percentile(diff, 99))
+    near.integrate_mesh(), far.integrate_mesh()
+    dist = sec.far_vertex_distances(far.mesh_layer(), near.mesh_layer(), offset)
+    med, p99 = sec.far_vertex_bounds(offset, FAR_SEQ["voxel"])
+    assert np.median(dist) <= med and np.percentile(dist, 99) <= p99, (np.median(dist), np.percentile(dist, 99))
+
+
+def test_slicer_image_and_slice_heights_cross_their_thresholds():
+    assert sec.slicer_pixels() >= 5_000_000
+    assert min(o[2] for o in sec.FAR_OFFSETS) <= -300.0 and max(o[2] for o in sec.FAR_OFFSETS) >= 300.0
+    # below the origin floor(h / block_size) and a truncating cast differ, so a slice split that truncated moves the band
+    for o in sec.FAR_OFFSETS:
+        for h in sec.SLICE_Z.values():
+            if o[2] < 0:
+                assert np.floor((h + o[2]) / 0.4) != np.trunc((h + o[2]) / 0.4)
