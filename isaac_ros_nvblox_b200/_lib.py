@@ -137,9 +137,14 @@ class NvbError(RuntimeError):
 _lib = None
 
 
-def load():
-    """Load libnvblox_b200.so (build it first with build_ext.build())."""
-    global _lib
+def load(path=None):
+    """Load libnvblox_b200.so (build it first with build_ext.build()). `path` overrides LIB_PATH (a variant build, e.g. the
+    profiling library of tools/wavex_profile.py); it has to be given before the first load of the process."""
+    global _lib, LIB_PATH
+    if path is not None and _lib is None:
+        LIB_PATH = path
+    elif path is not None and os.path.abspath(path) != os.path.abspath(LIB_PATH):
+        raise RuntimeError("%s is already loaded; cannot switch to %s" % (LIB_PATH, path))
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):

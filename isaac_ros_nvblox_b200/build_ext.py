@@ -30,9 +30,14 @@ def needs_build():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False):
-    if not force and not needs_build():
+def build(force=False, verbose=False, out=None, defines=()):
+    """Build the library into OUT (or `out`). `out` builds unconditionally: needs_build() compares file times only, so a
+    variant built with other `defines` (e.g. NVB_WAVEX_PROF=1) must go to its own path, never over OUT."""
+    if out is None and defines:
+        raise ValueError("a build with extra defines needs its own output path")
+    if out is None and not force and not needs_build():
         return OUT
+    target = out or OUT
     cmd = [
         nvcc_path(), "-std=c++17", "-O3", "-lineinfo",
         "-gencode", "arch=compute_90a,code=sm_90a",
@@ -41,14 +46,14 @@ def build(force=False, verbose=False):
         "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden,-O2",
         "-I", os.path.join(ROOT, "include"), "-I", CSRC,
         "-shared", "-cudart", "static",
-    ] + os.environ.get("NVB_EXTRA_NVCC_FLAGS", "").split() + [
-        "-o", OUT,
+    ] + os.environ.get("NVB_EXTRA_NVCC_FLAGS", "").split() + ["-D" + d for d in defines] + [
+        "-o", target,
     ] + [os.path.join(CSRC, s) for s in SOURCES]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
         print(" ".join(cmd))
     subprocess.check_call(cmd)
-    return OUT
+    return target
 
 
 if __name__ == "__main__":

@@ -20,7 +20,8 @@
 //     blocks whose state after pass p matters are D6 = {B}, D5 = D6 + {B+z}, D4 = D5 + {B-z}, D3 = D4 + (D4 + y),
 //     D2 = D3 + (D3 - y), D1 = D2 + (D2 + x) (backwards through -z,+z,-y,+y,-x,+x). With one to three member neighbours --
 //     the usual case -- one or two of the six passes are live and a few per cent of the 1 200 pair slots; halo voxels of
-//     blocks that are in no live pair are not fetched (they would miss L2: nobody wrote them lately).
+//     blocks that are in no live pair are not fetched (they would miss L2: nobody wrote them lately). The halo travels by
+//     cp.async straight into the region planes, so no registers are held across its round trip.
 //   * Region layout in shared memory: a plane of 16-byte cells {squared distance, parent} and a plane of flag words, voxel
 //     index rx*110 + ry*11 + rz. Every line of the three sweeps and every pair of the replay is ONE conflict-free 128-bit
 //     access per voxel (the 20-byte array-of-structures layout of the layer costs five 32-bit accesses with up to 8-way bank
@@ -55,12 +56,19 @@ namespace {
 #define NVB_WAVEX_TAIL 1
 #endif
 #ifndef NVB_WAVEX_PROF
-#define NVB_WAVEX_PROF 0  // 1: per-stage cycle counters of CTA 0 / group 0 (nvb_mapper_debug_phase_max); costs 16 registers
+#define NVB_WAVEX_PROF 0  // 1: per-phase times and per-stage cycle counters of CTA 0 / group 0 (nvb_mapper_debug_phase_max,
+                          // tools/wavex_profile.py); the timers spill at 96 registers, so quote its shares, not its times
+#endif
+#ifndef NVB_WAVEX_SPEC_HALO
+#define NVB_WAVEX_SPEC_HALO 0  // 1: the face halo of every allocated neighbour travels with the own block and the stamps (slower, DESIGN §9)
 #endif
 #if NVB_WAVEX_PROF
 #define X_PROF_BEGIN() long long tq = clock64();
-#define X_PROF(i) prof[i] += clock64() - tq, tq = clock64();
-#define X_PROF_COUNT(i) prof[i]++;
+#define X_PROF(i) \
+  if (lane64 == 0) xs.prof[group][i] += clock64() - tq; \
+  tq = clock64();
+#define X_PROF_COUNT(i) \
+  if (lane64 == 0) xs.prof[group][i]++;
 #else
 #define X_PROF_BEGIN()
 #define X_PROF(i)
@@ -95,7 +103,17 @@ struct XShared {
   int next;                // next unclaimed entry of this CTA's share of the ring (groups pull work: a changed candidate costs
                            // twice an unchanged one, a static deal left groups with two changed ones on the critical path)
   int cur[kXG];
+  int seeds[kXG];  // length of the seed list being processed (per group: written and read across the group's barriers)
   int bcast[4];
+  // Per-launch state kept here rather than in registers: processCandidate / processSeed are real calls, and whatever the
+  // kernel keeps live across them is saved to the stack at every call.
+  unsigned int generation;  // grid-barrier generation (thread 0)
+  int n_bar;                // grid barriers passed in this launch
+  int ring;                 // the ring being processed (written by thread 0 between two CTA barriers)
+  int swept, faces, rings, n_tail;  // statistics (thread 0)
+#if NVB_WAVEX_PROF
+  long long prof[kXG][8];   // per group, cycles: record, stamps + own block (+ speculative faces), halo, replay, sweep, stores; candidates, changed
+#endif
 };
 
 // What the per-candidate functions need of the kernel parameter, in shared memory: they are real calls (one copy of the code for
@@ -116,6 +134,13 @@ struct XCtx {
   float max_sq;
   __device__ __forceinline__ int* segment(int p, int cta) const { return recs[p] + (size_t)cta * seg * kRecInts; }
 };
+
+// The kernel's shared state lives at namespace scope: the per-candidate functions address it directly (32-bit shared
+// addresses folded into the instructions) instead of receiving generic pointers that would occupy registers for the whole call.
+__shared__ XTables x_tab;
+__shared__ XShared x_xs;
+__shared__ XCtx x_ctx;
+extern __shared__ __align__(16) unsigned int x_smem[];  // kXG regions of kXRegionWords
 
 __device__ __forceinline__ int rvox(int rx, int ry, int rz) { return rx * kRX + ry * kRY + rz; }
 __device__ __forceinline__ int faceEntry(int f) {  // +x,-x,+y,-y,+z,-z -> index into a 3x3x3 row
@@ -321,46 +346,45 @@ __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer
   }
 }
 
-// ---- halo voxels of the neighbours in `needed`, from the exchange slab of this ring. The eight batches of the table (six
-// faces, edges + corners) are walked four live ones at a time: a candidate with up to four live batches -- nearly all of them
-// -- pays one round trip.
-__device__ __forceinline__ void haloGather(const XTables& tab, unsigned int* R, const int* row, unsigned int needed,
-                                           const unsigned char* X, int lane64) {
-  uint4* A = reinterpret_cast<uint4*>(R);
-  // faces in batch order: +x,-x,+y,-y,+z,-z = blocks 22, 4, 16, 10, 14, 12; everything else is an edge or corner block
-  unsigned int bl = ((needed >> 22) & 1u) | (((needed >> 4) & 1u) << 1) | (((needed >> 16) & 1u) << 2) | (((needed >> 10) & 1u) << 3) |
-                    (((needed >> 14) & 1u) << 4) | (((needed >> 12) & 1u) << 5);
-  if (needed & ~((1u << 22) | (1u << 4) | (1u << 16) | (1u << 10) | (1u << 14) | (1u << 12))) bl |= 0xC0u;
-  while (bl) {  // group-uniform
-    unsigned int hw[4][5];
-    unsigned int ent[4];
+// ---- halo voxels, as 4-byte cp.async copies straight into the two region planes: no registers are held across the wait (the
+// register version held up to 20 words per lane and spilled at 96 registers). By default only the batches of the members in
+// a live pair are fetched, after the stamps. With NVB_WAVEX_SPEC_HALO the face halo of every ALLOCATED face neighbour is issued
+// before the member stamps are known, with the own block and the stamps (one round trip after the record instead of two);
+// on the H100 the extra, mostly cold face fetches cost more than the round trip they save (DESIGN §9). Speculation is safe:
+// the replay reads a halo voxel only if its block is a live source (live[p] is a subset of the members) or a member destination (liveMasks), and the sweeps and the stores
+// touch the inner 8x8x8 only, so the voxels copied from a non-member's stale exchange-slab entry land in shared memory and are
+// never read. (.ca: 4-byte copies have no .cg form. The L1 lines they leave behind cannot go stale unnoticed: every grid
+// barrier ends with a __threadfence, which invalidates the SM's L1, and within the single-CTA tail the writer is this SM.)
+__device__ __forceinline__ void cpAsync4(unsigned int* smem_dst, const unsigned int* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned int)__cvta_generic_to_shared(smem_dst)), "l"(gsrc)
+               : "memory");
+}
+// Halo batches `batches` (bit k: batch k of the table), the voxels whose block d has bit d in `blocks` and is allocated.
+__device__ __forceinline__ void haloAsync(const XTables& tab, unsigned int* R, const int* row, const unsigned char* X, int lane64,
+                                          unsigned int batches, unsigned int blocks) {
+#pragma unroll 1
+  while (batches) {  // group-uniform
+    const int k = __ffs(batches) - 1;
+    batches &= batches - 1;
+    const unsigned int e = tab.halo[k][lane64];
+    const int d = (e >> 20) & 31u;
+    const int slot = ((e >> 25) & 1u) && ((blocks >> d) & 1u) ? row[d] : -1;
+    if (slot >= 0) {
+      const unsigned int* src = reinterpret_cast<const unsigned int*>(X + (size_t)slot * kEsdfBlockBytes) + ((e >> 11) & 511u) * kEsdfVoxelWords;
+      const int v = e & 2047u;
 #pragma unroll
-    for (int j = 0; j < 4; j++) {
-      unsigned int e = 0;
-      if (bl) {
-        const int k = __ffs(bl) - 1;
-        bl &= bl - 1;
-        e = tab.halo[k][lane64];
-        if (!((e >> 25) & 1u) || !((needed >> ((e >> 20) & 31u)) & 1u)) e = 0;
-      }
-      ent[j] = e;
-      if (e) {
-        const int slot = row[(e >> 20) & 31u];
-        const unsigned int* src =
-            reinterpret_cast<const unsigned int*>(X + (size_t)slot * kEsdfBlockBytes) + ((e >> 11) & 511u) * kEsdfVoxelWords;
-#pragma unroll
-        for (int w = 0; w < 5; w++) hw[j][w] = __ldcg(src + w);
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      if (ent[j]) {
-        const int v = ent[j] & 2047u;
-        A[v] = make_uint4(hw[j][0], hw[j][1], hw[j][2], hw[j][3]);
-        R[kFlagBase + v] = hw[j][4];
-      }
+      for (int w = 0; w < 4; w++) cpAsync4(R + 4 * v + w, src + w);
+      cpAsync4(R + kFlagBase + v, src + 4);
     }
   }
+}
+// faces in batch order: +x,-x,+y,-y,+z,-z = blocks 22, 4, 16, 10, 14, 12; everything else is an edge or corner block (batches 6, 7)
+constexpr unsigned int kFaceBlocks = (1u << 22) | (1u << 4) | (1u << 16) | (1u << 10) | (1u << 14) | (1u << 12);
+__device__ __forceinline__ unsigned int haloBatches(unsigned int needed) {
+  unsigned int bl = ((needed >> 22) & 1u) | (((needed >> 4) & 1u) << 1) | (((needed >> 16) & 1u) << 2) | (((needed >> 10) & 1u) << 3) |
+                    (((needed >> 14) & 1u) << 4) | (((needed >> 12) & 1u) << 5);
+  if (needed & ~kFaceBlocks) bl |= 0xC0u;
+  return bl;
 }
 
 // ---- the six passes of updateLocalNeighborBands (:1323-1386) restricted to the pairs that matter, updateSingleNeighbor
@@ -548,31 +572,41 @@ __device__ __forceinline__ void registerFinish(const XCtx& c, XShared& xs, const
   if (lane64 < 6 && s.pos >= 0) __stcg(segment + (size_t)s.pos * kRecInts, xs.nb[group][lane64]);
 }
 
-struct XState {
-  int ring, ci;
-};
-// One candidate of ring `st.ring`: gather, replay, and if it changed: sweep, publish, register its neighbours for ring+1.
-__device__ __noinline__ void processCandidate(const XCtx& c, const XTables& tab, XShared& xs, unsigned int* R, int ring,
-                                              int seg_cta, int seg_idx, int cta, int group, int lane64, long long* prof) {
+// One candidate of ring `ring`: gather, replay, and if it changed: sweep, publish, register its neighbours for ring+1.
+// The entry is xs.seg[group] (registering CTA, index in its segment); the group is the caller's (threadIdx.x / 64).
+__device__ __noinline__ void processCandidate(int ring) {
+  const XCtx& c = x_ctx;
+  const XTables& tab = x_tab;
+  XShared& xs = x_xs;
+  const int cta = blockIdx.x, group = threadIdx.x >> 6, lane64 = threadIdx.x & 63;
+  unsigned int* R = x_smem + group * kXRegionWords;
   const int ci = ring & 1, ni = ci ^ 1;
   X_PROF_BEGIN()
-  if (lane64 < 28) xs.rec[group][lane64] = __ldcg(c.segment(ci, seg_cta) + (size_t)seg_idx * kRecInts + lane64);
+  if (lane64 < 28) xs.rec[group][lane64] = __ldcg(c.segment(ci, xs.seg[group][0]) + (size_t)xs.seg[group][1] * kRecInts + lane64);
   groupSync(group);
   X_PROF(0)
   const int slot = xs.rec[group][0];
   const int* row = &xs.rec[group][1];
-  // membership of the 27 blocks in this ring (sources of the passes); the loads travel with the loads of the own block
+  // membership of the 27 blocks in this ring (sources of the passes); the loads travel with the loads of the own block and
+  // (NVB_WAVEX_SPEC_HALO) the face halo
   int sv = ring - 1;
   if (lane64 < 27 && row[lane64] >= 0) sv = __ldcg(c.stamp[ci] + row[lane64]);
   OwnRegs own = ownLoad(c.blocks + (size_t)slot * kEsdfBlockBytes, lane64);
+  if (NVB_WAVEX_SPEC_HALO) haloAsync(tab, R, row, c.X[ci], lane64, 0x3Fu, 0x7FFFFFFu);
   const unsigned int m = __ballot_sync(0xffffffffu, lane64 < 27 && sv == ring);
   if (lane64 == 0) xs.mask[group] = m, xs.changed[group] = 0;
   ownToShared(R, own, lane64);
+  if (NVB_WAVEX_SPEC_HALO) cpAsyncWaitAll();
   groupSync(group);
   const LiveMasks L = liveMasks(xs.mask[group], xs.live[group], lane64 == 0);
   X_PROF(1)
-  haloGather(tab, R, row, L.needed, c.X[ci], lane64);
-  groupSync(group);
+  // the halo of the members that take part in a live pair (with NVB_WAVEX_SPEC_HALO: only their edge and corner batches)
+  const unsigned int rest = NVB_WAVEX_SPEC_HALO ? (L.needed & ~kFaceBlocks) : L.needed;
+  if (rest) {  // group-uniform
+    haloAsync(tab, R, row, c.X[ci], lane64, haloBatches(rest), rest);
+    cpAsyncWaitAll();
+  }
+  groupSync(group);  // (also publishes xs.live[group], written by lane 0 in liveMasks and read by every lane in replayX)
   X_PROF(2)
   const bool ch = replayX(tab, R, L, lane64, group, c.max_sq);
   if (ch) xs.changed[group] = 1;
@@ -600,10 +634,13 @@ __device__ __noinline__ void processCandidate(const XCtx& c, const XTables& tab,
   X_PROF(5)
 }
 
-// A member of the initial list of a computeEsdf call (ring `st.ring`): sweep in place, publish, register its neighbours as
+// A member of the initial list of a computeEsdf call (ring `ring`): sweep in place, publish, register its neighbours as
 // the candidates of this ring.
-__device__ __noinline__ void processSeed(const XCtx& c, XShared& xs, unsigned int* R, int ring, int slot, int cta, int group,
-                                         int lane64) {
+__device__ __noinline__ void processSeed(int ring, int slot) {
+  const XCtx& c = x_ctx;
+  XShared& xs = x_xs;
+  const int cta = blockIdx.x, group = threadIdx.x >> 6, lane64 = threadIdx.x & 63;
+  unsigned int* R = x_smem + group * kXRegionWords;
   const int ci = ring & 1;
   unsigned char* blk = c.blocks + (size_t)slot * kEsdfBlockBytes;
   OwnRegs own = ownLoad(blk, lane64);
@@ -626,18 +663,44 @@ __device__ __noinline__ void processSeed(const XCtx& c, XShared& xs, unsigned in
   groupSync(group);
 }
 
+#ifndef NVB_WAVEX_BARRIER_RA
+#define NVB_WAVEX_BARRIER_RA 1  // 0: gridBarrier (two __threadfence = fence.sc around a relaxed atomic and a volatile poll)
+#endif
+// Grid barrier with a release arrival and acquire polling: the same ordering as gridBarrier's two __threadfences (the CTA's
+// writes, gathered by the __syncthreads, are released by thread 0's arrival; its acquire load of the final count makes every
+// CTA's writes visible, and invalidates the SM's L1), without the heavier sequentially-consistent fences.
+__device__ __forceinline__ void gridBarrierRA(unsigned int* bar, unsigned int& generation, unsigned int nctas) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    generation++;
+    const unsigned int target = generation * nctas;
+    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(bar) : "memory");
+    unsigned int v;
+    do {
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory");
+    } while (v < target);
+  }
+  __syncthreads();
+}
+
 // Grid barrier + all-gather of the per-CTA counts {registrations, changed blocks}; leaves the exclusive scan of the
 // registrations in xs.pre and returns the totals: counts stored to per-CTA slots (two arrays by barrier parity), fence, atomic
 // arrival counter polled by thread 0, fence, then one read of the per-CTA slots. (The alternative -- one flag per CTA, every
 // CTA polling every other CTA's flag -- needs no read-modify-write on a shared word but grows with the square of the grid.)
 __device__ __forceinline__ void counterBarrierScan(XShared& xs, unsigned int* bar, unsigned int& generation, int2* counts, int nctas,
-                                                   int cta, int tid, int seg, int* K, int* M) {
+                                                   int cta, int tid, int seg, int ring_inc, int* K, int* M) {
+  // Barrier number xs.n_bar selects the parity of the count slots. Every thread reads it here, before the CTA barrier below;
+  // thread 0 advances it (and the ring) just before the last CTA barrier of this function, when nobody reads it any more.
+  counts += (xs.n_bar & 1) * kMaxCtas;
   __syncthreads();
   if (tid == 0) {
     __stcg(counts + cta, make_int2(min(xs.ncand, seg), xs.nchanged));  // (registrations past the segment were dropped)
     xs.ncand = 0, xs.nchanged = 0;
   }
-  gridBarrier(bar, generation, nctas);
+  if (NVB_WAVEX_BARRIER_RA)
+    gridBarrierRA(bar, generation, nctas);
+  else
+    gridBarrier(bar, generation, nctas);
   int2 v = make_int2(0, 0);
   if (tid < nctas) v = __ldcg(counts + tid);
   const int lane = tid & 31, warp = tid >> 5;
@@ -659,24 +722,24 @@ __device__ __forceinline__ void counterBarrierScan(XShared& xs, unsigned int* ba
     if (w * 32 < nctas) mtot += xs.warp_tot[1][w];
   }
   if (tid < nctas) xs.pre[tid + 1] = base + inc;
-  if (tid == 0) xs.pre[0] = 0, xs.next = 0;
+  if (tid == 0) xs.pre[0] = 0, xs.next = 0, xs.ring += ring_inc, xs.n_bar++;
   __syncthreads();
   *K = xs.pre[nctas];
   *M = mtot;
 }
 
 __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
-  extern __shared__ __align__(16) unsigned int smem[];
-  __shared__ XTables tab;
-  __shared__ XShared xs;
-  __shared__ XCtx xc;
+  XShared& xs = x_xs;
   const int cta = blockIdx.x, nctas = gridDim.x;
   const int tid = threadIdx.x, group = tid >> 6, lane64 = tid & 63;
   // Empty block list: integrateBlocksTemplate returns before touching anything (:226-228).
   if (*(volatile int*)c.work_count == 0) return;
-  initTables(tab, tid);
+  initTables(x_tab, tid);
   if (tid == 0) {
     xs.ncand = 0, xs.nchanged = 0, xs.next = 0;
+    xs.ring = *(volatile int*)c.ring_id;
+    xs.generation = 0, xs.n_bar = 0, xs.swept = 0, xs.faces = 0, xs.rings = 0, xs.n_tail = 0;
+    XCtx& xc = x_ctx;
     xc.blocks = c.esdf.blocks, xc.block_index = c.esdf.block_index, xc.hash = c.esdf.hash;
     xc.nbr = c.nbr, xc.nbr27 = c.nbr27, xc.cand_stamp = c.cand_stamp, xc.psum = c.psum;
     xc.stamp[0] = c.stamp_a, xc.stamp[1] = c.stamp_b;
@@ -684,65 +747,52 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
     xc.recs[0] = c.xrec, xc.recs[1] = c.xrec + (size_t)nctas * c.xseg * kRecInts;
     xc.seg = c.xseg, xc.error = c.error, xc.max_sq = c.max_sq;
   }
+#if NVB_WAVEX_PROF
+  if (lane64 < 8) xs.prof[group][lane64] = 0;
+#endif
   __syncthreads();
-  XState st;
-  st.ring = *(volatile int*)c.ring_id;
-  int swept = 0, faces = 0, rings = 0, n_bar = 0, n_tail = 0;
 #if NVB_WAVEX_PROF
   long long t_bar = 0, t_work = 0, t0 = globalTimerNs(), t1;
-#endif
-  unsigned int* R = smem + group * kXRegionWords;
-#if NVB_WAVEX_PROF
-  long long prof_store[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  long long* prof = prof_store;
-#else
-  long long* prof = nullptr;
-#endif
-  // prof: this group, cycles: record fetch, stamps + own block, halo, replay, sweep, stores + records; candidates, changed
-#if NVB_WAVEX_PROF
   int dbgK = 0, dbgM = 0;
 #define X_DBG(k, m) dbgK = (k), dbgM = (m);
-#else
-#define X_DBG(k, m)
-#endif
-#if NVB_WAVEX_PROF
-#define X_TIME_WORK()                                                                                               \
-  t1 = globalTimerNs(), t_work += t1 - t0;                                                                          \
-  if (tid == 0 && n_bar < 1000) atomicMax((unsigned long long*)c.phase_max + n_bar, (unsigned long long)(t1 - t0)); \
-  if (cta == 0 && tid == 0 && n_bar < 1000) c.phase_max[1000 + n_bar] = dbgK, c.phase_max[2000 + n_bar] = dbgM, c.phase_max[3000 + n_bar] = t1 - t0; \
+#define X_TIME_WORK()                                                                                                      \
+  t1 = globalTimerNs(), t_work += t1 - t0;                                                                                 \
+  if (tid == 0 && xs.n_bar < 1000) atomicMax((unsigned long long*)c.phase_max + xs.n_bar, (unsigned long long)(t1 - t0)); \
+  if (cta == 0 && tid == 0 && xs.n_bar < 1000)                                                                             \
+    c.phase_max[1000 + xs.n_bar] = dbgK, c.phase_max[2000 + xs.n_bar] = dbgM, c.phase_max[3000 + xs.n_bar] = t1 - t0;      \
   t0 = t1;
 #define X_TIME_BARRIER() t1 = globalTimerNs(), t_bar += t1 - t0, t0 = t1;
 #else
+#define X_DBG(k, m)
 #define X_TIME_WORK()
 #define X_TIME_BARRIER()
 #endif
-  // Barrier number n_bar of this launch: publishes what this CTA registered / changed in the phase, returns the totals and
+  // Barrier number xs.n_bar of this launch: publishes what this CTA registered / changed in the phase, returns the totals and
   // leaves the exclusive scan of the registrations in xs.pre.
-  int2* const count_base = reinterpret_cast<int2*>(c.xcounts);
-  unsigned int generation = 0;
-#define X_BARRIER(Kout, Mout)                                                                                                    \
-  X_TIME_WORK()                                                                                                                  \
-  counterBarrierScan(xs, c.barrier, generation, count_base + (n_bar & 1) * kMaxCtas, nctas, cta, tid, c.xseg, &(Kout), &(Mout));             \
-  X_TIME_BARRIER()                                                                                                               \
-  n_bar++;
+// `inc`: the ring advances by that much with the barrier.
+#define X_BARRIER(inc, Kout, Mout)                                                                                        \
+  X_TIME_WORK()                                                                                                           \
+  counterBarrierScan(xs, c.barrier, xs.generation, reinterpret_cast<int2*>(c.xcounts), nctas, cta, tid, c.xseg, inc,        \
+                     &(Kout), &(Mout));                                                                                   \
+  X_TIME_BARRIER()
   for (int pass = 0; pass < 2; pass++) {
     // pass 0: blocks with sites; pass 1: the persistent cleared list (:254-257)
     const int* src = pass ? c.cleared_list : c.upd_list;
     const int n0 = pass ? *(volatile int*)c.cleared_count : *(volatile int*)c.upd_count;
     if (n0 == 0) continue;
-    st.ci = st.ring & 1;
-    // ---- seeds: the call's block list is ring `ring`
+    // ---- seeds: the call's block list is ring xs.ring
     X_DBG(-1, n0)
+    if (lane64 == 0) xs.seeds[group] = n0;  // (n0 itself would be saved to the stack around every processSeed call)
     for (;;) {
       if (lane64 == 0) xs.cur[group] = atomicAdd(&xs.next, 1);
       groupSync(group);
       const long long e = (long long)cta + (long long)xs.cur[group] * nctas;
-      if (e >= n0) break;
-      processSeed(xc, xs, R, st.ring, __ldcg(src + e), cta, group, lane64);
+      if (e >= xs.seeds[group]) break;
+      processSeed(xs.ring, __ldcg(src + e));
     }
-    int M = n0, K, unused;
-    X_BARRIER(K, unused)  // K: candidates of ring `ring`
-    swept += n0;
+    int M = xs.seeds[group], K, unused;
+    X_BARRIER(0, K, unused)  // K: candidates of ring xs.ring
+    if (tid == 0) xs.swept += M;
     while (true) {
       X_DBG(K, M)
       if (NVB_WAVEX_TAIL && K <= kXG) {
@@ -756,32 +806,29 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
           }
           __syncthreads();
           while (true) {
-            if (group < K) processCandidate(xc, tab, xs, R, st.ring, xs.seg[group][0], xs.seg[group][1], 0, group, lane64, prof);
+            if (group < K) processCandidate(xs.ring);
             __syncthreads();
             const int K2 = min(xs.ncand, c.xseg), M2 = xs.nchanged;
             __syncthreads();
-            if (tid == 0) xs.ncand = 0, xs.nchanged = 0;
+            if (tid == 0) xs.ncand = 0, xs.nchanged = 0, xs.faces += 6 * M, xs.rings++, xs.swept += M2, xs.ring++;
             if (tid < kXG) xs.seg[tid][0] = 0, xs.seg[tid][1] = tid;  // the next ring's entries: segment 0, in order
-            faces += 6 * M, rings++, swept += M2, t++;
-            st.ring++, st.ci ^= 1;
+            t++;
             M = M2, K = K2;
             __syncthreads();
             if (M == 0 || K > kXG) break;
           }
-          n_tail += t;
-          if (tid == 0) c.xtail[0] = t, c.xtail[1] = K, c.xtail[2] = M;
+          if (tid == 0) xs.n_tail += t, c.xtail[0] = t, c.xtail[1] = K, c.xtail[2] = M;
         }
         {
           int k_unused, m_unused;  // (the tail's counts travel through xtail: CTA 0 alone registered)
-          X_BARRIER(k_unused, m_unused)
+          X_BARRIER(0, k_unused, m_unused)
         }
         if (cta != 0) {
           if (tid == 0) xs.bcast[0] = __ldcg(c.xtail + 0), xs.bcast[1] = __ldcg(c.xtail + 1), xs.bcast[2] = __ldcg(c.xtail + 2);
           __syncthreads();
-          const int t = xs.bcast[0];
           K = xs.bcast[1], M = xs.bcast[2];
+          if (tid == 0) xs.ring += xs.bcast[0];
           __syncthreads();
-          st.ring += t, st.ci ^= (t & 1);
         }
         if (M == 0) break;
         // the K candidates of the current ring were all registered by CTA 0
@@ -798,34 +845,32 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
         for (int s = lane64; s < nctas; s += 64)
           if (xs.pre[s] <= e && e < xs.pre[s + 1]) xs.seg[group][0] = s, xs.seg[group][1] = (int)e - xs.pre[s];
         groupSync(group);
-        processCandidate(xc, tab, xs, R, st.ring, xs.seg[group][0], xs.seg[group][1], cta, group, lane64, prof);
+        processCandidate(xs.ring);
       }
       int K2, M2;
-      X_BARRIER(K2, M2)
-      faces += 6 * M, rings++, swept += M2;
-      st.ring++, st.ci ^= 1;
+      X_BARRIER(1, K2, M2)
+      if (tid == 0) xs.faces += 6 * M, xs.rings++, xs.swept += M2;
       M = M2, K = K2;
       if (M == 0) break;
     }
-    st.ring++;  // the next computeEsdf call's stamps must not alias this one's
+    if (tid == 0) xs.ring++;  // the next computeEsdf call's stamps must not alias this one's
+    __syncthreads();
   }
 #undef X_BARRIER
 #undef X_TIME_WORK
 #undef X_TIME_BARRIER
 #undef X_DBG
   if (cta == 0 && tid == 0) {
-    *c.ring_id = st.ring + 1;
+    *c.ring_id = xs.ring + 1;
     c.stats[4] = *(volatile int*)c.cleared_count;
-    c.stats[5] = swept, c.stats[6] = faces, c.stats[7] = rings;
-    c.stats[10] = n_tail, c.stats[11] = n_bar;
+    c.stats[5] = xs.swept, c.stats[6] = xs.faces, c.stats[7] = xs.rings;
+    c.stats[10] = xs.n_tail, c.stats[11] = xs.n_bar;
 #if NVB_WAVEX_PROF
     c.stats[8] = t_bar, c.stats[9] = t_work;
     long long sum_max = 0;
-    for (int q = 0; q < n_bar && q < 1000; q++) sum_max += (long long)c.phase_max[q];
+    for (int q = 0; q < xs.n_bar && q < 1000; q++) sum_max += (long long)c.phase_max[q];
     c.stats[12] = sum_max;
-#endif
-#if NVB_WAVEX_PROF
-    for (int q = 0; q < 8; q++) c.phase_max[3990 + q] = prof[q];
+    for (int q = 0; q < 8; q++) c.phase_max[3990 + q] = xs.prof[0][q];
 #endif
   }
 }

@@ -560,6 +560,13 @@ class Mapper:
         check(self._L.nvb_mapper_esdf_time_split(self._h, out))
         return {"barrier_wait_ns_cta0": out[0], "axis_ns_cta0": out[1], "slowest_cta_work_ns": out[2], "barriers": out[3]}
 
+    def debug_phase_max(self, n=4000):
+        """The wavefront's per-phase debug words of the last update (filled only by a -DNVB_WAVEX_PROF=1 build; see
+        tools/wavex_profile.py for the layout) as an int64 array of `n` <= 4000 entries."""
+        out = (C.c_int64 * n)()
+        check(self._L.nvb_mapper_debug_phase_max(self._h, out, n))
+        return np.frombuffer(out, dtype=np.int64).copy()
+
     def __init__(self, voxel_size_m, device=0, tsdf_capacity_blocks=0, esdf_capacity_blocks=0,
                  esdf_persistent=3, projective_layer_type=ProjectiveLayerType.kTsdf, keep_last_view=False):
         self._L = _lib.load()
