@@ -27,7 +27,8 @@ class Plane {
   float d_;
 };
 
-// The subset of Eigen::AlignedBox3f the slicer's interface needs.
+// The subset of Eigen::AlignedBox3f the slicer's and the shape clearer's interfaces need (both builds: the reference's type is
+// Eigen::AlignedBox3f, whose arithmetic is restated here in Eigen's order).
 class AxisAlignedBoundingBox {
  public:
   AxisAlignedBoundingBox() = default;
@@ -43,6 +44,29 @@ class AxisAlignedBoundingBox {
     for (int a = 0; a < 3; a++) mn[a] = min_[a] < o.min_[a] ? min_[a] : o.min_[a], mx[a] = max_[a] > o.max_[a] ? max_[a] : o.max_[a];
     return AxisAlignedBoundingBox(mn, mx);
   }
+  // Eigen::AlignedBox::contains(point) / intersects(box): inclusive on both sides
+  bool contains(const Vector3f& p) const {
+    return min_[0] <= p[0] && min_[1] <= p[1] && min_[2] <= p[2] && p[0] <= max_[0] && p[1] <= max_[1] && p[2] <= max_[2];
+  }
+  bool intersects(const AxisAlignedBoundingBox& b) const {
+    return min_[0] <= b.max_[0] && min_[1] <= b.max_[1] && min_[2] <= b.max_[2] && b.min_[0] <= max_[0] &&
+           b.min_[1] <= max_[1] && b.min_[2] <= max_[2];
+  }
+  // Eigen::AlignedBox::squaredExteriorDistance / exteriorDistance: the axes accumulate in order from 0
+  float squaredExteriorDistance(const Vector3f& p) const {
+    float dist2 = 0.0f;
+    for (int k = 0; k < 3; k++) {
+      if (min_[k] > p[k]) {
+        const float aux = min_[k] - p[k];
+        dist2 += aux * aux;
+      } else if (p[k] > max_[k]) {
+        const float aux = p[k] - max_[k];
+        dist2 += aux * aux;
+      }
+    }
+    return dist2;
+  }
+  float exteriorDistance(const Vector3f& p) const { return std::sqrt(squaredExteriorDistance(p)); }
 
  private:
   Vector3f min_, max_;

@@ -9,6 +9,7 @@
 //                                                          mapper.h:52-53,119-124,374,456
 //   decayTsdfAllVoxels / decayTsdfExcludeLastView / decayOccupancy...   mapper.h:218-233
 //   tsdf_decay_integrator() / occupancy_decay_integrator()  mapper.h:496-504
+//   clearOutsideRadius / clearTsdfInsideShapes / getClearedBlocks  mapper.h:237,350,713
 #pragma once
 #include <memory>
 #include <type_traits>
@@ -16,6 +17,7 @@
 #include "nvblox/core/cuda_stream.h"
 #include "nvblox/integrators/weighting_function.h"
 #include "nvblox/geometry/plane.h"
+#include "nvblox/integrators/shape_clearer.h"
 #include "nvblox/map/layer.h"
 #include "nvblox/mesh/mesh_integrator.h"
 #include "nvblox/sensors/camera.h"
@@ -403,6 +405,32 @@ class Mapper {
     const float c[3] = {center[0], center[1], center[2]};
     b200_detail::check(nvb_mapper_mark_unobserved_free_inside_radius(m_, c, radius, nullptr, 0, nullptr),
                        "markUnobservedTsdfFreeInsideRadius", nvb_last_error());
+  }
+  // Mapper::clearOutsideRadius (mapper.h:350, src/mapper/mapper.cpp:473-492): the projective blocks farther than `radius` from
+  // `center` are deallocated with their ESDF, freespace, colour and mesh twins, and join getClearedBlocks' set.
+  void clearOutsideRadius(const Vector3f& center, float radius) {
+    const float c[3] = {center[0], center[1], center[2]};
+    b200_detail::check(nvb_mapper_clear_outside_radius(m_, c, radius, nullptr, 0, nullptr), "clearOutsideRadius", nvb_last_error());
+  }
+  // Mapper::clearTsdfInsideShapes (mapper.h:237, mapper.cpp:364-368): ShapeClearer<TsdfLayer> + addBlocksToUpdate
+  void clearTsdfInsideShapes(const std::vector<BoundingShape>& shapes) {
+    if (projective_layer_type_ == ProjectiveLayerType::kOccupancy) return;  // the TSDF layer is empty: nothing to clear
+    b200_detail::clearShapes(m_, NVB_LAYER_TSDF, shapes, tsdf_layer().numBlocks(), true);
+  }
+  // Mapper::getClearedBlocks (mapper.h:713, mapper.cpp:509-521): the blocks deallocated since the last call (by
+  // clearOutsideRadius or a decay), minus blocks_to_ignore, in (x, y, z) order; empties the set.
+  std::vector<Index3D> getClearedBlocks(const std::vector<Index3D>& blocks_to_ignore) {
+    std::vector<int32_t> ign;
+    for (const Index3D& k : blocks_to_ignore) ign.push_back(k[0]), ign.push_back(k[1]), ign.push_back(k[2]);
+    int32_t n = 0;
+    b200_detail::check(nvb_mapper_get_cleared_blocks(m_, nullptr, 0, nullptr, 0, &n), "getClearedBlocks", nvb_last_error());
+    std::vector<int32_t> raw(3 * (size_t)(n > 0 ? n : 1));
+    b200_detail::check(nvb_mapper_get_cleared_blocks(m_, ign.empty() ? nullptr : ign.data(), (int32_t)(ign.size() / 3), raw.data(),
+                                                     n, &n),
+                       "getClearedBlocks", nvb_last_error());
+    std::vector<Index3D> out;
+    for (int i = 0; i < n; i++) out.push_back(Index3D(raw[3 * i], raw[3 * i + 1], raw[3 * i + 2]));
+    return out;
   }
   // Mapper::integrateColor (mapper.h:202-207, mapper_impl.h:104-130)
   void integrateColor(const ColorImage& color_frame, const Transform& T_L_C, const Camera& camera) {

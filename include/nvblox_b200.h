@@ -392,6 +392,46 @@ NVB_API int32_t nvb_freespace_update_blocks(NvbMapper* m, const int32_t* blocks_
 NVB_API int32_t nvb_mapper_decay_exclude_last_view(NvbMapper* m, const NvbDecayExclusion* exclusion,
                                                    int32_t* removed_xyz_host, int32_t cap, int32_t* out_count);
 
+/* BoundingShape (C/include/nvblox/geometry/bounding_shape.h:26, bounding_spheres.h, bounding_boxes.h):
+ * NVB_SHAPE_SPHERE: a = centre, b[0] = radius; NVB_SHAPE_AABB: a = minimum corner, b = maximum corner. */
+typedef enum { NVB_SHAPE_SPHERE = 0, NVB_SHAPE_AABB = 1 } NvbShapeType;
+typedef struct NvbBoundingShape {
+  int32_t type; /* NvbShapeType */
+  float a[3];
+  float b[3];
+} NvbBoundingShape;
+
+/* Mapper::clearOutsideRadius(center, radius) (C/src/mapper/mapper.cpp:473-492): every block of the projective layer
+ * whose box is farther than `radius` from `center` (exteriorDistance > radius, strict; src/geometry/bounding_spheres.cpp:
+ * 23-31,47-50,69-74) is deallocated, and with it its twins (Mapper::clearBlocksInLayers, mapper.cpp:546-634): colour, mesh
+ * and freespace blocks, the ESDF block (3-D) or the column's slice block when no projective block is left in the column
+ * between the slice bounds (2-D). The blocks leave every initialised tracker consumer
+ * (BlocksToUpdateTracker::removeClearedBlocksFromTracking, src/map/blocks_to_update_tracker.cpp:75-90) and join the
+ * cleared-blocks set. The radius is not checked: radius <= 0 removes every block that does not contain the centre.
+ * removed_xyz_host (may be NULL) receives up to cap removed triples in (x, y, z) order; *out_count the number removed.
+ * Synchronous; waits for an ESDF update still in flight. */
+NVB_API int32_t nvb_mapper_clear_outside_radius(NvbMapper* m, const float center[3], float radius, int32_t* removed_xyz_host,
+                                                int32_t cap, int32_t* out_count);
+/* Mapper::clearTsdfInsideShapes(shapes) (mapper.cpp:364-368): ShapeClearer<TsdfLayer>::clear on the TSDF layer, then the
+ * touched blocks join every initialised tracker consumer (addBlocksToUpdate). Nothing is allocated or deallocated; on an
+ * occupancy mapper (no TSDF layer) nothing happens. updated_xyz_host (may be NULL) receives up to cap touched triples in
+ * (x, y, z) order; *out_count the number touched. Synchronous. */
+NVB_API int32_t nvb_mapper_clear_tsdf_inside_shapes(NvbMapper* m, const NvbBoundingShape* shapes, int32_t num_shapes,
+                                                    int32_t* updated_xyz_host, int32_t cap, int32_t* out_count);
+/* ShapeClearer<LayerType>::clear (C/include/nvblox/integrators/internal/cuda/impl/shape_clearer_impl.cuh:22-127) on the
+ * NVB_LAYER_TSDF, NVB_LAYER_OCCUPANCY or NVB_LAYER_COLOR layer: in every block a shape touches (sphere: exteriorDistance <
+ * radius; box: inclusive AlignedBox::intersects), the voxels whose centre a shape contains (sphere: distance <= radius; box:
+ * inclusive) are reset -- TSDF distance 0 and weight 0, occupancy log odds 0, colour Color::Gray() and weight 0. The
+ * tracker is not told. Output as for nvb_mapper_clear_tsdf_inside_shapes. Synchronous. */
+NVB_API int32_t nvb_layer_clear_shapes(NvbMapper* m, int32_t layer, const NvbBoundingShape* shapes, int32_t num_shapes,
+                                       int32_t* updated_xyz_host, int32_t cap, int32_t* out_count);
+/* Mapper::getClearedBlocks(blocks_to_ignore) (mapper.cpp:509-521): the blocks deallocated by nvb_mapper_clear_outside_radius
+ * or nvb_mapper_decay since the last call, minus ignore_xyz (may be NULL when n_ignore is 0), in (x, y, z) order; the set
+ * is emptied. out_xyz_host == NULL: *out_count receives the current set size and nothing changes. A set larger than cap
+ * fails with NVB_ERR_CAPACITY and stays as it is (the ignored blocks removed). */
+NVB_API int32_t nvb_mapper_get_cleared_blocks(NvbMapper* m, const int32_t* ignore_xyz, int32_t n_ignore, int32_t* out_xyz_host,
+                                              int32_t cap, int32_t* out_count);
+
 /* Mapper::updateEsdfSlice (mapper.h:331-343; EsdfMode::k2D) = EsdfIntegrator::integrateSlice with the constant-z
  * slice description (C/src/integrators/esdf_integrator.cu:283-347, markSitesInSlice :754-1055): the band
  * [slice_min_height, slice_max_height] of the projective layer (honouring the freespace layer if the mapper has one) is

@@ -970,42 +970,10 @@ __global__ void __launch_bounds__(kThreads) esdfRemoveBlocksKernel(EsdfCtx c, co
   }
 }
 
-// Drops the deallocated slots from the persistent cleared list (stable, one CTA).
-__global__ void __launch_bounds__(kThreads) esdfFilterClearedKernel(EsdfCtx c) {
-  __shared__ int s_base, s_warp[kThreads / 32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = *c.cleared_count;
-  if (tid == 0) s_base = 0;
-  __syncthreads();
-  for (int first = 0; first < n; first += kThreads) {
-    const int i = first + tid;
-    int slot = -1;
-    bool keep = false;
-    if (i < n) {
-      slot = c.cleared_list[i];
-      keep = c.esdf.block_index[3 * slot] != kDeadSlotX;
-    }
-    const unsigned int ballot = __ballot_sync(0xffffffffu, keep);
-    if (lane == 0) s_warp[warp] = __popc(ballot);
-    __syncthreads();  // also: every thread has read its entry before anyone overwrites the list
-    int off = s_base;
-    for (int w = 0; w < warp; w++) off += s_warp[w];
-    if (keep) c.cleared_list[off + __popc(ballot & ((1u << lane) - 1u))] = slot;
-    __syncthreads();
-    if (tid == 0) {
-      int total = 0;
-      for (int w = 0; w < kThreads / 32; w++) total += s_warp[w];
-      s_base += total;
-    }
-    __syncthreads();
-  }
-  if (tid == 0) *c.cleared_count = s_base;
-}
-
 void launchEsdfRemoveBlocks(const EsdfCtx& c, const int4* dead, const int* dead_count, int upper, cudaStream_t stream) {
   int grid = upper < 1184 ? (upper < 1 ? 1 : upper) : 1184;
   esdfRemoveBlocksKernel<<<grid, kThreads, 0, stream>>>(c, dead, dead_count);
-  esdfFilterClearedKernel<<<1, kThreads, 0, stream>>>(c);
+  launchDropDeadSlots(c.esdf, c.cleared_list, c.cleared_count, stream);  // off the persistent cleared list
 }
 
 // ---------------------------------------------------------------------------

@@ -69,6 +69,24 @@ __host__ __device__ __forceinline__ int3 blockIndexFromPosition(float block_size
                    floatToIntRz(floorf(p.z / block_size)));
 }
 
+// AlignedBox::exteriorDistance(c) of getAABBOfBlock(block_size, idx) (geometry/internal/impl/bounding_boxes_impl.h:55-60,
+// src/geometry/bounding_spheres.cpp:23-31): Eigen's squaredExteriorDistance accumulates the axes in order from 0.
+__host__ __device__ __forceinline__ float blockExteriorDistance(const int idx[3], float block_size, const float c[3]) {
+  float dist2 = 0.0f;
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    const float bmin = (float)idx[k] * block_size, bmax = ((float)idx[k] + 1.0f) * block_size;
+    if (bmin > c[k]) {
+      const float aux = bmin - c[k];
+      dist2 += aux * aux;
+    } else if (c[k] > bmax) {
+      const float aux = c[k] - bmax;
+      dist2 += aux * aux;
+    }
+  }
+  return sqrtf(dist2);
+}
+
 // ---------------------------------------------------------------------------
 // Radial-tangential lens distortion (sensors/internal/impl/distortion_impl.h). The reference mixes
 // float and double through its `1.0` / `2.0` literals; the same promotions are spelled out here.
@@ -594,5 +612,30 @@ void launchSliceImage(const DevLayer& esdf, float block_size, float min_x, float
                       int rows, int cols, float* image, signed char* grid, cudaStream_t stream);
 void launchRemoveBlocks(const DevLayer& layer, const int4* dead, const int* dead_count, int upper, cudaStream_t stream);
 void launchTodoAll(const DevLayer& tsdf, int* dirty, int* todo_slots, int* todo_count, cudaStream_t stream);
+// Drops the slots that are dead in `layer` from a list of its slots (*count entries), keeping the order of the others.
+void launchDropDeadSlots(const DevLayer& layer, int* list, int* count, cudaStream_t stream);
+
+// nvb_clear.cu: map clearing (Mapper::clearOutsideRadius, ShapeClearer)
+// Blocks of `layer` whose box is farther than `radius` from the centre -> dead {slot, x, y, z} (*dead_count zeroed before).
+void launchSelectOutsideRadius(const DevLayer& layer, const float center[3], float radius, float block_size, int4* dead,
+                               int* dead_count, cudaStream_t stream);
+// BlocksToUpdateTracker::removeClearedBlocksFromTracking: zero the dirty words of the dead slots (null arrays skipped); the
+// todo lists then lose them through launchDropDeadSlots.
+void launchTrackerDropDead(const int4* dead, const int* dead_count, int upper, int* dirty0, int* dirty1, int* dirty2,
+                           cudaStream_t stream);
+struct ShapeClearArgs {
+  DevLayer layer;
+  int voxel_kind;                    // 0 TsdfVoxel, 1 OccupancyVoxel, 2 ColorVoxel
+  const NvbBoundingShape* shapes;    // device
+  int num_shapes;
+  float block_size;
+  int4* sel;                         // {slot, x, y, z} of the blocks a shape touches
+  int* sel_count;
+  int *dirty, *todo_slots, *todo_count;     // ESDF tracker (null: not told)
+  int *dirty2, *todo2_slots, *todo2_count;  // freespace tracker
+  int *dirty3, *todo3_slots, *todo3_count;  // mesh tracker
+};
+void launchShapeSelect(const ShapeClearArgs& a, cudaStream_t stream);
+void launchShapeClear(const ShapeClearArgs& a, int num_sms, cudaStream_t stream);
 
 }  // namespace nvb

@@ -344,19 +344,7 @@ __global__ void __launch_bounds__(256) markFreeSphereKernel(const __grid_constan
   const float c[3] = {a.cx, a.cy, a.cz};
   for (int cell = warp; cell < a.cells; cell += nwarps) {
     const int idx[3] = {a.lo.x + cell / (a.size.y * a.size.z), a.lo.y + (cell / a.size.z) % a.size.y, a.lo.z + cell % a.size.z};
-    float dist2 = 0.0f;
-#pragma unroll
-    for (int k = 0; k < 3; k++) {  // Eigen AlignedBox::squaredExteriorDistance of getAABBOfBlock
-      const float bmin = (float)idx[k] * a.block_size, bmax = ((float)idx[k] + 1.0f) * a.block_size;
-      if (bmin > c[k]) {
-        const float aux = bmin - c[k];
-        dist2 += aux * aux;
-      } else if (c[k] > bmax) {
-        const float aux = c[k] - bmax;
-        dist2 += aux * aux;
-      }
-    }
-    if (!(sqrtf(dist2) < a.radius)) continue;
+    if (!(blockExteriorDistance(idx, a.block_size, c) < a.radius)) continue;
     int slot = -1;
     if (lane == 0) {
       bool was_new;

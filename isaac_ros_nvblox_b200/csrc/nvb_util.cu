@@ -147,6 +147,36 @@ __global__ void removeBlocksKernel(DevLayer L, const int4* dead, const int* dead
   }
 }
 
+// Drops the slots that are dead in L from a list of its slots, keeping the order of the others (the ESDF's persistent cleared
+// list, the tracker's todo lists). In place, one CTA: a chunk is read completely before any of it is written, and the write
+// position never passes the read position.
+__global__ void __launch_bounds__(1024) dropDeadSlotsKernel(DevLayer L, int* list, int* count) {
+  __shared__ int s_base, s_warp[32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int n = *count;
+  if (tid == 0) s_base = 0;
+  __syncthreads();
+  for (int first = 0; first < n; first += blockDim.x) {
+    const int i = first + tid;
+    const int slot = i < n ? list[i] : -1;
+    const bool keep = slot >= 0 && L.block_index[3 * slot] != kDeadSlotX;
+    const unsigned int ballot = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    int before = s_base;
+    for (int w = 0; w < warp; w++) before += s_warp[w];
+    if (keep) list[before + __popc(ballot & ((1u << lane) - 1u))] = slot;
+    __syncthreads();
+    if (tid == 0) {
+      int total = 0;
+      for (int w = 0; w < (int)(blockDim.x >> 5); w++) total += s_warp[w];
+      s_base += total;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) *count = s_base;
+}
+
 // EsdfSlicer::getAabbOfLayerAtHeight (src/integrators/esdf_slicer.cu:112-135): extreme x / y block indices at height zb.
 __global__ void sliceAabbKernel(DevLayer L, int zb, int* out4) {
   const int n = *L.count < L.capacity ? *L.count : L.capacity;
@@ -210,6 +240,10 @@ void launchSliceImage(const DevLayer& esdf, float block_size, float min_x, float
 void launchRemoveBlocks(const DevLayer& layer, const int4* dead, const int* dead_count, int upper, cudaStream_t stream) {
   int grid = upper < 1184 ? (upper < 1 ? 1 : upper) : 1184;
   removeBlocksKernel<<<grid, 256, 0, stream>>>(layer, dead, dead_count);
+}
+
+void launchDropDeadSlots(const DevLayer& layer, int* list, int* count, cudaStream_t stream) {
+  dropDeadSlotsKernel<<<1, 1024, 0, stream>>>(layer, list, count);
 }
 
 void launchGatherBlocks(const DevLayer& layer, const int* xyz_dev, int n, unsigned char* out, unsigned char* found,

@@ -18,7 +18,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (NvbCamera, NvbDecayExclusion, NvbEsdfParams, NvbEsdfSliceParams, NvbFreespaceParams, NvbMapperOptions, NvbOccupancyDecayParams,
+from ._lib import (NvbBoundingShape, NvbCamera, NvbDecayExclusion, NvbEsdfParams, NvbEsdfSliceParams, NvbFreespaceParams, NvbMapperOptions, NvbOccupancyDecayParams,
                    NvbOccupancyParams, NvbTsdfDecayParams, NvbTsdfParams, check)
 
 TSDF_VOXEL_DTYPE = np.dtype([("distance", "<f4"), ("weight", "<f4")])
@@ -75,6 +75,46 @@ class Camera:
     height = property(lambda s: s.c.height)
 
 
+class BoundingSphere:
+    """nvblox::BoundingSphere(center, radius) (geometry/bounding_spheres.h): contains p when |center - p| <= radius."""
+
+    def __init__(self, center, radius):
+        self.center = np.asarray(center, dtype=np.float32).reshape(3)
+        self.radius = np.float32(radius)
+
+    def _c(self):
+        return NvbBoundingShape(_lib.NVB_SHAPE_SPHERE, (C.c_float * 3)(*self.center.tolist()),
+                                (C.c_float * 3)(float(self.radius), 0.0, 0.0))
+
+
+class AxisAlignedBoundingBox:
+    """nvblox::AxisAlignedBoundingBox(min, max) (Eigen::AlignedBox3f, geometry/bounding_boxes.h): inclusive on both sides."""
+
+    def __init__(self, min, max):  # noqa: A002 (the reference's argument names)
+        self.min = np.asarray(min, dtype=np.float32).reshape(3)
+        self.max = np.asarray(max, dtype=np.float32).reshape(3)
+
+    def _c(self):
+        return NvbBoundingShape(_lib.NVB_SHAPE_AABB, (C.c_float * 3)(*self.min.tolist()), (C.c_float * 3)(*self.max.tolist()))
+
+
+def _shape_array(shapes):
+    shapes = list(shapes)
+    arr = (NvbBoundingShape * max(len(shapes), 1))()
+    for i, s in enumerate(shapes):
+        arr[i] = s._c()
+    return arr, len(shapes)
+
+
+def _clear_shapes_call(fn, cap, *args):
+    """Run a shape-clearing entry point and return the touched (n, 3) block indices in (x, y, z) order."""
+    cap = max(int(cap), 1)
+    out = np.zeros((cap, 3), dtype=np.int32)
+    n = C.c_int32(0)
+    check(fn(*args, _ip(out), cap, C.byref(n)))
+    return out[:n.value].copy()
+
+
 class _Layer:
     """BlockLayer queries (map/layer.h:76-311) answered from the device-resident map."""
 
@@ -120,6 +160,13 @@ class _Layer:
         idx = np.ascontiguousarray(indices, dtype=np.int32).reshape(-1, 3)
         v = np.ascontiguousarray(voxels, dtype=self._dtype).reshape(idx.shape[0], 8, 8, 8)
         check(self._m._L.nvb_layer_set_blocks(self._m._h, self._id, _ip(idx), idx.shape[0], v.ctypes.data))
+
+    def clear_shapes(self, shapes):
+        """ShapeClearer<LayerType>::clear(shapes, layer) (integrators/shape_clearer.h) on a TSDF, occupancy or colour layer:
+        voxels whose centre lies in a BoundingSphere / AxisAlignedBoundingBox are reset. The tracker is not told. Returns the
+        touched (n, 3) block indices in (x, y, z) order."""
+        arr, n = _shape_array(shapes)
+        return _clear_shapes_call(self._m._L.nvb_layer_clear_shapes, self.num_blocks(), self._m._h, self._id, arr, n)
 
     def block_device_ptr(self, index):
         k = np.asarray(index, dtype=np.int32)
@@ -752,6 +799,36 @@ class Mapper:
                                            depth.shape[1], _fp(T), C.byref(camera.c), _ip(out), cap, C.byref(n)))
         else:
             check(self._L.nvb_mapper_decay(self._h, C.byref(x), None, 0, 0, 0, None, None, _ip(out), cap, C.byref(n)))
+        return out[:n.value].copy()
+
+    def clear_outside_radius(self, center, radius):
+        """Mapper::clearOutsideRadius(center, radius) (mapper.h; src/mapper/mapper.cpp:473-492): deallocates every projective
+        block farther than `radius` from `center`, with its ESDF, freespace, colour and mesh twins. Returns the removed (n, 3)
+        block indices in (x, y, z) order."""
+        c = np.ascontiguousarray(center, dtype=np.float32).reshape(3)
+        cap = max(self._occupancy.num_blocks() if self._projective_layer_type == 1 else self._tsdf.num_blocks(), 1)
+        out = np.zeros((cap, 3), dtype=np.int32)
+        n = C.c_int32(0)
+        check(self._L.nvb_mapper_clear_outside_radius(self._h, _fp(c), float(radius), _ip(out), cap, C.byref(n)))
+        return out[:n.value].copy()
+
+    def clear_tsdf_inside_shapes(self, shapes):
+        """Mapper::clearTsdfInsideShapes(shapes) (src/mapper/mapper.cpp:364-368): TSDF voxels inside the shapes are reset and
+        their blocks join the tracker. Returns the touched (n, 3) block indices in (x, y, z) order (none on an occupancy
+        mapper)."""
+        arr, n = _shape_array(shapes)
+        cap = self._tsdf.num_blocks() if self._projective_layer_type != ProjectiveLayerType.kOccupancy else 0
+        return _clear_shapes_call(self._L.nvb_mapper_clear_tsdf_inside_shapes, cap, self._h, arr, n)
+
+    def get_cleared_blocks(self, blocks_to_ignore=()):
+        """Mapper::getClearedBlocks(blocks_to_ignore) (src/mapper/mapper.cpp:509-521): the blocks deallocated by
+        clear_outside_radius or a decay since the last call, minus `blocks_to_ignore`, in (x, y, z) order; empties the set."""
+        ign = np.ascontiguousarray(np.asarray(blocks_to_ignore, dtype=np.int32).reshape(-1, 3))
+        n = C.c_int32(0)
+        check(self._L.nvb_mapper_get_cleared_blocks(self._h, None, 0, None, 0, C.byref(n)))
+        cap = max(n.value, 1)
+        out = np.zeros((cap, 3), dtype=np.int32)
+        check(self._L.nvb_mapper_get_cleared_blocks(self._h, _ip(ign) if len(ign) else None, len(ign), _ip(out), cap, C.byref(n)))
         return out[:n.value].copy()
 
     def decay_exclude_last_view(self):
