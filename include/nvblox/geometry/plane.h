@@ -12,6 +12,14 @@ class Plane {
   Plane(const Vector3f& normal, const Vector3f& point) : normal_(normalized(normal)) {
     d_ = -(point[0] * normal_[0] + (point[1] * normal_[1] + point[2] * normal_[2]));
   }
+  // The plane with exactly these coefficients, without normalising again (the library's planes are already unit length;
+  // the reference hands its Plane objects back by copy).
+  static Plane fromCoefficients(const Vector3f& unit_normal, float d) {
+    Plane p;
+    p.normal_ = unit_normal;
+    p.d_ = d;
+    return p;
+  }
   const Vector3f& normal() const { return normal_; }
   float d() const { return d_; }
   float offset() const { return d_; }

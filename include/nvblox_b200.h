@@ -450,6 +450,46 @@ NVB_API int32_t nvb_esdf_integrate_slice_planar_blocks(NvbMapper* m, const float
 /* EsdfIntegrator::integrateSlice(layer, block_indices, esdf_layer) on an explicit block list (esdf_integrator.h:96-118). */
 NVB_API int32_t nvb_esdf_integrate_slice_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks);
 
+/* GroundPlaneEstimator (C/include/nvblox/experimental/ground_plane/ground_plane_estimator.h,
+ * ground_plane_estimator_params.h, ransac_plane_fitter_params.h, tsdf_zero_crossings_extractor.h), one per mapper. */
+typedef struct NvbGroundPlaneParams {
+  float ground_points_candidates_min_z_m; /* -0.1: candidates keep min_z <= z <= max_z */
+  float ground_points_candidates_max_z_m; /* 0.15 */
+  float ransac_distance_threshold_m;      /* 0.2: MSAC inlier threshold t */
+  int32_t num_ransac_iterations;          /* 1000, >= 1 */
+  float min_tsdf_weight;                  /* 0.1: both voxels of a crossing need weight >= this */
+  int32_t max_crossings;                  /* 360000: a layer with this many crossings or more gives no plane */
+} NvbGroundPlaneParams;
+NVB_API void nvb_default_ground_plane_params(NvbGroundPlaneParams* p);
+NVB_API int32_t nvb_mapper_set_ground_plane_params(NvbMapper* m, const NvbGroundPlaneParams* p);
+NVB_API int32_t nvb_mapper_get_ground_plane_params(const NvbMapper* m, NvbGroundPlaneParams* p);
+/* GroundPlaneEstimator::computeGroundPlane(tsdf_layer) (ground_plane_estimator.cpp:27-62):
+ *   1. the zero crossings from above of the TSDF layer (computeZeroCrossingsFromAboveOnGPU): every voxel pair (v, v + z)
+ *      with both weights >= min_tsdf_weight, distance(v + z) > 0 and distance(v) <= 0 gives the point
+ *      centre(v) + (0, 0, -d(v) * voxel_size / (d(v + z) - d(v))); pairs whose upper voxel lies in a missing block are
+ *      skipped. The list is in canonical order: block index (x, y, z) lexicographically, then voxel (x, y, z);
+ *   2. the ground candidates: the finite crossings with min_z <= z <= max_z, in the same order;
+ *   3. the MSAC plane of the candidates (as nvb_ransac_fit_plane).
+ * *found = 0 when the layer has no blocks, the mapper has no TSDF layer (occupancy), the crossings number max_crossings or
+ * more, fewer than 3 candidates remain or no sample gives a plane; the estimator's last crossings, candidates and plane are
+ * then cleared (resetInternal). Otherwise plane = {nx, ny, nz, d} (unit normal, n . p + d = 0) and all three are kept.
+ * Synchronous: reads back the two counts and the 20-byte result only. */
+NVB_API int32_t nvb_mapper_compute_ground_plane(NvbMapper* m, float plane[4], int32_t* found);
+/* GroundPlaneEstimator::ground_plane(): the plane of the last computeGroundPlane, *found = 0 if there is none. */
+NVB_API int32_t nvb_mapper_ground_plane(NvbMapper* m, float plane[4], int32_t* found);
+typedef enum { NVB_GROUND_POINTS_CROSSINGS = 0, NVB_GROUND_POINTS_CANDIDATES = 1 } NvbGroundPoints;
+/* tsdf_zero_crossings() / tsdf_zero_crossings_ground_candidates() of the last computeGroundPlane: *valid = 0 if there are
+ * none (never computed or cleared by a failure); else *n = the number of points and up to cap of them are written to
+ * xyz (x, y, z floats; may be NULL) in the canonical order. */
+NVB_API int32_t nvb_mapper_ground_plane_points(NvbMapper* m, int32_t which, float* xyz, int32_t cap, int32_t* n, int32_t* valid);
+/* RansacPlaneFitter::fit (ransac_plane_fitter.cu:29-144), MSAC: iteration i draws three indices curand() % n from the
+ * XORWOW state curand_init(1234, i, 0), builds Plane::planeFromPoints (rejects equal or collinear samples) and sums, over
+ * the points in order and in float, d^2 if |d| < threshold else threshold^2. The lowest cost wins (lowest iteration on
+ * ties). *found = 0 for n < 3 or when every sample is rejected. points: n x 3 floats on the host or the device (memory).
+ * Uses the mapper's device, stream and cached generator states; the estimator's state is not touched. Synchronous. */
+NVB_API int32_t nvb_ransac_fit_plane(NvbMapper* m, const float* points, int32_t memory, int32_t n, int32_t num_ransac_iterations,
+                                     float ransac_distance_threshold_m, float plane[4], int32_t* found);
+
 /* EsdfSlicer::sliceLayerToDistanceImage (C/include/nvblox/integrators/esdf_slicer.h:52-78, C/src/integrators/esdf_slicer.cu:
  * 25-67,112-215) and, if grid_host != NULL, EsdfSlicer::occupancyGridFromSliceImage (:78-110,254-300) of the ESDF layer
  * (3-D or 2-D) at slice_height_m: one pixel per voxel over the AABB of the ESDF blocks at that height, rows along y,

@@ -45,6 +45,8 @@ EXPORTED_SYMBOLS = [
     "nvb_mapper_kernel_launches",
     "nvb_mapper_clear_outside_radius", "nvb_mapper_clear_tsdf_inside_shapes", "nvb_layer_clear_shapes",
     "nvb_mapper_get_cleared_blocks",
+    "nvb_default_ground_plane_params", "nvb_mapper_set_ground_plane_params", "nvb_mapper_get_ground_plane_params",
+    "nvb_mapper_compute_ground_plane", "nvb_mapper_ground_plane", "nvb_mapper_ground_plane_points", "nvb_ransac_fit_plane",
 ]
 
 
@@ -128,6 +130,15 @@ NVB_SHAPE_SPHERE, NVB_SHAPE_AABB = 0, 1
 
 class NvbBoundingShape(C.Structure):
     _fields_ = [("type", C.c_int32), ("a", C.c_float * 3), ("b", C.c_float * 3)]
+
+
+NVB_GROUND_POINTS_CROSSINGS, NVB_GROUND_POINTS_CANDIDATES = 0, 1
+
+
+class NvbGroundPlaneParams(C.Structure):
+    _fields_ = [("ground_points_candidates_min_z_m", C.c_float), ("ground_points_candidates_max_z_m", C.c_float),
+                ("ransac_distance_threshold_m", C.c_float), ("num_ransac_iterations", C.c_int32),
+                ("min_tsdf_weight", C.c_float), ("max_crossings", C.c_int32)]
 
 
 class NvbMapperOptions(C.Structure):
@@ -273,6 +284,14 @@ def load(path=None):
     L.nvb_mapper_clear_tsdf_inside_shapes.argtypes = [vp, C.POINTER(NvbBoundingShape), i32, ip, i32, ip]
     L.nvb_layer_clear_shapes.argtypes = [vp, i32, C.POINTER(NvbBoundingShape), i32, ip, i32, ip]
     L.nvb_mapper_get_cleared_blocks.argtypes = [vp, ip, i32, ip, i32, ip]
+    L.nvb_default_ground_plane_params.argtypes = [C.POINTER(NvbGroundPlaneParams)]
+    L.nvb_default_ground_plane_params.restype = None
+    L.nvb_mapper_set_ground_plane_params.argtypes = [vp, C.POINTER(NvbGroundPlaneParams)]
+    L.nvb_mapper_get_ground_plane_params.argtypes = [vp, C.POINTER(NvbGroundPlaneParams)]
+    L.nvb_mapper_compute_ground_plane.argtypes = [vp, fp, ip]
+    L.nvb_mapper_ground_plane.argtypes = [vp, fp, ip]
+    L.nvb_mapper_ground_plane_points.argtypes = [vp, i32, fp, i32, ip, ip]
+    L.nvb_ransac_fit_plane.argtypes = [vp, vp, i32, i32, i32, f32, fp, ip]
     L.nvb_mapper_kernel_launches.restype = C.c_int64
     for name in EXPORTED_SYMBOLS:
         f = getattr(L, name)

@@ -208,6 +208,34 @@ struct NvbMapper {
   int shape_sel_cap = 0;
   NvbBoundingShape* shapes_dev = nullptr;
   int shapes_cap = 0;
+  // ground-plane estimator (nvb_ground.cu): parameters, device scratch, the last result (GroundPlaneEstimator's optionals)
+  NvbGroundPlaneParams gp{};
+  unsigned long long* gp_keys = nullptr;  // 2 x gp_blocks_cap: packIndex keys of the TSDF slots, then the sorted keys
+  int* gp_slots = nullptr;                // 2 x gp_blocks_cap: the slots, then the slots in (x, y, z) block-index order
+  int2* gp_counts = nullptr;              // gp_blocks_cap
+  int gp_blocks_cap = 0;
+  void* gp_sort_temp = nullptr;           // the radix sort's scratch
+  size_t gp_sort_temp_bytes = 0;
+  float* gp_fit_stage = nullptr;          // nvb_ransac_fit_plane: host points staged on the device (3 floats each)
+  int gp_fit_stage_cap = 0;
+  int* gp_totals = nullptr;
+  float3* gp_crossings = nullptr;
+  int gp_crossings_cap = 0;
+  float4* gp_candidates = nullptr;
+  int gp_candidates_cap = 0;
+  float4* gp_fit_points = nullptr;  // nvb_ransac_fit_plane's own copy of its points
+  int gp_fit_points_cap = 0;
+  void* gp_states = nullptr;        // curand_init(1234, i, 0) for i < gp_states_n
+  int gp_states_n = 0;
+  float* gp_costs = nullptr;  // per iteration
+  int gp_costs_cap = 0;
+  float4* gp_planes = nullptr;
+  int gp_planes_cap = 0;
+  float* gp_result = nullptr;       // {nx, ny, nz, d, found}
+  bool gp_valid = false;            // crossings and candidates of the last computation are kept
+  int gp_num_crossings = 0, gp_num_candidates = 0;
+  bool gp_found = false;
+  float gp_plane[4] = {0, 0, 0, 0};
   // last integrated view (Mapper::last_posed_depth_image_, mapper.h:830-833), kept when keep_last_view is set
   int keep_last_view = 0;
   float* last_depth = nullptr;
@@ -1216,6 +1244,7 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   nvb_default_freespace_params(&m->fp);
   nvb_default_esdf_slice_params(&m->sp);
   nvb_default_color_params(&m->cp);
+  nvb_default_ground_plane_params(&m->gp);
   m->projective_layer_type = opts->projective_layer_type;
   m->keep_last_view = opts->keep_last_view ? 1 : 0;
   m->esdf_persistent = opts->esdf_persistent;
@@ -1340,6 +1369,9 @@ void nvb_mapper_destroy(NvbMapper* m) {
   cudaFree(m->xslab), cudaFree(m->xrec), cudaFree(m->xcounts);
   cudaFree(m->dead), cudaFree(m->skip_stamp), cudaFree(m->dead_cleared_xyz), cudaFree(m->last_depth);
   cudaFree(m->shape_sel), cudaFree(m->shapes_dev);
+  cudaFree(m->gp_keys), cudaFree(m->gp_sort_temp), cudaFree(m->gp_fit_stage);
+  cudaFree(m->gp_slots), cudaFree(m->gp_counts), cudaFree(m->gp_totals), cudaFree(m->gp_crossings), cudaFree(m->gp_candidates);
+  cudaFree(m->gp_fit_points), cudaFree(m->gp_states), cudaFree(m->gp_costs), cudaFree(m->gp_planes), cudaFree(m->gp_result);
   cudaFree(m->pre_depth);
   cudaFree(m->union_list), cudaFree(m->union_list_count);
   if (m->mesh.blocks) freeLayer(&m->mesh);
@@ -2448,6 +2480,229 @@ static int32_t integrateSliceBlocksImpl(NvbMapper* m, const float* plane, const 
   if (rc) return rc;
   if ((rc = nvb_mapper_synchronize(m))) return rc;
   return tightenEsdfBound(m);
+}
+
+void nvb_default_ground_plane_params(NvbGroundPlaneParams* p) {
+  if (!p) return;
+  // ground_plane_estimator_params.h, ransac_plane_fitter_params.h, tsdf_zero_crossings_extractor.h
+  p->ground_points_candidates_min_z_m = -0.1f;
+  p->ground_points_candidates_max_z_m = 0.15f;
+  p->ransac_distance_threshold_m = 0.2f;
+  p->num_ransac_iterations = 1000;
+  p->min_tsdf_weight = 0.1f;
+  p->max_crossings = 360000;
+}
+int32_t nvb_mapper_set_ground_plane_params(NvbMapper* m, const NvbGroundPlaneParams* p) {
+  if (!m || !p) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (p->num_ransac_iterations < 1) return fail(NVB_ERR_INVALID_ARGUMENT, "num_ransac_iterations must be >= 1");
+  m->gp = *p;
+  return NVB_OK;
+}
+int32_t nvb_mapper_get_ground_plane_params(const NvbMapper* m, NvbGroundPlaneParams* p) {
+  if (!m || !p) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  *p = m->gp;
+  return NVB_OK;
+}
+}  // extern "C"
+
+namespace {
+// Grows a device array to at least n elements (contents not kept).
+template <typename T>
+int ensureDevice(T** p, int* cap, long long n) {
+  if (*cap >= n) return NVB_OK;
+  const long long want = std::max(n, 2ll * *cap);
+  if (*p) cudaFree(*p);
+  *p = nullptr;
+  *cap = 0;
+  NVB_CUDA(cudaMalloc(p, (size_t)want * sizeof(T)));
+  *cap = (int)want;
+  return NVB_OK;
+}
+
+// RansacPlaneFitter::fit on n points already on the device (float4); the generator states of new iterations are made
+// once and kept.
+int ransacFit(NvbMapper* m, const float4* pts, int n, int iterations, float threshold, float plane[4], int* found) {
+  *found = 0;
+  if (n < 3) return NVB_OK;  // "We need at least three points to form a plane"
+  if (iterations > m->gp_states_n) {
+    // The existing states are kept; the new array replaces them only once it is complete (no leak on failure).
+    void* st = nullptr;
+    NVB_CUDA(cudaMalloc(&st, (size_t)iterations * ransacStateBytes()));
+    cudaError_t e = cudaSuccess;
+    if (m->gp_states_n)
+      e = cudaMemcpyAsync(st, m->gp_states, (size_t)m->gp_states_n * ransacStateBytes(), cudaMemcpyDeviceToDevice, m->stream);
+    if (e == cudaSuccess) {
+      launchRansacInit(st, m->gp_states_n, iterations, m->stream);
+      m->launches++;
+      e = cudaStreamSynchronize(m->stream);
+    }
+    if (e != cudaSuccess) {
+      cudaFree(st);
+      return fail(NVB_ERR_CUDA, std::string("RANSAC generator states: ") + cudaGetErrorString(e));
+    }
+    cudaFree(m->gp_states);
+    m->gp_states = st;
+    m->gp_states_n = iterations;
+  }
+  int rc = ensureDevice(&m->gp_costs, &m->gp_costs_cap, iterations);
+  if (!rc) rc = ensureDevice(&m->gp_planes, &m->gp_planes_cap, iterations);
+  if (rc) return rc;
+  if (!m->gp_result) NVB_CUDA(cudaMalloc(&m->gp_result, 5 * sizeof(float)));
+  // A/B switch for measurements: the reference's launch shape (256-thread CTAs, points read from global memory)
+  const char* e = getenv("NVB_RANSAC_REFERENCE_SHAPE");
+  const bool reference_shape = e && atoi(e) == 1;
+  launchRansacFit(pts, n, iterations, threshold, m->gp_states, m->gp_costs, m->gp_planes, m->gp_result, reference_shape, m->stream);
+  m->launches += 2;
+  float out[5];
+  NVB_CUDA(cudaMemcpyAsync(out, m->gp_result, sizeof(out), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  int f = 0;
+  std::memcpy(&f, &out[4], sizeof(int));
+  if (f) {
+    std::memcpy(plane, out, 4 * sizeof(float));
+    *found = 1;
+  }
+  return NVB_OK;
+}
+
+void groundReset(NvbMapper* m) {  // GroundPlaneEstimator::resetInternal
+  m->gp_valid = false, m->gp_found = false;
+  m->gp_num_crossings = m->gp_num_candidates = 0;
+}
+}  // namespace
+
+extern "C" {
+
+int32_t nvb_mapper_compute_ground_plane(NvbMapper* m, float plane[4], int32_t* found) {
+  if (!m || !found) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  *found = 0;
+  groundReset(m);
+  // an occupancy mapper's TsdfLayer is empty: no blocks, no plane
+  if (m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY) return NVB_OK;
+  NVB_CUDA(cudaSetDevice(m->device));
+  // The TSDF layer is written on `stream` only; the ESDF stream does not touch it.
+  int hw = 0;
+  NVB_CUDA(cudaMemcpyAsync(&hw, m->tsdf.count, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  hw = std::min(hw, m->tsdf.capacity);
+  if (hw == 0) return NVB_OK;  // "tsdf_layer.numBlocks() == 0"
+  // The slots below the high-water mark in (x, y, z) block-index order, sorted on the device; free slots sort last and
+  // count nothing (a layer whose slots are all free gives no crossings, hence no plane, like an empty one).
+  if (hw > m->gp_blocks_cap) {
+    const int cap = std::max(hw, 2 * m->gp_blocks_cap);
+    int dummy = 0, rc = ensureDevice(&m->gp_keys, &dummy, 2ll * cap);
+    if (!rc) dummy = 0, rc = ensureDevice(&m->gp_slots, &dummy, 2ll * cap);
+    if (!rc) dummy = 0, rc = ensureDevice(&m->gp_counts, &dummy, cap);
+    if (rc) {
+      m->gp_blocks_cap = 0;
+      return rc;
+    }
+    m->gp_blocks_cap = cap;
+  }
+  const size_t temp_bytes = groundSortTempBytes(hw);
+  if (temp_bytes > m->gp_sort_temp_bytes) {
+    cudaFree(m->gp_sort_temp);
+    m->gp_sort_temp = nullptr;
+    m->gp_sort_temp_bytes = 0;
+    NVB_CUDA(cudaMalloc(&m->gp_sort_temp, temp_bytes));
+    m->gp_sort_temp_bytes = temp_bytes;
+  }
+  int rc = NVB_OK;
+  if (!m->gp_totals) NVB_CUDA(cudaMalloc(&m->gp_totals, 2 * sizeof(int)));
+  NVB_CUDA(launchGroundSortBlocks(m->tsdf, hw, m->gp_keys, m->gp_slots, m->gp_sort_temp, m->gp_sort_temp_bytes, m->stream));
+  m->launches += 2;
+  GroundExtractArgs a{};
+  a.tsdf = m->tsdf;
+  a.slots = m->gp_slots + hw, a.num_blocks = hw;
+  a.counts = m->gp_counts, a.totals = m->gp_totals;
+  a.block_size = m->block_size, a.voxel_size = m->voxel_size;
+  a.min_tsdf_weight = m->gp.min_tsdf_weight;
+  a.min_z = m->gp.ground_points_candidates_min_z_m, a.max_z = m->gp.ground_points_candidates_max_z_m;
+  launchGroundCount(a, m->stream);
+  m->launches += 2;
+  int totals[2];
+  NVB_CUDA(cudaMemcpyAsync(totals, m->gp_totals, sizeof(totals), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  // "Maximum number of crossings reached." (tsdf_zero_crossings_extractor.cu:126-131)
+  if (totals[0] >= m->gp.max_crossings) return checkDeviceError(m);
+  if ((rc = ensureDevice(&m->gp_crossings, &m->gp_crossings_cap, std::max(totals[0], 1)))) return rc;
+  if ((rc = ensureDevice(&m->gp_candidates, &m->gp_candidates_cap, std::max(totals[1], 1)))) return rc;
+  a.crossings = m->gp_crossings, a.candidates = m->gp_candidates;
+  launchGroundEmit(a, m->stream);
+  m->launches++;
+  m->gp_valid = true;
+  m->gp_num_crossings = totals[0], m->gp_num_candidates = totals[1];
+  int f = 0;
+  float pl[4];
+  if ((rc = ransacFit(m, m->gp_candidates, totals[1], m->gp.num_ransac_iterations, m->gp.ransac_distance_threshold_m, pl, &f))) {
+    groundReset(m);
+    return rc;
+  }
+  if (!f) {
+    groundReset(m);
+    return checkDeviceError(m);
+  }
+  m->gp_found = true;
+  std::memcpy(m->gp_plane, pl, sizeof(pl));
+  if (plane) std::memcpy(plane, pl, sizeof(pl));
+  *found = 1;
+  return checkDeviceError(m);
+}
+
+int32_t nvb_mapper_ground_plane(NvbMapper* m, float plane[4], int32_t* found) {
+  if (!m || !found) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  *found = m->gp_found ? 1 : 0;
+  if (m->gp_found && plane) std::memcpy(plane, m->gp_plane, sizeof(m->gp_plane));
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_ground_plane_points(NvbMapper* m, int32_t which, float* xyz, int32_t cap, int32_t* n, int32_t* valid) {
+  if (!m || !n || !valid) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (which != NVB_GROUND_POINTS_CROSSINGS && which != NVB_GROUND_POINTS_CANDIDATES)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "which must be NVB_GROUND_POINTS_CROSSINGS or NVB_GROUND_POINTS_CANDIDATES");
+  *valid = m->gp_valid ? 1 : 0;
+  *n = 0;
+  if (!m->gp_valid) return NVB_OK;
+  *n = which == NVB_GROUND_POINTS_CROSSINGS ? m->gp_num_crossings : m->gp_num_candidates;
+  const int k = std::min(*n, std::max(cap, 0));
+  if (!xyz || k == 0) return NVB_OK;
+  NVB_CUDA(cudaSetDevice(m->device));
+  if (which == NVB_GROUND_POINTS_CROSSINGS) {
+    NVB_CUDA(cudaMemcpyAsync(xyz, m->gp_crossings, (size_t)k * sizeof(float3), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+  } else {
+    std::vector<float4> c((size_t)k);
+    NVB_CUDA(cudaMemcpyAsync(c.data(), m->gp_candidates, (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int i = 0; i < k; i++) xyz[3 * i] = c[i].x, xyz[3 * i + 1] = c[i].y, xyz[3 * i + 2] = c[i].z;
+  }
+  return NVB_OK;
+}
+
+int32_t nvb_ransac_fit_plane(NvbMapper* m, const float* points, int32_t memory, int32_t n, int32_t num_ransac_iterations,
+                             float ransac_distance_threshold_m, float plane[4], int32_t* found) {
+  if (!m || !plane || !found) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (n < 0 || (n > 0 && !points)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad point list");
+  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (num_ransac_iterations < 1) return fail(NVB_ERR_INVALID_ARGUMENT, "num_ransac_iterations must be >= 1");
+  *found = 0;
+  if (n < 3) return NVB_OK;
+  NVB_CUDA(cudaSetDevice(m->device));
+  int rc = ensureDevice(&m->gp_fit_points, &m->gp_fit_points_cap, n);
+  if (rc) return rc;
+  const float* src = points;
+  if (memory == NVB_MEM_HOST) {
+    // staged on the device for the packing kernel, in a buffer kept by the mapper
+    if ((rc = ensureDevice(&m->gp_fit_stage, &m->gp_fit_stage_cap, 3ll * n))) return rc;
+    NVB_CUDA(cudaMemcpyAsync(m->gp_fit_stage, points, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    src = m->gp_fit_stage;
+  }
+  launchPackPoints(src, n, m->gp_fit_points, m->stream);
+  m->launches++;
+  int f = 0;
+  if ((rc = ransacFit(m, m->gp_fit_points, n, num_ransac_iterations, ransac_distance_threshold_m, plane, &f))) return rc;
+  *found = f;
+  return checkDeviceError(m);
 }
 
 int32_t nvb_esdf_slice_aabb(NvbMapper* m, float slice_height_m, float aabb_out[6], int32_t* empty_out) {

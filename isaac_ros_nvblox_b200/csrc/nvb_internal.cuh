@@ -638,4 +638,30 @@ struct ShapeClearArgs {
 void launchShapeSelect(const ShapeClearArgs& a, cudaStream_t stream);
 void launchShapeClear(const ShapeClearArgs& a, int num_sms, cudaStream_t stream);
 
+// nvb_ground.cu: the ground-plane estimator (GroundPlaneEstimator, src/experimental/ground_plane/)
+struct GroundExtractArgs {
+  DevLayer tsdf;
+  const int* slots;   // the TSDF slots below the high-water mark in (x, y, z) block-index order, free slots (-1) last
+  int num_blocks;
+  int2* counts;       // per listed block: {crossings, candidates}, then their exclusive prefix sums
+  int* totals;        // 2 ints: all crossings, all candidates
+  float3* crossings;  // emit: the crossings, in list order then voxel (x, y, z) order
+  float4* candidates; // emit: the crossings with min_z <= z <= max_z (finite), {x, y, z, 0}, same order
+  float block_size, voxel_size, min_tsdf_weight, min_z, max_z;
+};
+// keys[0, hw) / slots[0, hw): the slots below the high-water mark with their packIndex keys; sorted into keys[hw, 2 hw)
+// / slots[hw, 2 hw) (a stable radix sort, cub). temp: groundSortTempBytes(hw) bytes.
+size_t groundSortTempBytes(int n);
+cudaError_t launchGroundSortBlocks(const DevLayer& tsdf, int hw, unsigned long long* keys, int* slots, void* temp,
+                                   size_t temp_bytes, cudaStream_t stream);
+void launchGroundCount(const GroundExtractArgs& a, cudaStream_t stream);  // counts + scan + totals
+void launchGroundEmit(const GroundExtractArgs& a, cudaStream_t stream);
+void launchPackPoints(const float* xyz, int n, float4* out, cudaStream_t stream);
+size_t ransacStateBytes();  // one XORWOW state
+// curand_init(1234, i, 0) for the iterations first <= i < n
+void launchRansacInit(void* states, int first, int n, cudaStream_t stream);
+// MSAC over n >= 1 points (float4, w unused) -> out5 = {nx, ny, nz, d, found (int)}
+void launchRansacFit(const float4* pts, int n, int iterations, float threshold, const void* states, float* costs,
+                     float4* planes, float* out5, bool reference_shape, cudaStream_t stream);
+
 }  // namespace nvb

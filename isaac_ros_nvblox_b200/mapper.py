@@ -18,7 +18,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (NvbBoundingShape, NvbCamera, NvbDecayExclusion, NvbEsdfParams, NvbEsdfSliceParams, NvbFreespaceParams, NvbMapperOptions, NvbOccupancyDecayParams,
+from ._lib import (NvbBoundingShape, NvbCamera, NvbDecayExclusion, NvbEsdfParams, NvbEsdfSliceParams, NvbFreespaceParams, NvbGroundPlaneParams, NvbMapperOptions, NvbOccupancyDecayParams,
                    NvbOccupancyParams, NvbTsdfDecayParams, NvbTsdfParams, check)
 
 TSDF_VOXEL_DTYPE = np.dtype([("distance", "<f4"), ("weight", "<f4")])
@@ -599,6 +599,92 @@ class EsdfSlicer:
         return aabb, img, grid
 
 
+def _plane_or_none(fn, *args):
+    pl = (C.c_float * 4)()
+    found = C.c_int32(0)
+    check(fn(*args, pl, C.byref(found)))
+    return tuple(float(v) for v in pl) if found.value else None
+
+
+class GroundPlaneEstimator:
+    """GroundPlaneEstimator (experimental/ground_plane/ground_plane_estimator.h) of one mapper: the TSDF zero crossings from
+    above, the ground candidates among them (min_z <= z <= max_z) and their MSAC plane. Planes are (nx, ny, nz, d) with
+    n . p + d = 0; point lists are (n, 3) float32 in block-index (x, y, z) order, then voxel (x, y, z) order."""
+
+    def __init__(self, mapper):
+        self._m = mapper
+
+    def params(self, **kw):
+        """Sets the given fields of NvbGroundPlaneParams (ground_points_candidates_min_z_m / max_z_m,
+        ransac_distance_threshold_m, num_ransac_iterations, min_tsdf_weight, max_crossings); returns them all as a dict."""
+        p = NvbGroundPlaneParams()
+        check(self._m._L.nvb_mapper_get_ground_plane_params(self._m._h, C.byref(p)))
+        for k, v in kw.items():
+            if k not in dict(p._fields_):
+                raise TypeError("unknown ground-plane parameter %r" % k)
+            setattr(p, k, v)
+        if kw:
+            check(self._m._L.nvb_mapper_set_ground_plane_params(self._m._h, C.byref(p)))
+        return {k: getattr(p, k) for k, _ in p._fields_}
+
+    def compute_ground_plane(self):
+        """computeGroundPlane(tsdf_layer): the plane, or None (the last crossings, candidates and plane are then cleared)."""
+        return _plane_or_none(self._m._L.nvb_mapper_compute_ground_plane, self._m._h)
+
+    def ground_plane(self):
+        return _plane_or_none(self._m._L.nvb_mapper_ground_plane, self._m._h)
+
+    def _points(self, which):
+        L, h = self._m._L, self._m._h
+        n, valid = C.c_int32(0), C.c_int32(0)
+        check(L.nvb_mapper_ground_plane_points(h, which, None, 0, C.byref(n), C.byref(valid)))
+        if not valid.value:
+            return None
+        out = np.zeros((n.value, 3), dtype=np.float32)
+        if n.value:
+            check(L.nvb_mapper_ground_plane_points(h, which, _fp(out), n.value, C.byref(n), C.byref(valid)))
+        return out
+
+    def tsdf_zero_crossings(self):
+        return self._points(_lib.NVB_GROUND_POINTS_CROSSINGS)
+
+    def tsdf_zero_crossings_ground_candidates(self):
+        return self._points(_lib.NVB_GROUND_POINTS_CANDIDATES)
+
+
+_fit_mappers = {}
+
+
+def ransac_fit_plane(points, num_ransac_iterations=1000, ransac_distance_threshold_m=0.2, mapper=None, device=0):
+    """RansacPlaneFitter::fit (experimental/ground_plane/ransac_plane_fitter.h), MSAC on the GPU: (nx, ny, nz, d) or None.
+    `points` is an (n, 3) float32 array (host) or a CUDA tensor (device). Runs on `mapper`'s device and stream; without one,
+    on a small mapper kept per device."""
+    if mapper is None:
+        mapper = _fit_mappers.get(device)
+        if mapper is None:
+            mapper = _fit_mappers[device] = Mapper(0.05, device=device, tsdf_capacity_blocks=64, esdf_capacity_blocks=64)
+    if hasattr(points, "data_ptr"):  # a CUDA tensor
+        import torch
+        if not points.is_cuda:
+            raise ValueError("a tensor of points must be on the GPU")
+        if points.device.index != mapper._device:
+            raise ValueError("the points are on cuda:%d, the mapper on cuda:%d" % (points.device.index, mapper._device))
+        t = points.detach().float().contiguous().reshape(-1, 3)
+        # The mapper's stream does not wait for torch's: order this call after the producer of the points and after the
+        # conversion / copy above, both enqueued on torch's current stream.
+        torch.cuda.current_stream(t.device).synchronize()
+        ptr, n, mem, keep = t.data_ptr(), t.shape[0], _lib.NVB_MEM_DEVICE, t
+    else:
+        a = np.ascontiguousarray(points, dtype=np.float32).reshape(-1, 3)
+        ptr, n, mem, keep = a.ctypes.data, a.shape[0], _lib.NVB_MEM_HOST, a
+    pl = (C.c_float * 4)()
+    found = C.c_int32(0)
+    check(mapper._L.nvb_ransac_fit_plane(mapper._h, C.c_void_p(ptr), mem, int(n), int(num_ransac_iterations),
+                                          float(ransac_distance_threshold_m), pl, C.byref(found)))
+    del keep
+    return tuple(float(v) for v in pl) if found.value else None
+
+
 class Mapper:
     """nvblox::Mapper(voxel_size_m, projective_layer_type) with a projective (TSDF or occupancy) and an ESDF layer."""
 
@@ -621,6 +707,7 @@ class Mapper:
         self._L.nvb_default_mapper_options(C.byref(o))
         o.voxel_size_m = float(voxel_size_m)
         o.device = int(device)
+        self._device = int(device)
         if tsdf_capacity_blocks:
             o.tsdf_capacity_blocks = int(tsdf_capacity_blocks)
         if esdf_capacity_blocks:
@@ -659,6 +746,10 @@ class Mapper:
 
     def tsdf_layer(self):
         return self._tsdf
+
+    def ground_plane_estimator(self):
+        """MultiMapper::ground_plane_estimator() of this mapper (its state lives in the mapper)."""
+        return GroundPlaneEstimator(self)
 
     def occupancy_layer(self):
         return self._occupancy
