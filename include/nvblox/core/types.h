@@ -21,6 +21,7 @@ using Index2D = Eigen::Vector2i;
 using Vector3f = Eigen::Vector3f;
 using Vector2f = Eigen::Vector2f;
 using Transform = Eigen::Isometry3f;
+using Matrix3Xf = Eigen::Matrix3Xf;
 }  // namespace nvblox
 #else
 namespace nvblox {
@@ -77,6 +78,20 @@ struct Transform {
     for (int i = 0; i < 3; i++) o.m[12 + i] = -(o(i, 0) * m[12] + (o(i, 1) * m[13] + o(i, 2) * m[14]));
     return o;
   }
+};
+
+// Eigen::Matrix3Xf stand-in (DynamicsDetection::getDynamicPointsHost): 3 x cols, column-major.
+struct Matrix3Xf {
+  std::vector<float> m;
+  Matrix3Xf() = default;
+  Matrix3Xf(int rows, int cols) : m((size_t)3 * cols) { (void)rows; }
+  int rows() const { return 3; }
+  int cols() const { return (int)(m.size() / 3); }
+  float& operator()(int r, int c) { return m[(size_t)c * 3 + r]; }
+  const float& operator()(int r, int c) const { return m[(size_t)c * 3 + r]; }
+  Vector3f col(int c) const { return Vector3f(m[(size_t)c * 3], m[(size_t)c * 3 + 1], m[(size_t)c * 3 + 2]); }
+  float* data() { return m.data(); }
+  const float* data() const { return m.data(); }
 };
 }  // namespace nvblox
 #endif

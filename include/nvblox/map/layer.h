@@ -60,6 +60,8 @@ class VoxelBlockLayer {
     *out = b->voxels[voxel_idx[0]][voxel_idx[1]][voxel_idx[2]];
     return true;
   }
+ // The mapper this layer belongs to (DynamicsDetection::computeDynamics runs on the owner of its FreespaceLayer).
+  NvbMapper* c_abi() const { return m_; }
  private:
   NvbMapper* m_;
   int id_;

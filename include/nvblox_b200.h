@@ -490,6 +490,51 @@ NVB_API int32_t nvb_mapper_ground_plane_points(NvbMapper* m, int32_t which, floa
 NVB_API int32_t nvb_ransac_fit_plane(NvbMapper* m, const float* points, int32_t memory, int32_t n, int32_t num_ransac_iterations,
                                      float ransac_distance_threshold_m, float plane[4], int32_t* found);
 
+/* DynamicsDetection::computeDynamics(depth, freespace_layer, camera, T_L_C) (C/include/nvblox/dynamics/dynamics_detection.h,
+ * dynamics/internal/cuda/impl/dynamics_detection_impl.cuh:26-130) on the freespace layer of a
+ * NVB_PROJECTIVE_TSDF_WITH_FREESPACE mapper (NVB_ERR_INVALID_ARGUMENT on any other), as that layer stands. A pixel with
+ * depth > 0 (NaN included) whose point T_L_C * unproject(pixel, depth) falls into an allocated freespace voxel that is
+ * high-confidence freespace is dynamic: mask 255 and overlay (255, s, s), s = min(25.5 * depth, 255); other looked-up
+ * pixels get mask 0 and (0, s, s); the rest mask 0 and white. The dynamic points come in row-major pixel order (the
+ * reference's order is an atomicAdd race). Host depth is staged in a buffer the mapper keeps. The call is enqueued on
+ * the mapper's stream without a host synchronisation; the point count stays on the device until a getter asks. */
+NVB_API int32_t nvb_mapper_compute_dynamics(NvbMapper* m, const float* depth, int32_t memory, int32_t rows, int32_t cols,
+                                            const float* T_L_C, const NvbCamera* cam);
+/* MaskPreprocessor::removeSmallConnectedComponents(mask_in, threshold, mask_out) (C/src/sensors/mask_preprocessor.cpp:
+ * 140-183): threshold <= 0 copies the mask. Otherwise the mask is downscaled by 2 (pixel (2r, 2c)), its pixels > 0 are
+ * labelled into 4-connected components, components of fewer than threshold / 4 (integer division) downscaled pixels are
+ * erased, survivors hold 254, and the result is upscaled by 2. Unlike the reference, whose output shrinks to
+ * (rows / 2) * 2 x (cols / 2) * 2, mask_out keeps the input's size: a trailing odd row or column is 0. Both masks are
+ * rows x cols bytes in `memory`; they may be the same buffer. Runs on the mapper's stream with its scratch; with device
+ * masks it does not synchronise, with host masks it returns when mask_out is written. */
+NVB_API int32_t nvb_mapper_remove_small_components(NvbMapper* m, const uint8_t* mask_in, uint8_t* mask_out, int32_t memory,
+                                                   int32_t rows, int32_t cols, int32_t threshold);
+/* DynamicsDetection::getDynamicMaskImage / getDynamicOverlayImage of the last nvb_mapper_compute_dynamics: *rows, *cols of
+ * the frame (0 x 0 before the first call); out (rows x cols bytes, resp. x 3 for the RGB overlay, in `memory`) may be NULL.
+ * A host copy synchronises the mapper's stream; a device copy is enqueued on it. */
+NVB_API int32_t nvb_mapper_dynamic_mask(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols);
+NVB_API int32_t nvb_mapper_dynamic_overlay(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols);
+/* DynamicsDetection::getDynamicPointsHost / getDynamicPointcloudDevice: *out_count = the number of dynamic points of the
+ * last frame (read back here: this synchronises the mapper's stream), and the first min(count, cap) of them (x, y, z
+ * floats) are copied to xyz (in `memory`; may be NULL). */
+NVB_API int32_t nvb_mapper_dynamic_points(NvbMapper* m, float* xyz, int32_t memory, int32_t cap, int32_t* out_count);
+/* The detector's device buffers, for a consumer on another stream (a second mapper, through nvb_mapper_wait_for). They
+ * stay valid, and their contents unchanged, until the next nvb_mapper_compute_dynamics on this mapper or its destruction.
+ * cleaned_mask is a rows x cols buffer kept for nvb_mapper_remove_small_components' output. */
+typedef struct {
+  const float* depth;           /* the last frame's depth, staged on the device */
+  const uint8_t* mask;          /* the dynamic mask */
+  uint8_t* cleaned_mask;        /* scratch of the same size, for the filtered mask */
+  const uint8_t* overlay;       /* RGB */
+  const float* points;          /* x, y, z per dynamic point */
+  const int32_t* num_points;    /* device */
+  int32_t rows, cols;
+} NvbDynamicsBuffers;
+NVB_API int32_t nvb_mapper_dynamics_device_buffers(NvbMapper* m, NvbDynamicsBuffers* out);
+/* Device-side ordering between two mappers: work enqueued on waiter's stream after this call runs after everything
+ * enqueued so far on producer's stream. No host synchronisation. */
+NVB_API int32_t nvb_mapper_wait_for(NvbMapper* waiter, NvbMapper* producer);
+
 /* EsdfSlicer::sliceLayerToDistanceImage (C/include/nvblox/integrators/esdf_slicer.h:52-78, C/src/integrators/esdf_slicer.cu:
  * 25-67,112-215) and, if grid_host != NULL, EsdfSlicer::occupancyGridFromSliceImage (:78-110,254-300) of the ESDF layer
  * (3-D or 2-D) at slice_height_m: one pixel per voxel over the AABB of the ESDF blocks at that height, rows along y,

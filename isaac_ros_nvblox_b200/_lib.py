@@ -47,6 +47,8 @@ EXPORTED_SYMBOLS = [
     "nvb_mapper_get_cleared_blocks",
     "nvb_default_ground_plane_params", "nvb_mapper_set_ground_plane_params", "nvb_mapper_get_ground_plane_params",
     "nvb_mapper_compute_ground_plane", "nvb_mapper_ground_plane", "nvb_mapper_ground_plane_points", "nvb_ransac_fit_plane",
+    "nvb_mapper_compute_dynamics", "nvb_mapper_remove_small_components", "nvb_mapper_dynamic_mask", "nvb_mapper_dynamic_overlay",
+    "nvb_mapper_dynamic_points", "nvb_mapper_dynamics_device_buffers", "nvb_mapper_wait_for",
 ]
 
 
@@ -139,6 +141,11 @@ class NvbGroundPlaneParams(C.Structure):
     _fields_ = [("ground_points_candidates_min_z_m", C.c_float), ("ground_points_candidates_max_z_m", C.c_float),
                 ("ransac_distance_threshold_m", C.c_float), ("num_ransac_iterations", C.c_int32),
                 ("min_tsdf_weight", C.c_float), ("max_crossings", C.c_int32)]
+
+
+class NvbDynamicsBuffers(C.Structure):
+    _fields_ = [("depth", C.c_void_p), ("mask", C.c_void_p), ("cleaned_mask", C.c_void_p), ("overlay", C.c_void_p),
+                ("points", C.c_void_p), ("num_points", C.c_void_p), ("rows", C.c_int32), ("cols", C.c_int32)]
 
 
 class NvbMapperOptions(C.Structure):
@@ -292,6 +299,13 @@ def load(path=None):
     L.nvb_mapper_ground_plane.argtypes = [vp, fp, ip]
     L.nvb_mapper_ground_plane_points.argtypes = [vp, i32, fp, i32, ip, ip]
     L.nvb_ransac_fit_plane.argtypes = [vp, vp, i32, i32, i32, f32, fp, ip]
+    L.nvb_mapper_compute_dynamics.argtypes = [vp, vp, i32, i32, i32, fp, C.POINTER(NvbCamera)]
+    L.nvb_mapper_remove_small_components.argtypes = [vp, vp, vp, i32, i32, i32, i32]
+    L.nvb_mapper_dynamic_mask.argtypes = [vp, vp, i32, ip, ip]
+    L.nvb_mapper_dynamic_overlay.argtypes = [vp, vp, i32, ip, ip]
+    L.nvb_mapper_dynamic_points.argtypes = [vp, vp, i32, i32, ip]
+    L.nvb_mapper_dynamics_device_buffers.argtypes = [vp, C.POINTER(NvbDynamicsBuffers)]
+    L.nvb_mapper_wait_for.argtypes = [vp, vp]
     L.nvb_mapper_kernel_launches.restype = C.c_int64
     for name in EXPORTED_SYMBOLS:
         f = getattr(L, name)

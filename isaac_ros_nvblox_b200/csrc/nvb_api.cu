@@ -236,6 +236,23 @@ struct NvbMapper {
   int gp_num_crossings = 0, gp_num_candidates = 0;
   bool gp_found = false;
   float gp_plane[4] = {0, 0, 0, 0};
+  // dynamics detection (nvb_dynamics.cu): the last frame's outputs, sized by pixels; the filter's scratch
+  float* dyn_depth = nullptr;      // staged depth
+  unsigned char* dyn_mask = nullptr;
+  unsigned char* dyn_clean = nullptr;
+  unsigned char* dyn_overlay = nullptr;
+  float* dyn_points = nullptr;
+  int dyn_pixels_cap = 0;
+  int2* dyn_counts = nullptr;
+  int dyn_tiles_cap = 0;
+  int* dyn_totals = nullptr;       // {points, 0}
+  int dyn_rows = 0, dyn_cols = 0;
+  int* cc_labels = nullptr;
+  int* cc_sizes = nullptr;
+  int cc_cap = 0;
+  unsigned char* cc_stage = nullptr;  // host masks staged for the filter (input, then output)
+  int cc_stage_cap = 0;
+  cudaEvent_t dyn_event = nullptr;    // nvb_mapper_wait_for: recorded on this mapper's stream
   // last integrated view (Mapper::last_posed_depth_image_, mapper.h:830-833), kept when keep_last_view is set
   int keep_last_view = 0;
   float* last_depth = nullptr;
@@ -1373,6 +1390,9 @@ void nvb_mapper_destroy(NvbMapper* m) {
   cudaFree(m->gp_slots), cudaFree(m->gp_counts), cudaFree(m->gp_totals), cudaFree(m->gp_crossings), cudaFree(m->gp_candidates);
   cudaFree(m->gp_fit_points), cudaFree(m->gp_states), cudaFree(m->gp_costs), cudaFree(m->gp_planes), cudaFree(m->gp_result);
   cudaFree(m->pre_depth);
+  cudaFree(m->dyn_depth), cudaFree(m->dyn_mask), cudaFree(m->dyn_clean), cudaFree(m->dyn_overlay), cudaFree(m->dyn_points);
+  cudaFree(m->dyn_counts), cudaFree(m->dyn_totals), cudaFree(m->cc_labels), cudaFree(m->cc_sizes), cudaFree(m->cc_stage);
+  if (m->dyn_event) cudaEventDestroy(m->dyn_event);
   cudaFree(m->union_list), cudaFree(m->union_list_count);
   if (m->mesh.blocks) freeLayer(&m->mesh);
   cudaFree(m->mesh_v), cudaFree(m->mesh_n), cudaFree(m->mesh_t), cudaFree(m->mesh_c), cudaFree(m->mesh_state);
@@ -2703,6 +2723,185 @@ int32_t nvb_ransac_fit_plane(NvbMapper* m, const float* points, int32_t memory, 
   if ((rc = ransacFit(m, m->gp_fit_points, n, num_ransac_iterations, ransac_distance_threshold_m, plane, &f))) return rc;
   *found = f;
   return checkDeviceError(m);
+}
+
+}  // extern "C"
+
+namespace {
+constexpr long long kMaxDynamicsPixels = 1ll << 28;  // 3-byte overlay and 12-byte points per pixel stay below 2^32
+
+// Grows the detector's per-pixel buffers (nothing is kept: the next call rewrites them). Growing synchronises first, so
+// that no pending kernel, and no consumer ordered behind this stream, still reads the old buffers.
+int ensureDynamicsBuffers(NvbMapper* m, int pixels) {
+  const int tiles = dynamicsNumTiles(pixels);
+  if (pixels > m->dyn_pixels_cap) {
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+    cudaFree(m->dyn_depth), cudaFree(m->dyn_mask), cudaFree(m->dyn_clean), cudaFree(m->dyn_overlay), cudaFree(m->dyn_points);
+    m->dyn_depth = nullptr, m->dyn_mask = m->dyn_clean = m->dyn_overlay = nullptr, m->dyn_points = nullptr;
+    m->dyn_pixels_cap = 0;
+    NVB_CUDA(cudaMalloc(&m->dyn_depth, (size_t)pixels * sizeof(float)));
+    NVB_CUDA(cudaMalloc(&m->dyn_mask, (size_t)pixels));
+    NVB_CUDA(cudaMalloc(&m->dyn_clean, (size_t)pixels));
+    NVB_CUDA(cudaMalloc(&m->dyn_overlay, (size_t)pixels * 3));
+    NVB_CUDA(cudaMalloc(&m->dyn_points, (size_t)pixels * 3 * sizeof(float)));
+    m->dyn_pixels_cap = pixels;
+  }
+  if (tiles > m->dyn_tiles_cap) {
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+    cudaFree(m->dyn_counts);
+    m->dyn_counts = nullptr, m->dyn_tiles_cap = 0;
+    NVB_CUDA(cudaMalloc(&m->dyn_counts, (size_t)tiles * sizeof(int2)));
+    m->dyn_tiles_cap = tiles;
+  }
+  if (!m->dyn_totals) {
+    NVB_CUDA(cudaMalloc(&m->dyn_totals, 2 * sizeof(int)));
+    NVB_CUDA(cudaMemsetAsync(m->dyn_totals, 0, 2 * sizeof(int), m->stream));
+  }
+  return NVB_OK;
+}
+
+int validMemory(int32_t memory) { return memory == NVB_MEM_HOST || memory == NVB_MEM_DEVICE; }
+
+// Copies `bytes` of a detector output to the caller's buffer; a host copy waits for it.
+int copyDynamicsOut(NvbMapper* m, void* out, const void* src, size_t bytes, int32_t memory) {
+  if (!out || bytes == 0 || !src) return NVB_OK;
+  NVB_CUDA(cudaMemcpyAsync(out, src, bytes, memory == NVB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, m->stream));
+  if (memory == NVB_MEM_HOST) NVB_CUDA(cudaStreamSynchronize(m->stream));
+  return NVB_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int32_t nvb_mapper_compute_dynamics(NvbMapper* m, const float* depth, int32_t memory, int32_t rows, int32_t cols,
+                                    const float* T_L_C, const NvbCamera* cam) {
+  int rc = validateFrameArgs(m, depth, rows, cols, T_L_C, cam);
+  if (rc) return rc;
+  if (m->projective_layer_type != NVB_PROJECTIVE_TSDF_WITH_FREESPACE)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper has no freespace layer");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if ((long long)rows * cols > kMaxDynamicsPixels) return fail(NVB_ERR_INVALID_ARGUMENT, "depth image too large");
+  NVB_CUDA(cudaSetDevice(m->device));
+  const int pixels = rows * cols;
+  if ((rc = ensureDynamicsBuffers(m, pixels))) return rc;
+  // The freespace layer is written on `stream` only (nvb_mapper_update_freespace); the detection follows it there.
+  NVB_CUDA(cudaMemcpyAsync(m->dyn_depth, depth, (size_t)pixels * sizeof(float),
+                           memory == NVB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, m->stream));
+  DynamicsArgs a{};
+  a.depth = m->dyn_depth, a.rows = rows, a.cols = cols;
+  a.T_L_C = rigidFromColMajor(T_L_C);
+  a.cam = *cam;
+  a.fs = m->freespace;
+  a.block_size = m->block_size;
+  a.voxel_size_inv = (float)(1.0 / (double)(m->block_size * (1.0f / kVps)));  // 1.0 / blockSizeToVoxelSize(block_size)
+  a.mask = m->dyn_mask, a.overlay = m->dyn_overlay, a.counts = m->dyn_counts, a.points = m->dyn_points;
+  launchDynamicsDetect(a, m->dyn_totals, m->stream);
+  m->launches += 3;
+  m->dyn_rows = rows, m->dyn_cols = cols;
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_remove_small_components(NvbMapper* m, const uint8_t* mask_in, uint8_t* mask_out, int32_t memory,
+                                           int32_t rows, int32_t cols, int32_t threshold) {
+  if (!m || !mask_in || !mask_out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (rows <= 0 || cols <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "mask must have positive size");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if ((long long)rows * cols > kMaxDynamicsPixels) return fail(NVB_ERR_INVALID_ARGUMENT, "mask too large");
+  const int pixels = rows * cols;
+  if (threshold <= 0) {  // "Simply copy the output if threshold is zero."
+    if (memory == NVB_MEM_HOST) {
+      if (mask_out != mask_in) std::memmove(mask_out, mask_in, (size_t)pixels);
+      return NVB_OK;
+    }
+    NVB_CUDA(cudaSetDevice(m->device));
+    if (mask_out != mask_in)
+      NVB_CUDA(cudaMemcpyAsync(mask_out, mask_in, (size_t)pixels, cudaMemcpyDeviceToDevice, m->stream));
+    return NVB_OK;
+  }
+  NVB_CUDA(cudaSetDevice(m->device));
+  CcArgs a{};
+  a.rows = rows, a.cols = cols, a.drows = rows / 2, a.dcols = cols / 2;
+  a.min_size = threshold / 4;  // size_threshold / (kDownScaleFactor * kDownScaleFactor)
+  const int down = std::max(a.drows * a.dcols, 1);
+  if (down > m->cc_cap) {
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+    cudaFree(m->cc_labels), cudaFree(m->cc_sizes);
+    m->cc_labels = m->cc_sizes = nullptr, m->cc_cap = 0;
+    const int cap = std::max(down, 2 * m->cc_cap);
+    NVB_CUDA(cudaMalloc(&m->cc_labels, (size_t)cap * sizeof(int)));
+    NVB_CUDA(cudaMalloc(&m->cc_sizes, (size_t)cap * sizeof(int)));
+    m->cc_cap = cap;
+  }
+  a.labels = m->cc_labels, a.sizes = m->cc_sizes;
+  if (memory == NVB_MEM_HOST) {
+    if (pixels > m->cc_stage_cap) {
+      NVB_CUDA(cudaStreamSynchronize(m->stream));
+      cudaFree(m->cc_stage);
+      m->cc_stage = nullptr, m->cc_stage_cap = 0;
+      NVB_CUDA(cudaMalloc(&m->cc_stage, (size_t)pixels));
+      m->cc_stage_cap = pixels;
+    }
+    NVB_CUDA(cudaMemcpyAsync(m->cc_stage, mask_in, (size_t)pixels, cudaMemcpyHostToDevice, m->stream));
+    a.in = m->cc_stage, a.out = m->cc_stage;
+  } else {
+    a.in = mask_in, a.out = mask_out;
+  }
+  launchRemoveSmallComponents(a, m->num_sms, m->stream);
+  m->launches += a.drows > 0 && a.dcols > 0 ? 4 : 1;
+  if (memory == NVB_MEM_HOST) {
+    NVB_CUDA(cudaMemcpyAsync(mask_out, m->cc_stage, (size_t)pixels, cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+  }
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_dynamic_mask(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols) {
+  if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  *rows = m->dyn_rows, *cols = m->dyn_cols;
+  NVB_CUDA(cudaSetDevice(m->device));
+  return copyDynamicsOut(m, out, m->dyn_mask, (size_t)m->dyn_rows * m->dyn_cols, memory);
+}
+
+int32_t nvb_mapper_dynamic_overlay(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols) {
+  if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  *rows = m->dyn_rows, *cols = m->dyn_cols;
+  NVB_CUDA(cudaSetDevice(m->device));
+  return copyDynamicsOut(m, out, m->dyn_overlay, (size_t)m->dyn_rows * m->dyn_cols * 3, memory);
+}
+
+int32_t nvb_mapper_dynamic_points(NvbMapper* m, float* xyz, int32_t memory, int32_t cap, int32_t* out_count) {
+  if (!m || !out_count) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  *out_count = 0;
+  if (!m->dyn_totals) return NVB_OK;  // never computed
+  NVB_CUDA(cudaSetDevice(m->device));
+  int n = 0;
+  NVB_CUDA(cudaMemcpyAsync(&n, m->dyn_totals, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  *out_count = n;
+  const int k = std::min(n, std::max(cap, 0));
+  return copyDynamicsOut(m, xyz, m->dyn_points, (size_t)k * 3 * sizeof(float), memory);
+}
+
+int32_t nvb_mapper_dynamics_device_buffers(NvbMapper* m, NvbDynamicsBuffers* out) {
+  if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  out->depth = m->dyn_depth, out->mask = m->dyn_mask, out->cleaned_mask = m->dyn_clean, out->overlay = m->dyn_overlay;
+  out->points = m->dyn_points, out->num_points = m->dyn_totals;
+  out->rows = m->dyn_rows, out->cols = m->dyn_cols;
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_wait_for(NvbMapper* waiter, NvbMapper* producer) {
+  if (!waiter || !producer) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (waiter == producer) return NVB_OK;  // one stream: already ordered
+  NVB_CUDA(cudaSetDevice(producer->device));
+  if (!producer->dyn_event) NVB_CUDA(cudaEventCreateWithFlags(&producer->dyn_event, cudaEventDisableTiming));
+  NVB_CUDA(cudaEventRecord(producer->dyn_event, producer->stream));
+  NVB_CUDA(cudaSetDevice(waiter->device));
+  NVB_CUDA(cudaStreamWaitEvent(waiter->stream, producer->dyn_event, 0));
+  return NVB_OK;
 }
 
 int32_t nvb_esdf_slice_aabb(NvbMapper* m, float slice_height_m, float aabb_out[6], int32_t* empty_out) {

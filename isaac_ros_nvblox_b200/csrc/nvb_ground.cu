@@ -91,16 +91,16 @@ __global__ void __launch_bounds__(kPairThreads) groundCountKernel(GroundExtractA
   if (threadIdx.x == 0) a.counts[blockIdx.x] = make_int2(n_hit, n_cand);
 }
 
-// Exclusive scan of the per-block counts in place (one CTA); totals -> a.totals[0..1].
-__global__ void __launch_bounds__(kScanThreads) groundScanKernel(GroundExtractArgs a) {
+// Exclusive scan of n int2 counts in place (one CTA); totals -> totals[0..1]. Shared with nvb_dynamics.cu.
+__global__ void __launch_bounds__(kScanThreads) exclusiveScanInt2Kernel(int2* counts, int n, int* totals) {
   __shared__ int2 s_warp[kScanThreads / 32];
   __shared__ int2 s_carry;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (threadIdx.x == 0) s_carry = make_int2(0, 0);
   __syncthreads();
-  for (int base = 0; base < a.num_blocks; base += kScanThreads) {
+  for (int base = 0; base < n; base += kScanThreads) {
     const int i = base + threadIdx.x;
-    const int2 c = i < a.num_blocks ? a.counts[i] : make_int2(0, 0);
+    const int2 c = i < n ? counts[i] : make_int2(0, 0);
     int2 incl = c;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
@@ -121,12 +121,12 @@ __global__ void __launch_bounds__(kScanThreads) groundScanKernel(GroundExtractAr
     }
     __syncthreads();
     const int2 carry = s_carry, wo = s_warp[warp];
-    if (i < a.num_blocks) a.counts[i] = make_int2(carry.x + wo.x + incl.x - c.x, carry.y + wo.y + incl.y - c.y);
+    if (i < n) counts[i] = make_int2(carry.x + wo.x + incl.x - c.x, carry.y + wo.y + incl.y - c.y);
     __syncthreads();
     if (threadIdx.x == kScanThreads - 1) s_carry = make_int2(carry.x + wo.x + incl.x, carry.y + wo.y + incl.y);
     __syncthreads();
   }
-  if (threadIdx.x == 0) a.totals[0] = s_carry.x, a.totals[1] = s_carry.y;
+  if (threadIdx.x == 0) totals[0] = s_carry.x, totals[1] = s_carry.y;
 }
 
 // Block-wide exclusive rank of `flag` in thread order; 16 warps.
@@ -323,7 +323,11 @@ cudaError_t launchGroundSortBlocks(const DevLayer& tsdf, int hw, unsigned long l
 
 void launchGroundCount(const GroundExtractArgs& a, cudaStream_t stream) {
   groundCountKernel<<<a.num_blocks, kPairThreads, 0, stream>>>(a);
-  groundScanKernel<<<1, kScanThreads, 0, stream>>>(a);
+  exclusiveScanInt2Kernel<<<1, kScanThreads, 0, stream>>>(a.counts, a.num_blocks, a.totals);
+}
+
+void launchExclusiveScanInt2(int2* counts, int n, int* totals, cudaStream_t stream) {
+  exclusiveScanInt2Kernel<<<1, kScanThreads, 0, stream>>>(counts, n, totals);
 }
 
 void launchGroundEmit(const GroundExtractArgs& a, cudaStream_t stream) {

@@ -656,6 +656,8 @@ cudaError_t launchGroundSortBlocks(const DevLayer& tsdf, int hw, unsigned long l
                                    size_t temp_bytes, cudaStream_t stream);
 void launchGroundCount(const GroundExtractArgs& a, cudaStream_t stream);  // counts + scan + totals
 void launchGroundEmit(const GroundExtractArgs& a, cudaStream_t stream);
+// Exclusive prefix sums of n int2 counts in place, one CTA; the two totals -> totals[0..1].
+void launchExclusiveScanInt2(int2* counts, int n, int* totals, cudaStream_t stream);
 void launchPackPoints(const float* xyz, int n, float4* out, cudaStream_t stream);
 size_t ransacStateBytes();  // one XORWOW state
 // curand_init(1234, i, 0) for the iterations first <= i < n
@@ -663,5 +665,32 @@ void launchRansacInit(void* states, int first, int n, cudaStream_t stream);
 // MSAC over n >= 1 points (float4, w unused) -> out5 = {nx, ny, nz, d, found (int)}
 void launchRansacFit(const float4* pts, int n, int iterations, float threshold, const void* states, float* costs,
                      float4* planes, float* out5, bool reference_shape, cudaStream_t stream);
+
+// nvb_dynamics.cu: DynamicsDetection::computeDynamics and MaskPreprocessor::removeSmallConnectedComponents
+struct DynamicsArgs {
+  const float* depth;  // rows x cols, device
+  int rows, cols;
+  Rigid T_L_C;
+  NvbCamera cam;
+  DevLayer fs;          // the FreespaceLayer
+  float block_size, voxel_size_inv;
+  unsigned char* mask;     // rows x cols: 255 dynamic, 0 not
+  unsigned char* overlay;  // rows x cols x 3 (RGB)
+  int2* counts;            // per 256-pixel tile: dynamic pixels, then their exclusive prefix sums
+  float* points;           // xyz of the dynamic pixels' points, in row-major pixel order
+};
+int dynamicsNumTiles(int pixels);
+// detect + scan + emit; the number of points -> totals[0] (totals[1] is 0)
+void launchDynamicsDetect(const DynamicsArgs& a, int* totals, cudaStream_t stream);
+struct CcArgs {
+  const unsigned char* in;  // rows x cols
+  unsigned char* out;       // rows x cols (may alias `in`: the input is only read by the first pass)
+  int rows, cols;
+  int drows, dcols;         // rows / 2, cols / 2
+  int min_size;             // components of fewer downscaled pixels are erased
+  int* labels;              // drows x dcols
+  int* sizes;               // drows x dcols
+};
+void launchRemoveSmallComponents(const CcArgs& a, int num_sms, cudaStream_t stream);
 
 }  // namespace nvb

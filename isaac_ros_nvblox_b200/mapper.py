@@ -685,6 +685,100 @@ def ransac_fit_plane(points, num_ransac_iterations=1000, ransac_distance_thresho
     return tuple(float(v) for v in pl) if found.value else None
 
 
+class DynamicsDetection:
+    """DynamicsDetection (dynamics/dynamics_detection.h) on the freespace layer of one kTsdfWithFreespace mapper: a depth pixel
+    is dynamic when its surface point falls into a high-confidence freespace voxel. Outputs stay on the device until a getter
+    reads them; points come in row-major pixel order. The *_device variants take and fill raw device pointers, enqueued on
+    the mapper's stream (cuda_stream()) without synchronising."""
+
+    def __init__(self, mapper):
+        self._m = mapper
+
+    def compute_dynamics(self, depth, T_L_C, camera):
+        """computeDynamics(depth_frame, freespace_layer, camera, T_L_C); depth: (rows, cols) float32 host array."""
+        d = np.ascontiguousarray(depth, dtype=np.float32)
+        check(self._m._L.nvb_mapper_compute_dynamics(self._m._h, d.ctypes.data, _lib.NVB_MEM_HOST, d.shape[0], d.shape[1],
+                                                     _fp(colmajor(T_L_C)), C.byref(camera.c)))
+
+    def compute_dynamics_device(self, depth_ptr, rows, cols, T_L_C, camera):
+        check(self._m._L.nvb_mapper_compute_dynamics(self._m._h, depth_ptr, _lib.NVB_MEM_DEVICE, int(rows), int(cols),
+                                                     _fp(colmajor(T_L_C)), C.byref(camera.c)))
+
+    def _image(self, fn, channels):
+        rows, cols = C.c_int32(0), C.c_int32(0)
+        check(fn(self._m._h, None, _lib.NVB_MEM_HOST, C.byref(rows), C.byref(cols)))
+        out = np.zeros((rows.value, cols.value, channels) if channels > 1 else (rows.value, cols.value), dtype=np.uint8)
+        if out.size:
+            check(fn(self._m._h, out.ctypes.data, _lib.NVB_MEM_HOST, C.byref(rows), C.byref(cols)))
+        return out
+
+    def dynamic_mask(self):
+        """getDynamicMaskImage(): (rows, cols) uint8, 255 on dynamic pixels."""
+        return self._image(self._m._L.nvb_mapper_dynamic_mask, 1)
+
+    def dynamic_overlay(self):
+        """getDynamicOverlayImage(): (rows, cols, 3) uint8 RGB."""
+        return self._image(self._m._L.nvb_mapper_dynamic_overlay, 3)
+
+    def dynamic_mask_device(self, out_ptr):
+        """Copies the mask into rows x cols device bytes at out_ptr (enqueued); returns (rows, cols)."""
+        rows, cols = C.c_int32(0), C.c_int32(0)
+        check(self._m._L.nvb_mapper_dynamic_mask(self._m._h, out_ptr, _lib.NVB_MEM_DEVICE, C.byref(rows), C.byref(cols)))
+        return rows.value, cols.value
+
+    def dynamic_overlay_device(self, out_ptr):
+        rows, cols = C.c_int32(0), C.c_int32(0)
+        check(self._m._L.nvb_mapper_dynamic_overlay(self._m._h, out_ptr, _lib.NVB_MEM_DEVICE, C.byref(rows), C.byref(cols)))
+        return rows.value, cols.value
+
+    def dynamic_points(self):
+        """getDynamicPointsHost(): (n, 3) float32, in row-major pixel order."""
+        n = C.c_int32(0)
+        check(self._m._L.nvb_mapper_dynamic_points(self._m._h, None, _lib.NVB_MEM_HOST, 0, C.byref(n)))
+        out = np.zeros((n.value, 3), dtype=np.float32)
+        if n.value:
+            check(self._m._L.nvb_mapper_dynamic_points(self._m._h, out.ctypes.data, _lib.NVB_MEM_HOST, n.value, C.byref(n)))
+        return out
+
+    def dynamic_points_device(self, out_ptr, cap):
+        """Copies up to cap points (3 floats each) to device memory at out_ptr; returns the number of dynamic points."""
+        n = C.c_int32(0)
+        check(self._m._L.nvb_mapper_dynamic_points(self._m._h, out_ptr, _lib.NVB_MEM_DEVICE, int(cap), C.byref(n)))
+        return n.value
+
+    def device_buffers(self):
+        """The detector's own device buffers (raw pointers), valid until the next compute_dynamics on this mapper."""
+        b = _lib.NvbDynamicsBuffers()
+        check(self._m._L.nvb_mapper_dynamics_device_buffers(self._m._h, C.byref(b)))
+        return {k: getattr(b, k) for k, _ in b._fields_}
+
+
+_filter_mappers = {}
+
+
+def remove_small_connected_components(mask, threshold, mapper=None, device=0):
+    """MaskPreprocessor::removeSmallConnectedComponents(mask, threshold): (rows, cols) uint8 host mask -> the filtered mask of
+    the same size (survivors 254, the rest 0; a trailing odd row / column is 0). Runs on `mapper`'s device, stream and
+    scratch; without one, on a small mapper kept per device."""
+    if mapper is None:
+        mapper = _filter_mappers.get(device)
+        if mapper is None:
+            mapper = _filter_mappers[device] = Mapper(0.05, device=device, tsdf_capacity_blocks=64, esdf_capacity_blocks=64)
+    a = np.ascontiguousarray(mask, dtype=np.uint8)
+    if a.ndim != 2:
+        raise ValueError("the mask must be a (rows, cols) image")
+    out = np.empty_like(a)
+    check(mapper._L.nvb_mapper_remove_small_components(mapper._h, a.ctypes.data, out.ctypes.data, _lib.NVB_MEM_HOST,
+                                                        a.shape[0], a.shape[1], int(threshold)))
+    return out
+
+
+def remove_small_connected_components_device(mask_in_ptr, mask_out_ptr, rows, cols, threshold, mapper):
+    """The same on rows x cols device bytes, enqueued on mapper.cuda_stream() without synchronising."""
+    check(mapper._L.nvb_mapper_remove_small_components(mapper._h, mask_in_ptr, mask_out_ptr, _lib.NVB_MEM_DEVICE, int(rows),
+                                                        int(cols), int(threshold)))
+
+
 class Mapper:
     """nvblox::Mapper(voxel_size_m, projective_layer_type) with a projective (TSDF or occupancy) and an ESDF layer."""
 
@@ -750,6 +844,14 @@ class Mapper:
     def ground_plane_estimator(self):
         """MultiMapper::ground_plane_estimator() of this mapper (its state lives in the mapper)."""
         return GroundPlaneEstimator(self)
+
+    def dynamics_detection(self):
+        """The DynamicsDetection of this mapper's freespace layer (its state lives in the mapper)."""
+        return DynamicsDetection(self)
+
+    def wait_for(self, producer):
+        """Later work on this mapper's stream runs after everything enqueued so far on producer's (device-side)."""
+        check(self._L.nvb_mapper_wait_for(self._h, producer._h))
 
     def occupancy_layer(self):
         return self._occupancy

@@ -63,7 +63,7 @@ def timed(fn):
     return (time.perf_counter() - t0) * 1e6, out
 
 
-KERNELS = ("groundCountKernel", "groundScanKernel", "groundEmitKernel", "ransacFitKernel", "ransacArgminKernel")
+KERNELS = ("groundCountKernel", "exclusiveScanInt2Kernel", "groundEmitKernel", "ransacFitKernel", "ransacArgminKernel")
 
 
 def kernel_times(m, repeats):
