@@ -691,6 +691,10 @@ NVB_API int32_t nvb_mapper_esdf_time_split(NvbMapper* m, int64_t out[4]);
  * `clear_candidates` statistic keeps counting the reference's candidates). */
 NVB_API int32_t nvb_mapper_esdf_clear_blocks_read(NvbMapper* m, int64_t* out);
 
+/* The exchange-slab wavefront's own-block fetches in the last ESDF update: [0] candidates whose block was fetched split
+ * (boundary planes first), [1] of those, the ones that changed and fetched the rest of their block. Synchronising. */
+NVB_API int32_t nvb_mapper_esdf_split_stats(NvbMapper* m, int64_t out[2]);
+
 /* Debug: work time (ns) of the slowest CTA in each barrier-delimited phase of the last wavefront. */
 NVB_API int32_t nvb_mapper_debug_phase_max(NvbMapper* m, int64_t* out, int32_t cap);
 

@@ -69,6 +69,7 @@ struct NvbMapper {
   int projective_layer_type = 0;
   int esdf_persistent = 1;
   int esdf_reserved_sms = 2;  // SMs the exchange-slab wavefront leaves to concurrently running kernels (nvb_esdf_wavex.cu)
+  int esdf_split_min_k = 0;   // exchange-slab wavefront: smallest grid ring that fetches its candidates' blocks split
 
   DevLayer tsdf{}, esdf{};
   DevLayer freespace{};    // FreespaceLayer of a NVB_PROJECTIVE_TSDF_WITH_FREESPACE mapper
@@ -515,6 +516,7 @@ EsdfCtx makeEsdfCtx(NvbMapper* m) {
   c.psum = m->psum, c.prune = (m->prune_ok && m->esdf_persistent == 3) ? 1 : 0;
   c.nbr27 = m->nbr27, c.shadow = m->shadow, c.cand_stamp = m->cand_stamp;
   c.xslab = m->xslab, c.xrec = m->xrec, c.xtail = m->esdf_ints + kXTail, c.xseg = m->xseg, c.xcounts = m->xcounts;
+  c.xsplit_min_k = m->esdf_split_min_k;
   c.ges_counts = m->esdf_ints + kGesCounts;
   c.cand_a = m->cand_a, c.cand_b = m->cand_b, c.ges_switch = m->ges_switch;
   c.colset_keys = m->colset, c.colset_mask = m->colset_n ? (unsigned int)(m->colset_n - 1) : 0u;
@@ -1268,6 +1270,7 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   // A/B switch for measurements: 0 host loop, 1 four-phase wavefront, 2 gather-emulate-sweep wavefront
   if (const char* e = getenv("NVB_ESDF_MODE")) m->esdf_persistent = atoi(e);
   if (const char* e = getenv("NVB_WAVEX_RESERVED_SMS")) m->esdf_reserved_sms = std::max(0, std::min(64, atoi(e)));
+  m->esdf_split_min_k = esdfWaveXSplitMinK();
   if (const char* e = getenv("NVB_GES_SWITCH")) m->ges_switch = atoi(e);
   {
     const char* e = getenv("NVB_CLEAR_PRUNE");
@@ -3347,6 +3350,16 @@ int32_t nvb_mapper_esdf_clear_blocks_read(NvbMapper* m, int64_t* out) {
   long long v = 0;
   NVB_CUDA(cudaMemcpy(&v, m->stats + 13, sizeof(v), cudaMemcpyDeviceToHost));
   *out = v;
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_esdf_split_stats(NvbMapper* m, int64_t out[2]) {
+  if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  NVB_CUDA(cudaSetDevice(m->device));
+  NVB_CUDA(syncAll(m));
+  long long tmp[2];
+  NVB_CUDA(cudaMemcpy(tmp, m->stats + 14, sizeof(tmp), cudaMemcpyDeviceToHost));
+  out[0] = tmp[0], out[1] = tmp[1];
   return NVB_OK;
 }
 

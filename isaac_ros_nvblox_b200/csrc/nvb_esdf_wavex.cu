@@ -69,10 +69,20 @@ namespace {
   tq = clock64();
 #define X_PROF_COUNT(i) \
   if (lane64 == 0) xs.prof[group][i]++;
+// stage i, also binned by the ring's candidate count K (bins K <= 256, <= 1 040, > 1 040 at index j, j + 1, j + 2; the
+// candidates per bin at j + 3 ..): the own-block fetch of all of a ring's candidates leaves at once after the barrier
+#define X_PROF_BIN(i, j, K)                                                  \
+  if (lane64 == 0) {                                                         \
+    const int kb = (K) <= 256 ? 0 : ((K) <= 1040 ? 1 : 2);                   \
+    const long long dt = clock64() - tq;                                     \
+    xs.prof[group][i] += dt, xs.prof[group][(j) + kb] += dt, xs.prof[group][(j) + 3 + kb]++; \
+  }                                                                          \
+  tq = clock64();
 #else
 #define X_PROF_BEGIN()
 #define X_PROF(i)
 #define X_PROF_COUNT(i)
+#define X_PROF_BIN(i, j, K)
 #endif
 constexpr int kXT = NVB_WAVEX_THREADS;
 constexpr int kXG = kXT / 64;
@@ -111,8 +121,12 @@ struct XShared {
   int n_bar;                // grid barriers passed in this launch
   int ring;                 // the ring being processed (written by thread 0 between two CTA barriers)
   int swept, faces, rings, n_tail;  // statistics (thread 0)
+  int n_split, n_rest;              // statistics: candidates fetched split, rest-of-block fetches (lane 0 of each group)
 #if NVB_WAVEX_PROF
-  long long prof[kXG][8];   // per group, cycles: record, stamps + own block (+ speculative faces), halo, replay, sweep, stores; candidates, changed
+  // per group, cycles: [0] record, [1] stamps (+ own block when not split; + speculative faces), [2] halo (+ the own block's
+  // live planes when split), [3] replay, [4] sweep (+ registration), [5] stores; [6] candidates, [7] changed; [8] rest of
+  // the block (issue + registerBegin + wait; changed candidates); [9..11] [1] by K bin, [12..14] candidates by K bin
+  long long prof[kXG][16];
 #endif
 };
 
@@ -130,6 +144,7 @@ struct XCtx {
   unsigned char* X[2];    // exchange slabs by ring parity
   int* recs[2];           // candidate records by ring parity: one segment of `seg` records per CTA
   int seg;
+  int split_min_k;        // grid rings with at least this many candidates fetch the own block split (processCandidate)
   int* error;             // bit 8: a registration did not fit its CTA's segment (dropped, the launch's result is invalid)
   float max_sq;
   __device__ __forceinline__ int* segment(int p, int cta) const { return recs[p] + (size_t)cta * seg * kRecInts; }
@@ -245,6 +260,7 @@ __device__ __forceinline__ void initTables(XTables& tab, int tid) {
 struct LiveMasks {
   unsigned int* live;   // [6], in shared memory (indexed by a run-time pass number)
   unsigned int needed;  // members (without B) that take part in a live pair
+  unsigned int axes;    // bit a: a pass along axis a is live (liveAxes)
 };
 __device__ __forceinline__ LiveMasks liveMasks(unsigned int mask, unsigned int* live_smem, bool writer) {
   LiveMasks L;
@@ -253,6 +269,7 @@ __device__ __forceinline__ LiveMasks liveMasks(unsigned int mask, unsigned int* 
   // D(p+1): blocks whose state after pass p can still reach B; bit d = (dx+1)*9 + (dy+1)*3 + (dz+1)
   const unsigned int D[6] = {0x7FFFE00u, 0x3FE00u, 0x3F000u, 0x7000u, 0x6000u, 0x2000u};
   unsigned int acc = 0;
+  L.axes = 0;
 #pragma unroll
   for (int p = 0; p < 6; p++) {
     const int axis = p >> 1;
@@ -268,6 +285,7 @@ __device__ __forceinline__ LiveMasks liveMasks(unsigned int mask, unsigned int* 
       dst = lv >> A;
     }
     if (writer) live_smem[p] = lv;
+    if (lv) L.axes |= 1u << axis;
     acc |= lv | dst;
   }
   L.needed = acc & mask & ~(1u << 13);
@@ -284,6 +302,9 @@ __device__ __forceinline__ OwnRegs ownLoad(const unsigned char* blk, int lane64)
 #pragma unroll
   for (int i = 0; i < 10; i++) o.q[i] = __ldcg(src + i);
   return o;
+}
+__device__ __forceinline__ unsigned int liveAxes(const unsigned int* live) {  // bit a: a pass along axis a is live
+  return ((live[0] | live[1]) ? 1u : 0u) | ((live[2] | live[3]) ? 2u : 0u) | ((live[4] | live[5]) ? 4u : 0u);
 }
 __device__ __forceinline__ unsigned int ownWord(const OwnRegs& o, int w) {  // w is a compile-time constant after unrolling
   const uint4& v = o.q[w >> 2];
@@ -358,6 +379,29 @@ __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer
 __device__ __forceinline__ void cpAsync4(unsigned int* smem_dst, const unsigned int* gsrc) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned int)__cvta_generic_to_shared(smem_dst)), "l"(gsrc)
                : "memory");
+}
+// ---- the own block split in two (grid rings, processCandidate): first the voxels on the boundary planes of
+// the axes `axes` (bit a: the planes 0 and 7 along axis a), which hold every voxel of B the replay reads or writes, then -- only
+// if B changed -- the rest. 4-byte copies like the halo's (the block's 20-byte voxels are not 16-byte aligned), one voxel per
+// lane and x plane (lane = y * 8 + z: a warp's copies of one word cover 640 contiguous bytes). `planes`: copy the voxels on
+// those planes, else every other voxel. (.ca: the layer's blocks are written with .cg stores by the owners of earlier rings,
+// and the grid barrier between them and this read invalidates the SM's L1; the single-CTA tail does not fetch split.)
+__device__ __forceinline__ void ownAsync(unsigned int* R, const unsigned char* blk, int lane64, unsigned int axes, bool planes) {
+  const int y = lane64 >> 3, z = lane64 & 7;
+  const bool lane_on = ((axes & 2u) && (y == 0 || y == 7)) || ((axes & 4u) && (z == 0 || z == 7));
+  const unsigned int* src = reinterpret_cast<const unsigned int*>(blk) + lane64 * kEsdfVoxelWords;
+  const int v0 = rvox(1, y + 1, z + 1);
+#pragma unroll
+  for (int x = 0; x < 8; x++) {
+    const bool on = lane_on || ((axes & 1u) && (x == 0 || x == 7));
+    if (on == planes) {
+      const unsigned int* s = src + x * 64 * kEsdfVoxelWords;
+      const int v = v0 + x * kRX;
+#pragma unroll
+      for (int w = 0; w < 4; w++) cpAsync4(R + 4 * v + w, s + w);
+      cpAsync4(R + kFlagBase + v, s + 4);
+    }
+  }
 }
 // Halo batches `batches` (bit k: batch k of the table), the voxels whose block d has bit d in `blocks` and is allocated.
 __device__ __forceinline__ void haloAsync(const XTables& tab, unsigned int* R, const int* row, const unsigned char* X, int lane64,
@@ -574,38 +618,52 @@ __device__ __forceinline__ void registerFinish(const XCtx& c, XShared& xs, const
 
 // One candidate of ring `ring`: gather, replay, and if it changed: sweep, publish, register its neighbours for ring+1.
 // The entry is xs.seg[group] (registering CTA, index in its segment); the group is the caller's (threadIdx.x / 64).
-__device__ __noinline__ void processCandidate(int ring) {
+// K: the ring's candidate count, -1 in the single-CTA tail. A grid ring with K >= c.split_min_k fetches the own block SPLIT:
+// right after a grid barrier every group of every CTA asks for a 10 KiB block at once, and most candidates do not change
+// (they outnumber the members 2.5-3.5x), so the candidate first fetches only the boundary planes of B along the live passes'
+// axes, with the halo, after the stamps; the rest of B follows only if B changed, with registerBegin's atomics and row loads.
+__device__ __noinline__ void processCandidate(int ring, int K) {
   const XCtx& c = x_ctx;
   const XTables& tab = x_tab;
   XShared& xs = x_xs;
   const int cta = blockIdx.x, group = threadIdx.x >> 6, lane64 = threadIdx.x & 63;
   unsigned int* R = x_smem + group * kXRegionWords;
   const int ci = ring & 1, ni = ci ^ 1;
+  const bool split = K >= c.split_min_k;
   X_PROF_BEGIN()
   if (lane64 < 28) xs.rec[group][lane64] = __ldcg(c.segment(ci, xs.seg[group][0]) + (size_t)xs.seg[group][1] * kRecInts + lane64);
   groupSync(group);
   X_PROF(0)
   const int slot = xs.rec[group][0];
   const int* row = &xs.rec[group][1];
-  // membership of the 27 blocks in this ring (sources of the passes); the loads travel with the loads of the own block and
-  // (NVB_WAVEX_SPEC_HALO) the face halo
+  const unsigned char* blk = c.blocks + (size_t)slot * kEsdfBlockBytes;
+  // membership of the 27 blocks in this ring (sources of the passes); the loads travel with the loads of the own block (when
+  // not split) and (NVB_WAVEX_SPEC_HALO) the face halo
   int sv = ring - 1;
   if (lane64 < 27 && row[lane64] >= 0) sv = __ldcg(c.stamp[ci] + row[lane64]);
-  OwnRegs own = ownLoad(c.blocks + (size_t)slot * kEsdfBlockBytes, lane64);
   if (NVB_WAVEX_SPEC_HALO) haloAsync(tab, R, row, c.X[ci], lane64, 0x3Fu, 0x7FFFFFFu);
-  const unsigned int m = __ballot_sync(0xffffffffu, lane64 < 27 && sv == ring);
-  if (lane64 == 0) xs.mask[group] = m, xs.changed[group] = 0;
-  ownToShared(R, own, lane64);
+  if (split) {
+    const unsigned int m = __ballot_sync(0xffffffffu, lane64 < 27 && sv == ring);
+    if (lane64 == 0) xs.mask[group] = m, xs.changed[group] = 0;
+  } else {
+    OwnRegs own = ownLoad(blk, lane64);
+    const unsigned int m = __ballot_sync(0xffffffffu, lane64 < 27 && sv == ring);
+    if (lane64 == 0) xs.mask[group] = m, xs.changed[group] = 0;
+    ownToShared(R, own, lane64);
+  }
   if (NVB_WAVEX_SPEC_HALO) cpAsyncWaitAll();
   groupSync(group);
   const LiveMasks L = liveMasks(xs.mask[group], xs.live[group], lane64 == 0);
-  X_PROF(1)
-  // the halo of the members that take part in a live pair (with NVB_WAVEX_SPEC_HALO: only their edge and corner batches)
+  X_PROF_BIN(1, 9, K)
+  // the halo of the members that take part in a live pair (with NVB_WAVEX_SPEC_HALO: only their edge and corner batches),
+  // and when split, B's boundary planes along the live passes' axes
   const unsigned int rest = NVB_WAVEX_SPEC_HALO ? (L.needed & ~kFaceBlocks) : L.needed;
-  if (rest) {  // group-uniform
-    haloAsync(tab, R, row, c.X[ci], lane64, haloBatches(rest), rest);
-    cpAsyncWaitAll();
+  if (split) {
+    ownAsync(R, blk, lane64, L.axes, true);
+    if (lane64 == 0) atomicAdd(&xs.n_split, 1);
   }
+  if (rest) haloAsync(tab, R, row, c.X[ci], lane64, haloBatches(rest), rest);  // group-uniform
+  if (rest || split) cpAsyncWaitAll();
   groupSync(group);  // (also publishes xs.live[group], written by lane 0 in liveMasks and read by every lane in replayX)
   X_PROF(2)
   const bool ch = replayX(tab, R, L, lane64, group, c.max_sq);
@@ -621,7 +679,14 @@ __device__ __noinline__ void processCandidate(int ring) {
       atomicAdd(&xs.nchanged, 1);
     }
     groupSync(group);
+    if (split) ownAsync(R, blk, lane64, liveAxes(xs.live[group]), false);  // the rest of B (the replay wrote only the planes)
     RegState rs = registerBegin(c, xs, group, lane64, ring + 1);
+    if (split) {
+      if (lane64 == 0) atomicAdd(&xs.n_rest, 1);
+      cpAsyncWaitAll();
+      groupSync(group);
+    }
+    X_PROF(8)
     sweepBlockX(R, group, lane64, c.max_sq);
     registerClaim(c, xs, rs, group, lane64, ring + 1);
     groupSync(group);
@@ -738,17 +803,17 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
   if (tid == 0) {
     xs.ncand = 0, xs.nchanged = 0, xs.next = 0;
     xs.ring = *(volatile int*)c.ring_id;
-    xs.generation = 0, xs.n_bar = 0, xs.swept = 0, xs.faces = 0, xs.rings = 0, xs.n_tail = 0;
+    xs.generation = 0, xs.n_bar = 0, xs.swept = 0, xs.faces = 0, xs.rings = 0, xs.n_tail = 0, xs.n_split = 0, xs.n_rest = 0;
     XCtx& xc = x_ctx;
     xc.blocks = c.esdf.blocks, xc.block_index = c.esdf.block_index, xc.hash = c.esdf.hash;
     xc.nbr = c.nbr, xc.nbr27 = c.nbr27, xc.cand_stamp = c.cand_stamp, xc.psum = c.psum;
     xc.stamp[0] = c.stamp_a, xc.stamp[1] = c.stamp_b;
     xc.X[0] = c.xslab, xc.X[1] = c.xslab + (size_t)c.esdf.capacity * kEsdfBlockBytes;
     xc.recs[0] = c.xrec, xc.recs[1] = c.xrec + (size_t)nctas * c.xseg * kRecInts;
-    xc.seg = c.xseg, xc.error = c.error, xc.max_sq = c.max_sq;
+    xc.seg = c.xseg, xc.split_min_k = c.xsplit_min_k, xc.error = c.error, xc.max_sq = c.max_sq;
   }
 #if NVB_WAVEX_PROF
-  if (lane64 < 8) xs.prof[group][lane64] = 0;
+  if (lane64 < 16) xs.prof[group][lane64] = 0;
 #endif
   __syncthreads();
 #if NVB_WAVEX_PROF
@@ -806,7 +871,7 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
           }
           __syncthreads();
           while (true) {
-            if (group < K) processCandidate(xs.ring);
+            if (group < K) processCandidate(xs.ring, -1);
             __syncthreads();
             const int K2 = min(xs.ncand, c.xseg), M2 = xs.nchanged;
             __syncthreads();
@@ -845,7 +910,7 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
         for (int s = lane64; s < nctas; s += 64)
           if (xs.pre[s] <= e && e < xs.pre[s + 1]) xs.seg[group][0] = s, xs.seg[group][1] = (int)e - xs.pre[s];
         groupSync(group);
-        processCandidate(xs.ring);
+        processCandidate(xs.ring, K);
       }
       int K2, M2;
       X_BARRIER(1, K2, M2)
@@ -860,6 +925,10 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
 #undef X_TIME_WORK
 #undef X_TIME_BARRIER
 #undef X_DBG
+  if (tid == 0 && xs.n_split) {  // (the counts are final: the last ring ended with a CTA barrier)
+    atomicAdd((unsigned long long*)&c.stats[14], (unsigned long long)xs.n_split);
+    atomicAdd((unsigned long long*)&c.stats[15], (unsigned long long)xs.n_rest);
+  }
   if (cta == 0 && tid == 0) {
     *c.ring_id = xs.ring + 1;
     c.stats[4] = *(volatile int*)c.cleared_count;
@@ -870,7 +939,7 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
     long long sum_max = 0;
     for (int q = 0; q < xs.n_bar && q < 1000; q++) sum_max += (long long)c.phase_max[q];
     c.stats[12] = sum_max;
-    for (int q = 0; q < 8; q++) c.phase_max[3990 + q] = xs.prof[0][q];
+    for (int q = 0; q < 16; q++) c.phase_max[3984 + q] = xs.prof[0][q];
 #endif
   }
 }
@@ -883,6 +952,17 @@ int esdfWaveXGrid(int num_sms, int reserved_sms) {
   return grid;
 }
 size_t esdfWaveXFlagBytes() { return 2 * (size_t)kMaxCtas * sizeof(int2); }
+
+// Grid rings with at least this many candidates fetch their candidates' own blocks split (processCandidate). 0: every grid
+// ring (K > 8; the single-CTA tail and the seeds fetch whole blocks). 80-frame c2 bench on one H100 SXM at a 700 W power
+// limit, two runs each: threshold 0 / 256 / 1 040 / never -> 2 835, 2 833 / 2 811, 2 814 / 2 732, 2 723 / 2 651, 2 582 frames/s.
+constexpr int kSplitMinK = 0;
+int esdfWaveXSplitMinK() {
+  // Test hook: NVB_WAVEX_SPLIT_MIN_K=<n> replaces kSplitMinK (0: every grid ring fetches split, 1000000000: none does).
+  const char* e = getenv("NVB_WAVEX_SPLIT_MIN_K");
+  const int v = e ? atoi(e) : kSplitMinK;
+  return v < 0 ? 0 : v;
+}
 
 cudaError_t launchEsdfComputeX(const EsdfCtx& c, int num_sms, int reserved_sms, cudaStream_t stream, int* launches) {
   static int per_sm = -1;

@@ -389,7 +389,8 @@ struct EsdfCtx {
   int* xrec;              // exchange-slab wavefront: candidate records {slot, 27 neighbour slots, pad}, 32 ints; per ring parity one
                           // segment of `xseg` records per CTA
   int xseg;
-  int* xcounts;           // exchange-slab wavefront: barrier flags, per barrier parity and CTA {generation, registrations, changed blocks}
+  int xsplit_min_k;       // exchange-slab wavefront: grid rings with at least this many candidates fetch the own block split
+  int* xcounts;          // exchange-slab wavefront: barrier flags, per barrier parity and CTA {generation, registrations, changed blocks}
   int slice_mode;  // the ESDF layer is a 2-D slice (EsdfMode::k2D)
   // constant-z slice (2-D ESDF): block / voxel z of the band's bottom and top and of the output layer
   int slice_min_bz, slice_min_vz, slice_max_bz, slice_max_vz, slice_out_bz, slice_out_vz;
@@ -424,7 +425,7 @@ struct EsdfCtx {
   int* tracker_todo_count;
   unsigned int* barrier;  // grid barrier counter
   unsigned long long* phase_max;  // debug: per-phase max-over-CTAs work time (1000 entries)
-  long long* stats;    // 8 counters
+  long long* stats;    // 16 counters ([14], [15]: the exchange-slab wavefront's split candidates and rest-of-block fetches)
   int* error;
   float max_sq;
   float max_esdf_distance_m;
@@ -446,6 +447,7 @@ cudaError_t launchEsdfComputePersistent(const EsdfCtx& c, int num_sms, cudaStrea
 cudaError_t launchEsdfComputeX(const EsdfCtx& c, int num_sms, int reserved_sms, cudaStream_t stream, int* launches);  // nvb_esdf_wavex.cu
 int esdfWaveXGrid(int num_sms, int reserved_sms);  // CTAs of an exchange-slab launch
 size_t esdfWaveXFlagBytes();
+int esdfWaveXSplitMinK();  // kSplitMinK, or NVB_WAVEX_SPLIT_MIN_K (read at mapper creation)
 // Reference-like driver: one launch per phase, host reads the ring counter.
 cudaError_t runEsdfComputeHostLoop(const EsdfCtx& c, int num_sms, cudaStream_t stream, int* launches);
 int esdfPersistentMaxCtas(int num_sms);

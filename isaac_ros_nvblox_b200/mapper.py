@@ -425,7 +425,12 @@ class _EsdfIntegrator:
         out = (C.c_int64 * 8)()
         check(self._m._L.nvb_mapper_last_esdf_stats(self._m._h, out))
         keys = ("marked", "with_sites", "to_clear", "clear_candidates", "cleared", "swept", "face_passes", "rings")
-        return dict(zip(keys, list(out)))
+        s = dict(zip(keys, list(out)))
+        # exchange-slab wavefront: candidates whose own block was fetched split, and those that then fetched the rest
+        split = (C.c_int64 * 2)()
+        check(self._m._L.nvb_mapper_esdf_split_stats(self._m._h, split))
+        s.update(split_candidates=split[0], rest_fetches=split[1])
+        return s
 
     def clear_blocks_read(self):
         """Blocks the last clear pass read (<= clear_candidates: candidates whose parents cannot lie in a to-clear block are skipped)."""

@@ -6,9 +6,13 @@ tests), runs bench.py's c2 frames through it with a synchronise after every upda
 
   phases  : per grid-barrier phase of every frame: kind (seed / grid ring / tail), K (candidates; -1 for the seed phase),
             M (members), the maximum work time over CTAs and CTA 0's work time (ns, %globaltimer)
-  stages  : per frame, the cycles group 0 of CTA 0 spent in each stage of processCandidate (record; stamps + own block; halo;
-            replay; sweep (+ registration); stores + records) and its candidate / changed counts
-  summary : totals per phase kind, the stage shares, and the barrier time = wavefront stage time - summed work maxima
+  stages  : per frame, the cycles group 0 of CTA 0 spent in each stage of processCandidate (record; stamps (+ own block
+            when not split); halo (+ the own block's live planes when split); replay; rest of block (changed candidates:
+            issue + registration atomics + wait); sweep (+ registration); stores + records), the stamps stage binned by
+            the ring's candidate count K (<= 256, <= 1 040, > 1 040) with the candidates per bin, its candidate / changed
+            counts, and the launch's split candidates and rest-of-block fetches (esdf_integrator().last_stats())
+  summary : totals per phase kind, a least-squares line of the grid rings' slowest-CTA work time against K, the stage
+            shares, the stamps stage per K bin, and the barrier time = wavefront stage time - summed work maxima
 
 The profiling counters cost registers (and spills), so the absolute times of this build are inflated: quote its SHARES, and
 take absolute times from the normal build (bench.py's `stages`). The card's name and power limit are recorded alongside.
@@ -28,6 +32,8 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 STAGE_KEYS = ("record", "stamps_own_block", "halo", "replay", "sweep", "stores_records")
+PROF_BASE = 3984  # NVB_WAVEX_PROF words of debug_phase_max: 16 counters of CTA 0's group 0 (XShared::prof)
+K_BINS = ("k_le_256", "k_le_1040", "k_gt_1040")
 KIND_TAIL_MAX_K = 8  # rings with at most one candidate per 64-thread group of one CTA run as a single-CTA tail
 
 
@@ -89,8 +95,13 @@ def main():
                     k = int(pm[1000 + q])
                     phases.append({"frame": i, "phase": q, "kind": phase_kind(k), "K": k, "M": int(pm[2000 + q]),
                                    "max_work_ns": int(pm[q]), "cta0_work_ns": int(pm[3000 + q])})
-                s = {key: int(pm[3990 + j]) for j, key in enumerate(STAGE_KEYS)}
-                s.update(frame=i, candidates=int(pm[3996]), changed=int(pm[3997]))
+                p = pm[PROF_BASE:PROF_BASE + 16]
+                s = {key: int(p[j]) for j, key in enumerate(STAGE_KEYS)}
+                s.update(frame=i, candidates=int(p[6]), changed=int(p[7]), rest_of_block=int(p[8]),
+                         stamps_own_block_by_k={b: int(p[9 + j]) for j, b in enumerate(K_BINS)},
+                         candidates_by_k={b: int(p[12 + j]) for j, b in enumerate(K_BINS)})
+                st = m.esdf_integrator().last_stats()
+                s.update(split_candidates=int(st["split_candidates"]), rest_fetches=int(st["rest_fetches"]))
                 stages.append(s)
             return phases, stages, compute_ms
 
@@ -113,22 +124,39 @@ def main():
         d["phases_per_frame"] = d["phases"] / F
     wave_us = 1e3 * sum(compute_ms) / F
     work_us = sum(d["max_work_us_per_frame"] for d in by_kind.values())
-    cyc = {key: sum(s[key] for s in stages) for key in STAGE_KEYS}
+    cyc = {key: sum(s[key] for s in stages) for key in STAGE_KEYS + ("rest_of_block",)}
     tot = max(sum(cyc.values()), 1)
     cands = sum(s["candidates"] for s in stages)
+    changed = sum(s["changed"] for s in stages)
+    grid = [(p["K"], p["max_work_ns"]) for p in phases if p["kind"] == "grid"]
+    fit = None
+    if len(grid) >= 2:
+        slope, icpt = np.polyfit([k for k, _ in grid], [t for _, t in grid], 1)
+        fit = {"rings": len(grid), "ns_per_candidate": float(slope), "ns_at_k0": float(icpt)}
+    by_k = {}
+    for b in K_BINS:
+        n = sum(s["candidates_by_k"][b] for s in stages)
+        c = sum(s["stamps_own_block_by_k"][b] for s in stages)
+        by_k[b] = {"candidates": n, "cycles_per_candidate": c / n if n else None}
     summary = {
         "frames": F,
         "wavefront_us_per_frame": wave_us,
         "summed_work_max_us_per_frame": work_us,
         "barrier_us_per_frame": wave_us - work_us,
         "by_kind": by_kind,
+        "grid_ring_work_vs_k": fit,
         "group0_stage_share": {k: v / tot for k, v in cyc.items()},
         "group0_cycles_per_candidate": {k: v / max(cands, 1) for k, v in cyc.items()},
+        "group0_rest_of_block_cycles_per_changed": cyc["rest_of_block"] / max(changed, 1),
+        "group0_stamps_own_block_by_k": by_k,
         "group0_candidates": cands,
-        "group0_changed": sum(s["changed"] for s in stages),
+        "group0_changed": changed,
+        "split_candidates_per_frame": sum(s["split_candidates"] for s in stages) / max(F, 1),
+        "rest_fetches_per_frame": sum(s["rest_fetches"] for s in stages) / max(F, 1),
     }
     os.makedirs(args.out, exist_ok=True)
-    res = {"gpu": gpu_info(), "build": "NVB_WAVEX_PROF=1 " + args.nvcc_flags, "summary": summary,
+    res = {"gpu": gpu_info(), "build": "NVB_WAVEX_PROF=1 " + args.nvcc_flags,
+           "NVB_WAVEX_SPLIT_MIN_K": os.environ.get("NVB_WAVEX_SPLIT_MIN_K"), "summary": summary,
            "stages": stages, "phases": phases}
     with open(os.path.join(args.out, "wavex_profile.json"), "w") as f:
         json.dump(res, f, indent=1)
