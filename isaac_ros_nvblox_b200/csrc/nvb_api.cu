@@ -187,7 +187,7 @@ struct NvbMapper {
   int* nbr27 = nullptr;
   unsigned char* shadow = nullptr;
   int shadow_cap = 0;
-  unsigned char* xslab = nullptr;  // exchange-slab wavefront (esdf_persistent == 3): 2 x capacity ESDF blocks
+  unsigned char* xslab = nullptr;  // exchange-slab wavefront (esdf_persistent == 3): 2 x capacity slots of six faces (7.5 KiB)
   int* xrec = nullptr;             // ... 2 x CTAs x xseg candidate records of 32 ints ...
   int xseg = 0;
   int xseg_grid = 0;               // CTAs of the exchange-slab launch the segments were sized for
@@ -460,7 +460,7 @@ int allocEsdfScratch(NvbMapper* m, int old_cap, int cap) {
     NVB_CUDA(syncAll(m));
     if (m->xslab) cudaFree(m->xslab);
     m->xslab = nullptr;
-    NVB_CUDA(cudaMalloc(&m->xslab, 2 * (size_t)cap * kEsdfBlockBytes));
+    NVB_CUDA(cudaMalloc(&m->xslab, esdfWaveXSlabBytes(cap)));
     int rc;
     if ((rc = allocWaveXRecords(m, cap))) return rc;
     if (!m->xcounts) {

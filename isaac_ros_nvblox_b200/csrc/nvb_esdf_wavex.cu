@@ -13,15 +13,17 @@
 //     it at once (sweepBlockBandKernel, :1390-1431). No communication inside a ring.
 //   * Sources are always MEMBERS. Every member's state at the start of the ring is published in an exchange slab indexed by
 //     slot, X[ring & 1]: the owner of a block that changes in ring r writes the new block to the layer (read by the block's
-//     next owner only) and to X[(r+1) & 1] (read by its neighbours' owners during ring r+1) while ring r's readers read
-//     X[r & 1]. Two slabs by ring parity, one barrier per ring, no version words, no copy-back phase.
+//     next owner only) and its six faces to X[(r+1) & 1] (read by its neighbours' owners during ring r+1, who only ever read
+//     boundary voxels) while ring r's readers read X[r & 1]. Two slabs by ring parity, one barrier per ring, no version words,
+//     no copy-back phase. A slot is face-major and in the region's split form (kXSlotBytes: 6 x 64 16-byte cells, then
+//     6 x 64 flag words, 7.5 KiB), so a halo voxel is one 16-byte and one 4-byte copy and a face 1 KiB + 256 contiguous bytes.
 //   * Only what can matter is fetched and replayed. A pass-p pair (source voxel -> destination voxel) matters iff its source
 //     block is a member and its destination block is B or a member that can still influence B through the LATER passes: the
 //     blocks whose state after pass p matters are D6 = {B}, D5 = D6 + {B+z}, D4 = D5 + {B-z}, D3 = D4 + (D4 + y),
 //     D2 = D3 + (D3 - y), D1 = D2 + (D2 + x) (backwards through -z,+z,-y,+y,-x,+x). With one to three member neighbours --
 //     the usual case -- one or two of the six passes are live and a few per cent of the 1 200 pair slots; halo voxels of
 //     blocks that are in no live pair are not fetched (they would miss L2: nobody wrote them lately). The halo travels by
-//     cp.async straight into the region planes, so no registers are held across its round trip.
+//     cp.async from the exchange slab straight into the region planes, so no registers are held across its round trip.
 //   * Region layout in shared memory: a plane of 16-byte cells {squared distance, parent} and a plane of flag words, voxel
 //     index rx*110 + ry*11 + rz. Every line of the three sweeps and every pair of the replay is ONE conflict-free 128-bit
 //     access per voxel (the 20-byte array-of-structures layout of the layer costs five 32-bit accesses with up to 8-way bank
@@ -78,11 +80,20 @@ namespace {
     xs.prof[group][i] += dt, xs.prof[group][(j) + kb] += dt, xs.prof[group][(j) + 3 + kb]++; \
   }                                                                          \
   tq = clock64();
+// stage i, also binned by K at index j + bin (the candidates per bin are counted by X_PROF_BIN)
+#define X_PROF_KBIN(i, j, K)                                \
+  if (lane64 == 0) {                                        \
+    const int kb = (K) <= 256 ? 0 : ((K) <= 1040 ? 1 : 2);  \
+    const long long dt = clock64() - tq;                    \
+    xs.prof[group][i] += dt, xs.prof[group][(j) + kb] += dt; \
+  }                                                         \
+  tq = clock64();
 #else
 #define X_PROF_BEGIN()
 #define X_PROF(i)
 #define X_PROF_COUNT(i)
 #define X_PROF_BIN(i, j, K)
+#define X_PROF_KBIN(i, j, K)
 #endif
 constexpr int kXT = NVB_WAVEX_THREADS;
 constexpr int kXG = kXT / 64;
@@ -93,9 +104,20 @@ constexpr int kRegionVox = 1100;
 constexpr int kFlagBase = 4 * kRegionVox;        // word offset of the flag plane
 constexpr int kXRegionWords = 5 * kRegionVox;    // 5 500 words = 22 000 bytes per group
 constexpr size_t kXSmemBytes = (size_t)kXG * kXRegionWords * sizeof(unsigned int);
+// Exchange-slab slot: the block's six faces (+x,-x,+y,-y,+z,-z), 64 voxels each in the order of the halo batches (face f, voxel
+// (c1, c2) of the two other axes in axis order at index f * 64 + c1 * 8 + c2), as a plane of 16-byte cells {squared distance,
+// parent} followed by a plane of flag words: 7.5 KiB instead of the layer's 10 KiB block, and the interior, which no halo
+// reads, is not written at all.
+constexpr int kXFaceCells = 6 * 64;
+constexpr int kXFlagOff = kXFaceCells * 16;           // byte offset of the flag plane in a slot
+constexpr int kXSlotBytes = kXFaceCells * (16 + 4);  // 7 680
+#if NVB_WAVEX_PROF
+constexpr int kXProfWords = 24;  // counters per group, copied to phase_max[kXProfBase ..] (tools/wavex_profile.py)
+constexpr int kXProfBase = 4000 - kXProfWords;
+#endif
 
 struct XTables {
-  unsigned int halo[8][64];     // halo voxel copies: dst voxel | src voxel in its block << 11 | d27 << 20 | valid << 25
+  unsigned int halo[8][64];     // halo voxel copies: dst voxel | src cell in its block's exchange-slab slot << 11 | d27 << 20 | valid << 25
   unsigned int pair[6][4][64];  // boundary pairs per pass: src voxel | dst voxel << 11 | d27 of the source block << 22 | inner << 27 | valid << 28
 };
 
@@ -125,8 +147,9 @@ struct XShared {
 #if NVB_WAVEX_PROF
   // per group, cycles: [0] record, [1] stamps (+ own block when not split; + speculative faces), [2] halo (+ the own block's
   // live planes when split), [3] replay, [4] sweep (+ registration), [5] stores; [6] candidates, [7] changed; [8] rest of
-  // the block (issue + registerBegin + wait; changed candidates); [9..11] [1] by K bin, [12..14] candidates by K bin
-  long long prof[kXG][16];
+  // the block (issue + registerBegin + wait; changed candidates); [9..11] [1] by K bin, [12..14] candidates by K bin,
+  // [15..17] [2] by K bin, [18..20] [5] by K bin
+  long long prof[kXG][kXProfWords];
 #endif
 };
 
@@ -190,20 +213,23 @@ __device__ __forceinline__ int neighbor6(const XCtx& c, int slot, int dir) {
 // Per-launch tables (the same for every candidate).
 __device__ __forceinline__ void initTables(XTables& tab, int tid) {
   // ---- halo copies. Batches 0..5: the six faces (+x,-x,+y,-y,+z,-z), one voxel per lane, so a batch is live or dead for the
-  // whole group; lanes follow the source block's memory order where its face is contiguous. Batches 6, 7: edges and corners.
+  // whole group; lane l of batch k reads cell l of the opposite face (k ^ 1) of its block's slot, so a batch is 1 KiB of
+  // contiguous cells and 256 bytes of contiguous flags. Batches 6, 7: edges and corners, each read from one face of its block
+  // that holds it (an edge voxel from the face across the first other axis, a corner from the x face).
   for (int i = tid; i < 512; i += kXT) {
     const int k = i >> 6, lane = i & 63;
     unsigned int e = 0;
     int ra = 1, r1 = 1, r2 = 1, axis = 0;  // region coordinates: along `axis`, and the two others in axis order
+    int fa = 0;                            // axis of the face the voxel is read from
     bool valid = true;
     if (k < 6) {
-      axis = k >> 1;
+      axis = k >> 1, fa = axis;
       ra = (k & 1) ? 0 : 9, r1 = (lane >> 3) + 1, r2 = (lane & 7) + 1;
     } else {
       const int n = i - 384;
       if (n < 96) {  // 12 edges x 8 voxels
         const int edge = n >> 3, cn = edge & 3;
-        axis = edge >> 2;
+        axis = edge >> 2, fa = axis == 0 ? 1 : 0;
         ra = (n & 7) + 1, r1 = (cn & 1) ? 9 : 0, r2 = (cn & 2) ? 9 : 0;
       } else if (n < 104) {
         const int cn = n - 96;
@@ -215,8 +241,10 @@ __device__ __forceinline__ void initTables(XTables& tab, int tid) {
     if (valid) {
       const int rx = axis == 0 ? ra : r1, ry = axis == 0 ? r1 : (axis == 1 ? ra : r2), rz = axis == 2 ? ra : r2;
       const int d = (boundaryOff(rx) + 1) * 9 + (boundaryOff(ry) + 1) * 3 + (boundaryOff(rz) + 1);
-      e = (unsigned)rvox(rx, ry, rz) | ((unsigned)(boundaryLoc(rx) * 64 + boundaryLoc(ry) * 8 + boundaryLoc(rz)) << 11) |
-          ((unsigned)d << 20) | (1u << 25);
+      const int lx = boundaryLoc(rx), ly = boundaryLoc(ry), lz = boundaryLoc(rz);  // voxel coordinates in block d
+      const int lf = fa == 0 ? lx : (fa == 1 ? ly : lz), l1 = fa == 0 ? ly : lx, l2 = fa == 2 ? ly : lz;  // on / across the face
+      const int cell = (2 * fa + (lf == 0 ? 1 : 0)) * 64 + l1 * 8 + l2;
+      e = (unsigned)rvox(rx, ry, rz) | ((unsigned)cell << 11) | ((unsigned)d << 20) | (1u << 25);
     }
     tab.halo[k][lane] = e;
   }
@@ -319,17 +347,26 @@ __device__ __forceinline__ void ownToShared(unsigned int* R, const OwnRegs& o, i
     R[kFlagBase + v0 + z] = ownWord(o, 5 * z + 4);
   }
 }
-// inner 8x8x8 of the region -> the block in the layer (if `to_layer`) and its copy in an exchange slab; half a z-row (four
-// voxels = 80 bytes = five 16-byte words) at a time. On the way the box of the BLOCK OFFSETS the voxels' parents point into is
-// collected and published in c.psum (EsdfCtx::psum; one word per warp of the group, so no barrier is needed): the clear pass of
-// later updates reads a candidate block only if that box contains a to-clear block.
-__device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer, unsigned char* x_blk, const unsigned int* R,
+// inner 8x8x8 of the region -> the block in the layer (if `to_layer`), half a z-row (four voxels = 80 bytes = five 16-byte words)
+// at a time, and its six faces -> its slot in an exchange slab, one cell and one flag word per lane and face. On the way the box
+// of the BLOCK OFFSETS the voxels' parents point into is collected and published in c.psum (EsdfCtx::psum; one word per warp of
+// the group, so no barrier is needed): the clear pass of later updates reads a candidate block only if that box contains a
+// to-clear block.
+__device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer, unsigned char* x_slot, const unsigned int* R,
                                          unsigned int* psum_slot, int lane64) {
   const uint4* A = reinterpret_cast<const uint4*>(R);
   const int x = lane64 >> 3, y = lane64 & 7;
   const int v0 = rvox(x + 1, y + 1, 1);
   uint4* dl = reinterpret_cast<uint4*>(layer_blk) + lane64 * 10;
-  uint4* dx = reinterpret_cast<uint4*>(x_blk) + lane64 * 10;
+  uint4* xc = reinterpret_cast<uint4*>(x_slot) + lane64;
+  unsigned int* xf = reinterpret_cast<unsigned int*>(x_slot + kXFlagOff) + lane64;
+#pragma unroll
+  for (int f = 0; f < 6; f++) {  // face f: region coordinate 8 (+) or 1 (-) along f's axis, lane = c1 * 8 + c2 (halo batch order)
+    const int fa = f >> 1, p = (f & 1) ? 1 : 8;
+    const int v = fa == 0 ? rvox(p, x + 1, y + 1) : (fa == 1 ? rvox(x + 1, p, y + 1) : rvox(x + 1, y + 1, p));
+    __stcg(xc + f * 64, A[v]);
+    __stcg(xf + f * 64, R[kFlagBase + v]);
+  }
   int lo0 = 99, lo1 = 99, lo2 = 99, hi0 = -99, hi1 = -99, hi2 = -99;
 #pragma unroll
   for (int h = 0; h < 2; h++) {
@@ -345,11 +382,8 @@ __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer
       }
     }
 #pragma unroll
-    for (int i = 0; i < 5; i++) {
-      const uint4 v = make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
-      if (to_layer) __stcg(dl + 5 * h + i, v);
-      __stcg(dx + 5 * h + i, v);
-    }
+    for (int i = 0; i < 5; i++)
+      if (to_layer) __stcg(dl + 5 * h + i, make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]));
   }
   if (psum_slot) {
     lo0 = __reduce_min_sync(0xffffffffu, lo0), lo1 = __reduce_min_sync(0xffffffffu, lo1), lo2 = __reduce_min_sync(0xffffffffu, lo2);
@@ -367,22 +401,28 @@ __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer
   }
 }
 
-// ---- halo voxels, as 4-byte cp.async copies straight into the two region planes: no registers are held across the wait (the
-// register version held up to 20 words per lane and spilled at 96 registers). By default only the batches of the members in
+// ---- halo voxels, as cp.async copies straight into the two region planes -- the 16-byte cell and the flag word of a voxel
+// from its block's exchange-slab slot: no registers are held across the wait (the register version held up to 20 words per
+// lane and spilled at 96 registers). By default only the batches of the members in
 // a live pair are fetched, after the stamps. With NVB_WAVEX_SPEC_HALO the face halo of every ALLOCATED face neighbour is issued
 // before the member stamps are known, with the own block and the stamps (one round trip after the record instead of two);
 // on the H100 the extra, mostly cold face fetches cost more than the round trip they save (DESIGN §9). Speculation is safe:
 // the replay reads a halo voxel only if its block is a live source (live[p] is a subset of the members) or a member destination (liveMasks), and the sweeps and the stores
 // touch the inner 8x8x8 only, so the voxels copied from a non-member's stale exchange-slab entry land in shared memory and are
-// never read. (.ca: 4-byte copies have no .cg form. The L1 lines they leave behind cannot go stale unnoticed: every grid
-// barrier ends with a __threadfence, which invalidates the SM's L1, and within the single-CTA tail the writer is this SM.)
+// never read. (The cells travel .cg, through L2 only. The flag words and the own block's words (ownAsync) are 4-byte copies,
+// which have no .cg form, so they go .ca. The L1 lines those leave behind cannot go stale unnoticed: every grid barrier ends
+// with an acquire (or a __threadfence), which invalidates the SM's L1, and within the single-CTA tail the writer is this SM.)
 __device__ __forceinline__ void cpAsync4(unsigned int* smem_dst, const unsigned int* gsrc) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned int)__cvta_generic_to_shared(smem_dst)), "l"(gsrc)
                : "memory");
 }
+__device__ __forceinline__ void cpAsyncCell(unsigned int* smem_dst, const void* gsrc) {  // 16 bytes, both 16-byte aligned
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned int)__cvta_generic_to_shared(smem_dst)), "l"(gsrc)
+               : "memory");
+}
 // ---- the own block split in two (grid rings, processCandidate): first the voxels on the boundary planes of
 // the axes `axes` (bit a: the planes 0 and 7 along axis a), which hold every voxel of B the replay reads or writes, then -- only
-// if B changed -- the rest. 4-byte copies like the halo's (the block's 20-byte voxels are not 16-byte aligned), one voxel per
+// if B changed -- the rest. 4-byte copies (the layer's 20-byte voxels are not 16-byte aligned), one voxel per
 // lane and x plane (lane = y * 8 + z: a warp's copies of one word cover 640 contiguous bytes). `planes`: copy the voxels on
 // those planes, else every other voxel. (.ca: the layer's blocks are written with .cg stores by the owners of earlier rings,
 // and the grid barrier between them and this read invalidates the SM's L1; the single-CTA tail does not fetch split.)
@@ -414,11 +454,10 @@ __device__ __forceinline__ void haloAsync(const XTables& tab, unsigned int* R, c
     const int d = (e >> 20) & 31u;
     const int slot = ((e >> 25) & 1u) && ((blocks >> d) & 1u) ? row[d] : -1;
     if (slot >= 0) {
-      const unsigned int* src = reinterpret_cast<const unsigned int*>(X + (size_t)slot * kEsdfBlockBytes) + ((e >> 11) & 511u) * kEsdfVoxelWords;
-      const int v = e & 2047u;
-#pragma unroll
-      for (int w = 0; w < 4; w++) cpAsync4(R + 4 * v + w, src + w);
-      cpAsync4(R + kFlagBase + v, src + 4);
+      const unsigned char* xslot = X + (size_t)slot * kXSlotBytes;
+      const int cell = (e >> 11) & 511u, v = e & 2047u;
+      cpAsyncCell(R + 4 * v, xslot + 16 * cell);
+      cpAsync4(R + kFlagBase + v, reinterpret_cast<const unsigned int*>(xslot + kXFlagOff) + cell);
     }
   }
 }
@@ -665,7 +704,7 @@ __device__ __noinline__ void processCandidate(int ring, int K) {
   if (rest) haloAsync(tab, R, row, c.X[ci], lane64, haloBatches(rest), rest);  // group-uniform
   if (rest || split) cpAsyncWaitAll();
   groupSync(group);  // (also publishes xs.live[group], written by lane 0 in liveMasks and read by every lane in replayX)
-  X_PROF(2)
+  X_PROF_KBIN(2, 15, K)
   const bool ch = replayX(tab, R, L, lane64, group, c.max_sq);
   if (ch) xs.changed[group] = 1;
   groupSync(group);
@@ -691,12 +730,12 @@ __device__ __noinline__ void processCandidate(int ring, int K) {
     registerClaim(c, xs, rs, group, lane64, ring + 1);
     groupSync(group);
     X_PROF(4)
-    ownStore(c.blocks + (size_t)slot * kEsdfBlockBytes, true, c.X[ni] + (size_t)slot * kEsdfBlockBytes, R, c.psum + 2 * (size_t)slot, lane64);
+    ownStore(c.blocks + (size_t)slot * kEsdfBlockBytes, true, c.X[ni] + (size_t)slot * kXSlotBytes, R, c.psum + 2 * (size_t)slot, lane64);
     registerFinish(c, xs, rs, group, lane64, c.segment(ni, cta));
     X_PROF_COUNT(7)
   }
   groupSync(group);
-  X_PROF(5)
+  X_PROF_KBIN(5, 18, K)
 }
 
 // A member of the initial list of a computeEsdf call (ring `ring`): sweep in place, publish, register its neighbours as
@@ -723,7 +762,7 @@ __device__ __noinline__ void processSeed(int ring, int slot) {
   if (ch) xs.changed[group] = 1;
   groupSync(group);
   // (an unchanged block keeps its parent box)
-  ownStore(blk, xs.changed[group] != 0, c.X[ci] + (size_t)slot * kEsdfBlockBytes, R, xs.changed[group] ? c.psum + 2 * (size_t)slot : nullptr, lane64);
+  ownStore(blk, xs.changed[group] != 0, c.X[ci] + (size_t)slot * kXSlotBytes, R, xs.changed[group] ? c.psum + 2 * (size_t)slot : nullptr, lane64);
   registerFinish(c, xs, rs, group, lane64, c.segment(ci, cta));
   groupSync(group);
 }
@@ -808,12 +847,12 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
     xc.blocks = c.esdf.blocks, xc.block_index = c.esdf.block_index, xc.hash = c.esdf.hash;
     xc.nbr = c.nbr, xc.nbr27 = c.nbr27, xc.cand_stamp = c.cand_stamp, xc.psum = c.psum;
     xc.stamp[0] = c.stamp_a, xc.stamp[1] = c.stamp_b;
-    xc.X[0] = c.xslab, xc.X[1] = c.xslab + (size_t)c.esdf.capacity * kEsdfBlockBytes;
+    xc.X[0] = c.xslab, xc.X[1] = c.xslab + (size_t)c.esdf.capacity * kXSlotBytes;
     xc.recs[0] = c.xrec, xc.recs[1] = c.xrec + (size_t)nctas * c.xseg * kRecInts;
     xc.seg = c.xseg, xc.split_min_k = c.xsplit_min_k, xc.error = c.error, xc.max_sq = c.max_sq;
   }
 #if NVB_WAVEX_PROF
-  if (lane64 < 16) xs.prof[group][lane64] = 0;
+  if (lane64 < kXProfWords) xs.prof[group][lane64] = 0;
 #endif
   __syncthreads();
 #if NVB_WAVEX_PROF
@@ -901,16 +940,17 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
         __syncthreads();
         continue;
       }
-      // ---- grid ring: candidates dealt round-robin over CTAs, then over the CTA's groups
+      // ---- grid ring: candidates dealt round-robin over CTAs, then over the CTA's groups. The loop reads K from xs.pre[nctas]
+      // (= K) rather than a register: whatever it keeps live across processCandidate is saved to the stack at every call.
       for (;;) {
         if (lane64 == 0) xs.cur[group] = atomicAdd(&xs.next, 1);
         groupSync(group);
         const long long e = (long long)cta + (long long)xs.cur[group] * nctas;
-        if (e >= K) break;
+        if (e >= xs.pre[nctas]) break;
         for (int s = lane64; s < nctas; s += 64)
           if (xs.pre[s] <= e && e < xs.pre[s + 1]) xs.seg[group][0] = s, xs.seg[group][1] = (int)e - xs.pre[s];
         groupSync(group);
-        processCandidate(xs.ring, K);
+        processCandidate(xs.ring, xs.pre[nctas]);
       }
       int K2, M2;
       X_BARRIER(1, K2, M2)
@@ -939,7 +979,7 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
     long long sum_max = 0;
     for (int q = 0; q < xs.n_bar && q < 1000; q++) sum_max += (long long)c.phase_max[q];
     c.stats[12] = sum_max;
-    for (int q = 0; q < 16; q++) c.phase_max[3984 + q] = xs.prof[0][q];
+    for (int q = 0; q < kXProfWords; q++) c.phase_max[kXProfBase + q] = xs.prof[0][q];
 #endif
   }
 }
@@ -952,6 +992,7 @@ int esdfWaveXGrid(int num_sms, int reserved_sms) {
   return grid;
 }
 size_t esdfWaveXFlagBytes() { return 2 * (size_t)kMaxCtas * sizeof(int2); }
+size_t esdfWaveXSlabBytes(int capacity) { return 2 * (size_t)capacity * kXSlotBytes; }
 
 // Grid rings with at least this many candidates fetch their candidates' own blocks split (processCandidate). 0: every grid
 // ring (K > 8; the single-CTA tail and the seeds fetch whole blocks). 80-frame c2 bench on one H100 SXM at a 700 W power

@@ -384,7 +384,8 @@ struct EsdfCtx {
   int* nbr27;         // 27 ints per ESDF slot: slot of the block at offset (dx,dy,dz), entry (dx+1)*9+(dy+1)*3+(dz+1);
                       // -1 none, < -1 unknown (never linked)
   unsigned char* shadow;  // second ESDF slab (same slot indexing): results of a ring wait here until all reads are done
-  unsigned char* xslab;   // exchange-slab wavefront: two ESDF slabs (ring parity), members' blocks as their neighbours' owners read them
+  unsigned char* xslab;   // exchange-slab wavefront: two slabs (ring parity) of per-slot block faces, members' faces as their
+                          // neighbours' owners read them (esdfWaveXSlabBytes)
   int* xtail;             // exchange-slab wavefront: 4 ints, hand-over of a single-CTA tail episode (rings advanced, K, M)
   int* xrec;              // exchange-slab wavefront: candidate records {slot, 27 neighbour slots, pad}, 32 ints; per ring parity one
                           // segment of `xseg` records per CTA
@@ -447,6 +448,7 @@ cudaError_t launchEsdfComputePersistent(const EsdfCtx& c, int num_sms, cudaStrea
 cudaError_t launchEsdfComputeX(const EsdfCtx& c, int num_sms, int reserved_sms, cudaStream_t stream, int* launches);  // nvb_esdf_wavex.cu
 int esdfWaveXGrid(int num_sms, int reserved_sms);  // CTAs of an exchange-slab launch
 size_t esdfWaveXFlagBytes();
+size_t esdfWaveXSlabBytes(int capacity);  // both exchange slabs: 2 x capacity x 7.5 KiB
 int esdfWaveXSplitMinK();  // kSplitMinK, or NVB_WAVEX_SPLIT_MIN_K (read at mapper creation)
 // Reference-like driver: one launch per phase, host reads the ring counter.
 cudaError_t runEsdfComputeHostLoop(const EsdfCtx& c, int num_sms, cudaStream_t stream, int* launches);

@@ -10,9 +10,10 @@ tests), runs bench.py's c2 frames through it with a synchronise after every upda
             when not split); halo (+ the own block's live planes when split); replay; rest of block (changed candidates:
             issue + registration atomics + wait); sweep (+ registration); stores + records), the stamps stage binned by
             the ring's candidate count K (<= 256, <= 1 040, > 1 040) with the candidates per bin, its candidate / changed
-            counts, and the launch's split candidates and rest-of-block fetches (esdf_integrator().last_stats())
+            counts, the halo and stores stages binned the same way, and the launch's split candidates and rest-of-block
+            fetches (esdf_integrator().last_stats())
   summary : totals per phase kind, a least-squares line of the grid rings' slowest-CTA work time against K, the stage
-            shares, the stamps stage per K bin, and the barrier time = wavefront stage time - summed work maxima
+            shares, the stamps, halo and stores stages per K bin, and the barrier time = wavefront stage time - summed work maxima
 
 The profiling counters cost registers (and spills), so the absolute times of this build are inflated: quote its SHARES, and
 take absolute times from the normal build (bench.py's `stages`). The card's name and power limit are recorded alongside.
@@ -32,7 +33,8 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 STAGE_KEYS = ("record", "stamps_own_block", "halo", "replay", "sweep", "stores_records")
-PROF_BASE = 3984  # NVB_WAVEX_PROF words of debug_phase_max: 16 counters of CTA 0's group 0 (XShared::prof)
+PROF_WORDS = 24  # NVB_WAVEX_PROF counters of CTA 0's group 0 (XShared::prof), the last words of debug_phase_max
+PROF_BASE = 4000 - PROF_WORDS
 K_BINS = ("k_le_256", "k_le_1040", "k_gt_1040")
 KIND_TAIL_MAX_K = 8  # rings with at most one candidate per 64-thread group of one CTA run as a single-CTA tail
 
@@ -95,10 +97,12 @@ def main():
                     k = int(pm[1000 + q])
                     phases.append({"frame": i, "phase": q, "kind": phase_kind(k), "K": k, "M": int(pm[2000 + q]),
                                    "max_work_ns": int(pm[q]), "cta0_work_ns": int(pm[3000 + q])})
-                p = pm[PROF_BASE:PROF_BASE + 16]
+                p = pm[PROF_BASE:PROF_BASE + PROF_WORDS]
                 s = {key: int(p[j]) for j, key in enumerate(STAGE_KEYS)}
                 s.update(frame=i, candidates=int(p[6]), changed=int(p[7]), rest_of_block=int(p[8]),
                          stamps_own_block_by_k={b: int(p[9 + j]) for j, b in enumerate(K_BINS)},
+                         halo_by_k={b: int(p[15 + j]) for j, b in enumerate(K_BINS)},
+                         stores_records_by_k={b: int(p[18 + j]) for j, b in enumerate(K_BINS)},
                          candidates_by_k={b: int(p[12 + j]) for j, b in enumerate(K_BINS)})
                 st = m.esdf_integrator().last_stats()
                 s.update(split_candidates=int(st["split_candidates"]), rest_fetches=int(st["rest_fetches"]))
@@ -133,11 +137,14 @@ def main():
     if len(grid) >= 2:
         slope, icpt = np.polyfit([k for k, _ in grid], [t for _, t in grid], 1)
         fit = {"rings": len(grid), "ns_per_candidate": float(slope), "ns_at_k0": float(icpt)}
-    by_k = {}
-    for b in K_BINS:
-        n = sum(s["candidates_by_k"][b] for s in stages)
-        c = sum(s["stamps_own_block_by_k"][b] for s in stages)
-        by_k[b] = {"candidates": n, "cycles_per_candidate": c / n if n else None}
+
+    def by_k(stage):  # cycles per candidate of a stage, per K bin
+        r = {}
+        for b in K_BINS:
+            n = sum(s["candidates_by_k"][b] for s in stages)
+            c = sum(s[stage][b] for s in stages)
+            r[b] = {"candidates": n, "cycles_per_candidate": c / n if n else None}
+        return r
     summary = {
         "frames": F,
         "wavefront_us_per_frame": wave_us,
@@ -148,7 +155,9 @@ def main():
         "group0_stage_share": {k: v / tot for k, v in cyc.items()},
         "group0_cycles_per_candidate": {k: v / max(cands, 1) for k, v in cyc.items()},
         "group0_rest_of_block_cycles_per_changed": cyc["rest_of_block"] / max(changed, 1),
-        "group0_stamps_own_block_by_k": by_k,
+        "group0_stamps_own_block_by_k": by_k("stamps_own_block_by_k"),
+        "group0_halo_by_k": by_k("halo_by_k"),
+        "group0_stores_records_by_k": by_k("stores_records_by_k"),
         "group0_candidates": cands,
         "group0_changed": changed,
         "split_candidates_per_frame": sum(s["split_candidates"] for s in stages) / max(F, 1),
