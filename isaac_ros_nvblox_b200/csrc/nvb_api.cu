@@ -177,7 +177,6 @@ struct NvbMapper {
   int* esdf_ints = nullptr;  // small counters block
   int* upd_list = nullptr;
   int* clr_list = nullptr;
-  int* clr_cand = nullptr;  // candidates of the clear pass that survive the pruning (select kernel -> process kernel)
   int* cleared_list = nullptr;
   int* ring_a = nullptr;
   int* ring_b = nullptr;
@@ -415,7 +414,6 @@ int allocEsdfScratch(NvbMapper* m, int old_cap, int cap) {
   if ((rc = reallocCopy(&m->work, 0, (size_t)cap, false, m->stream))) return rc;
   if ((rc = reallocCopy(&m->upd_list, 0, (size_t)cap, false, m->stream))) return rc;
   if ((rc = reallocCopy(&m->clr_list, 0, (size_t)cap, false, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->clr_cand, 0, (size_t)cap, false, m->stream))) return rc;
   if ((rc = reallocCopy(&m->cleared_list, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
   if ((rc = reallocCopy(&m->ring_a, 0, (size_t)cap, false, m->stream))) return rc;
   if ((rc = reallocCopy(&m->ring_b, 0, (size_t)cap, false, m->stream))) return rc;
@@ -490,7 +488,7 @@ constexpr int kHostListCap = 1 << 15;  // entries of the pinned frame-list buffe
 
 // esdf_ints layout
 enum { kWorkCount = 0, kUpdCount = 1, kClrCount = 2, kClrAabb = 3, kClearedCount = 9, kRingCount = 10, kRingId = 14,
-       kTodoCount = 15, kFrameCount = 16, kError = 17, kClearedSeq = 18, kTailState = 20, kDeadCount = 22, kDeadClearedCount = 23, kGesCounts = 24, kTodoFsCount = 28, kFsWorkCount = 29, kColsCount = 30, kColorWorkCount = 31, kXTail = 32, kTodoMeshCount = 36, kClrCandCount = 37, kNumInts = 40 };
+       kTodoCount = 15, kFrameCount = 16, kError = 17, kClearedSeq = 18, kTailState = 20, kDeadCount = 22, kDeadClearedCount = 23, kGesCounts = 24, kTodoFsCount = 28, kFsWorkCount = 29, kColsCount = 30, kColorWorkCount = 31, kXTail = 32, kTodoMeshCount = 36, kNumInts = 40 };
 
 float logOddsFromProbability(float p);
 
@@ -503,7 +501,6 @@ EsdfCtx makeEsdfCtx(NvbMapper* m) {
   c.work_count = m->esdf_ints + kWorkCount;
   c.upd_list = m->upd_list, c.upd_count = m->esdf_ints + kUpdCount;
   c.clr_list = m->clr_list, c.clr_count = m->esdf_ints + kClrCount;
-  c.clr_cand = m->clr_cand, c.clr_cand_count = m->esdf_ints + kClrCandCount;
   c.clr_aabb = m->esdf_ints + kClrAabb;
   c.cleared_list = m->cleared_list, c.cleared_count = m->esdf_ints + kClearedCount;
   c.ring_a = m->ring_a, c.ring_b = m->ring_b;
@@ -1162,7 +1159,8 @@ int enqueueEsdf(NvbMapper* m, const int* in_xyz_dev, int n_explicit, bool from_t
     NVB_CUDA(cudaEventRecord(m->mark_done, es));
     NVB_CUDA(cudaStreamWaitEvent(m->stream, m->mark_done, 0));
     beginStageOn(m, 4, es);
-    m->launches += launchEsdfClear(c, m->esdf.capacity, m->num_sms, es);
+    launchEsdfClear(c, m->esdf.capacity, m->num_sms, es);
+    m->launches++;
     endStageOn(m, es);
     beginStageOn(m, 5, es);
     e = m->esdf_persistent == 3   ? launchEsdfComputeX(c, m->num_sms, m->esdf_reserved_sms, es, &launches)
@@ -1179,7 +1177,8 @@ int enqueueEsdf(NvbMapper* m, const int* in_xyz_dev, int n_explicit, bool from_t
     allocAndMark(m->stream);
     endStage(m);
     beginStage(m, 4);
-    m->launches += launchEsdfClear(c, m->esdf.capacity, m->num_sms, m->stream);
+    launchEsdfClear(c, m->esdf.capacity, m->num_sms, m->stream);
+    m->launches++;
     endStage(m);
     beginStage(m, 5);
     e = runEsdfComputeHostLoop(c, m->num_sms, m->stream, &launches);
@@ -1382,7 +1381,7 @@ void nvb_mapper_destroy(NvbMapper* m) {
     cudaEventDestroy(m->stage_copied[k]), cudaEventDestroy(m->stage_consumed[k]);
   }
   cudaFree(m->dirty), cudaFree(m->todo_slots);
-  cudaFree(m->work), cudaFree(m->esdf_ints), cudaFree(m->upd_list), cudaFree(m->clr_list), cudaFree(m->clr_cand), cudaFree(m->cleared_list);
+  cudaFree(m->work), cudaFree(m->esdf_ints), cudaFree(m->upd_list), cudaFree(m->clr_list), cudaFree(m->cleared_list);
   cudaFree(m->ring_a), cudaFree(m->ring_b), cudaFree(m->stamp_a), cudaFree(m->stamp_b);
   cudaFree(m->nbr), cudaFree(m->seed_upd), cudaFree(m->seed_clr), cudaFree(m->psum);
   cudaFree(m->nbr27), cudaFree(m->shadow), cudaFree(m->cand_stamp), cudaFree(m->cand_a), cudaFree(m->cand_b);

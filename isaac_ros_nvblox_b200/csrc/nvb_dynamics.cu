@@ -48,8 +48,7 @@ __device__ __forceinline__ bool detectPixel(const DynamicsArgs& a, int pix) {
   const int vy = min(floatToIntRz((p.y - a.block_size * (float)b.y) * a.voxel_size_inv), kVps - 1);
   const int vz = min(floatToIntRz((p.z - a.block_size * (float)b.z) * a.voxel_size_inv), kVps - 1);
   const int v = (vx * kVps + vy) * kVps + vz;
-  // FreespaceVoxel::is_high_confidence_freespace: byte 16 of the 24-byte voxel
-  const bool dyn = a.fs.blocks[(size_t)slot * kFreespaceBlockBytes + (size_t)v * kFreespaceVoxelBytes + 16] != 0;
+  const bool dyn = isVoxelFreespace(a.fs, slot, v);  // FreespaceVoxel::is_high_confidence_freespace
   // getOverlayColor (:26-34): red for dynamics, grey scaled by depth
   constexpr float kMaxDisplayDepthM = 10.f;
   constexpr float kDepthScaleFactor = 255.0f / kMaxDisplayDepthM;

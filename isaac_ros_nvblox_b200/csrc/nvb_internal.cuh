@@ -412,8 +412,6 @@ struct EsdfCtx {
   unsigned int* psum; // two words per slot (the two halves of the block, x < 4 and x >= 4): 0 = no voxel has a parent; bit 31 set: box of the BLOCK OFFSETS the voxels' parents
                       // point into, 5 bits per bound (lo x, hi x, lo y, hi y, lo z, hi z, each + 16); 0xffffffff = unknown.
                       // An upper bound kept by the exchange-slab wavefront (the only writer of non-zero parents in that mode).
-  int* clr_cand;        // clear pass: candidates that survive the pruning, and their count
-  int* clr_cand_count;
   unsigned int* clr_bits;  // bitmap of the to-clear blocks over their AABB (2048 words), built by the mark kernel's last CTA
   int prune;          // clear pass: skip candidates whose parent box holds no to-clear block (exact: a voxel is cleared iff its
                       // parent voxel lost its site flag, and sites are only lost in to-clear blocks)
@@ -441,7 +439,7 @@ void launchEsdfSliceAllocateAndMark(const EsdfCtx& c, const int* in_xyz, const i
 void launchEsdfAllocate(const EsdfCtx& c, const int* in_xyz, const int* in_slots, const int* in_count_dev,
                         int in_count_upper, cudaStream_t stream);
 void launchEsdfMark(const EsdfCtx& c, int count_upper, int num_sms, cudaStream_t stream);
-int launchEsdfClear(const EsdfCtx& c, int esdf_count_upper, int num_sms, cudaStream_t stream);  // returns the number of launches
+void launchEsdfClear(const EsdfCtx& c, int esdf_count_upper, int num_sms, cudaStream_t stream);
 // Whole wavefront (both computeEsdf calls) in one cooperative launch. Returns cudaError.
 cudaError_t launchEsdfComputeGes(const EsdfCtx& c, int num_sms, cudaStream_t stream, int* launches);
 cudaError_t launchEsdfComputePersistent(const EsdfCtx& c, int num_sms, cudaStream_t stream, int* launches);
@@ -456,6 +454,13 @@ int esdfPersistentMaxCtas(int num_sms);
 
 constexpr int kFreespaceVoxelBytes = 24;
 constexpr int kFreespaceBlockBytes = 512 * kFreespaceVoxelBytes;  // 12 288
+#ifdef __CUDACC__
+// FreespaceVoxel::is_high_confidence_freespace (byte 16 of the 24-byte voxel) of voxel v of the freespace block in `slot`;
+// false if there is no block (slot < 0), like isVoxelFreespace (esdf_integrator.cu:101-111).
+__device__ __forceinline__ bool isVoxelFreespace(const DevLayer& layer, int slot, int v) {
+  return slot >= 0 && layer.blocks[(size_t)slot * kFreespaceBlockBytes + (size_t)v * kFreespaceVoxelBytes + 16] != 0;
+}
+#endif
 // nvb_tsdf.cu: freespace (FreespaceIntegrator, integrators/internal/cuda/impl/freespace_integrator_impl.cuh)
 struct FreespaceArgs {
   DevLayer tsdf, fs;

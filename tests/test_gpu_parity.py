@@ -384,10 +384,10 @@ def test_esdf_clear_pass_pruning_is_exact(gpu, monkeypatch, prune):
     m.close()
 
 
-@pytest.mark.parametrize("mark_tma", ["1", "0"])
-def test_esdf_small_grids_exercise_multi_round_paths(gpu, mark_tma):
-    """Runs in a subprocess with NVB_ESDF_GRID_CAP=3 (the cap is read once per process): three CTAs mark ~1000 blocks
-    each (per-CTA lists flush when full) and the clear kernel needs several selection rounds of 256 slots per CTA."""
+def test_esdf_small_grids_exercise_multi_round_paths(gpu):
+    """Runs in a subprocess with NVB_ESDF_GRID_CAP=3 (the cap is read once per process): three CTAs of esdfMarkTmaKernel
+    mark ~1000 blocks each (per-CTA lists flush when full) and esdfClearKernel needs several selection rounds of 256
+    slots per CTA. (The plain-staged esdfMarkKernel on a capped grid: test_gpu_scale_edges_f.py, with freespace.)"""
     import subprocess, sys, textwrap
     code = textwrap.dedent("""
         import sys
@@ -410,8 +410,7 @@ def test_esdf_small_grids_exercise_multi_round_paths(gpu, mark_tma):
         m.close()
         print("ok")
     """) % (os.path.dirname(os.path.abspath(__file__)), os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    # (the second variant also runs the clear pass as two kernels, select + balanced process: NVB_CLEAR_SPLIT=1)
-    env = dict(os.environ, NVB_ESDF_GRID_CAP="3", NVB_MARK_TMA=mark_tma, NVB_CLEAR_SPLIT="0" if mark_tma == "1" else "1")
+    env = dict(os.environ, NVB_ESDF_GRID_CAP="3")
     r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=600)
     assert r.returncode == 0 and "ok" in r.stdout, r.stdout + r.stderr
 
