@@ -60,6 +60,19 @@ class VoxelBlockLayer {
     *out = b->voxels[voxel_idx[0]][voxel_idx[1]][voxel_idx[2]];
     return true;
   }
+  // VoxelBlockLayer::getVoxels (map/layer.h:265-276): the voxel holding each position and whether its block exists. Runs on
+  // the GPU (nvb_layer_query_voxels); a missing voxel is VoxelType{}.
+  void getVoxels(const std::vector<Vector3f>& positions_L, std::vector<VoxelType>* voxels_ptr,
+                 std::vector<bool>* success_flags_ptr) const {
+    const size_t n = positions_L.size();
+    std::vector<float> xyz(n * 3);
+    for (size_t i = 0; i < n; i++) xyz[3 * i] = positions_L[i][0], xyz[3 * i + 1] = positions_L[i][1], xyz[3 * i + 2] = positions_L[i][2];
+    voxels_ptr->assign(n, VoxelType{});
+    std::vector<uint8_t> ok(n, 0);
+    b200_detail::check(nvb_layer_query_voxels(m_, id_, xyz.data(), NVB_MEM_HOST, (int64_t)n, voxels_ptr->data(), ok.data()),
+                       "getVoxels", nvb_last_error());
+    success_flags_ptr->assign(ok.begin(), ok.end());
+  }
  // The mapper this layer belongs to (DynamicsDetection::computeDynamics runs on the owner of its FreespaceLayer).
   NvbMapper* c_abi() const { return m_; }
  private:

@@ -676,6 +676,48 @@ NVB_API int32_t nvb_layer_block_device_ptr(NvbMapper* m, int32_t layer, const in
                                            void** out_ptr);
 NVB_API int32_t nvb_layer_block_bytes(int32_t layer);
 
+/* ---- Point queries: the map read at arbitrary points on the GPU. A query reads the map and never writes it.
+ * Points are n x 3 floats (x, y, z); spheres n x 4 floats (x, y, z, radius). A point's voxel is the one
+ * getBlockAndVoxelIndexFromPositionInLayer names (C/include/nvblox/core/internal/impl/indexing_impl.h:37-49).
+ * Deviations from the reference, whose behaviour on these inputs is undefined or accidental:
+ *  - a point with a non-finite coordinate, or whose block index lies outside the hash's +-2^20 key range, is a miss;
+ *  - the mappers of one nvb_query_* call must be on the same device (NVB_ERR_INVALID_ARGUMENT otherwise).
+ * Ordering: a query runs after all work already enqueued on every mapper it reads (including a pending ESDF update), and
+ * each of those mappers' later work runs after the query. With device buffers nothing synchronises the host: the waits are
+ * event hops. n == 0 launches nothing; a bad layer or a null pointer is NVB_ERR_INVALID_ARGUMENT. */
+/* VoxelBlockLayer::getVoxels / getVoxelsGPU (C/include/nvblox/map/layer.h:265-295, map/internal/cuda/impl/layer_impl.cuh:29-80)
+ * on any voxel layer (TSDF, ESDF, occupancy, freespace, colour): out_voxels receives n voxels as stored (NvbTsdfVoxel,
+ * NvbEsdfVoxel, float log-odds, NvbFreespaceVoxel, NvbColorVoxel), written only where out_success[i] = 1. All three buffers
+ * are in `memory`; host buffers are written when the call returns, device ones are enqueued on the mapper's stream. */
+NVB_API int32_t nvb_layer_query_voxels(NvbMapper* m, int32_t layer, const float* xyz, int32_t memory, int64_t n,
+                                       void* out_voxels, uint8_t* out_success);
+/* interpolation::interpolateOnCPU (C/src/interpolation/interpolation_3d.cpp) of the TSDF, ESDF or occupancy layer, on the GPU:
+ * trilinear interpolation of the 8 voxels around each point (the low corner is the voxel of p - voxel_size / 2; they may lie
+ * in up to 8 blocks). TSDF: `distance`, every voxel needs weight > 1e-4. ESDF: sqrt(squared_distance_vox) -- unsigned and in
+ * voxels, as in the reference --, every voxel needs `observed`. Occupancy: the probability exp(l) / (1 + exp(l)). A point
+ * fails (out_success 0, value 0) when a block is missing or a voxel is invalid. The weighted sum q . (T . m) runs left to
+ * right over the non-zero entries of the reference's 8x8 table. Buffers in `memory`, as nvb_layer_query_voxels. */
+NVB_API int32_t nvb_layer_interpolate(NvbMapper* m, int32_t layer, const float* xyz, int32_t memory, int64_t n,
+                                      float* out_values, uint8_t* out_success);
+/* nvblox_torch's ESDF sphere query (nvblox_torch/cpp/src/sdf_query.cu:63-205) over the ESDF layers of num_mappers mappers
+ * (at most 16). Device buffers. out is n x 4 {gx, gy, gz, d} with_gradient, else n x 1 {d}. Per mapper holding the sphere's
+ * voxel: unobserved -> d = 100; else distance = +-voxel_size * sqrt(squared_distance_vox) (negative inside), d = distance -
+ * radius, gradient = (-voxel_size / distance) * parent_direction, or 0 when distance <= 1e-6. With several mappers the
+ * minimum is kept from 100 down: a mapper whose d exceeds the running minimum writes that minimum and leaves the gradient.
+ * Outputs a sphere never writes keep their contents (the caller pre-fills them, nvblox_torch uses 100). The query is
+ * enqueued on caller_stream (a cudaStream_t; NULL is the default stream, as in CUDA): it also runs after the work already
+ * there, and that stream's next work follows it. One mapper takes the single-mapper rules (no minimum). */
+NVB_API int32_t nvb_query_esdf(NvbMapper* const* mappers, int32_t num_mappers, const float* spheres_xyzr, int64_t n,
+                               int32_t with_gradient, float* out, void* caller_stream);
+/* nvblox_torch's TSDF point query (sdf_query.cu:240-318): out n x 2 {distance, weight}. One mapper: written where the voxel
+ * exists. Several: the smallest distance and the weight at it, starting from {100, 0}. Ordering as nvb_query_esdf. */
+NVB_API int32_t nvb_query_tsdf(NvbMapper* const* mappers, int32_t num_mappers, const float* xyz, int64_t n, float* out,
+                               void* caller_stream);
+/* nvblox_torch's occupancy point query (sdf_query.cu:320-351) over the mappers' occupancy layers: out n x 1, the largest
+ * log-odds of the voxels that exist, starting from logOddsFromProbability(0). Ordering as nvb_query_esdf. */
+NVB_API int32_t nvb_query_occupancy(NvbMapper* const* mappers, int32_t num_mappers, const float* xyz, int64_t n, float* out,
+                                    void* caller_stream);
+
 /* Counters of the last ESDF update (for the roofline's algorithmic bytes):
  * [0] blocks marked, [1] blocks with sites, [2] blocks to clear, [3] clear-pass
  * candidate blocks, [4] blocks cleared, [5] swept blocks, [6] (block,direction)

@@ -49,6 +49,7 @@ EXPORTED_SYMBOLS = [
     "nvb_mapper_compute_ground_plane", "nvb_mapper_ground_plane", "nvb_mapper_ground_plane_points", "nvb_ransac_fit_plane",
     "nvb_mapper_compute_dynamics", "nvb_mapper_remove_small_components", "nvb_mapper_dynamic_mask", "nvb_mapper_dynamic_overlay",
     "nvb_mapper_dynamic_points", "nvb_mapper_dynamics_device_buffers", "nvb_mapper_wait_for",
+    "nvb_layer_query_voxels", "nvb_layer_interpolate", "nvb_query_esdf", "nvb_query_tsdf", "nvb_query_occupancy",
 ]
 
 
@@ -307,6 +308,12 @@ def load(path=None):
     L.nvb_mapper_dynamic_points.argtypes = [vp, vp, i32, i32, ip]
     L.nvb_mapper_dynamics_device_buffers.argtypes = [vp, C.POINTER(NvbDynamicsBuffers)]
     L.nvb_mapper_wait_for.argtypes = [vp, vp]
+    i64 = C.c_int64
+    L.nvb_layer_query_voxels.argtypes = [vp, i32, vp, i32, i64, vp, vp]
+    L.nvb_layer_interpolate.argtypes = [vp, i32, vp, i32, i64, vp, vp]
+    L.nvb_query_esdf.argtypes = [C.POINTER(vp), i32, vp, i64, i32, vp, vp]
+    L.nvb_query_tsdf.argtypes = [C.POINTER(vp), i32, vp, i64, vp, vp]
+    L.nvb_query_occupancy.argtypes = [C.POINTER(vp), i32, vp, i64, vp, vp]
     L.nvb_mapper_kernel_launches.restype = C.c_int64
     for name in EXPORTED_SYMBOLS:
         f = getattr(L, name)

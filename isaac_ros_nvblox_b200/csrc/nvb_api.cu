@@ -12,6 +12,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <set>
 #include <string>
 #include <vector>
@@ -253,6 +254,7 @@ struct NvbMapper {
   unsigned char* cc_stage = nullptr;  // host masks staged for the filter (input, then output)
   int cc_stage_cap = 0;
   cudaEvent_t dyn_event = nullptr;    // nvb_mapper_wait_for: recorded on this mapper's stream
+  cudaEvent_t query_event = nullptr;  // point queries (nvb_query_*): the hand-over between this mapper and the query's stream
   // last integrated view (Mapper::last_posed_depth_image_, mapper.h:830-833), kept when keep_last_view is set
   int keep_last_view = 0;
   float* last_depth = nullptr;
@@ -1395,6 +1397,7 @@ void nvb_mapper_destroy(NvbMapper* m) {
   cudaFree(m->dyn_depth), cudaFree(m->dyn_mask), cudaFree(m->dyn_clean), cudaFree(m->dyn_overlay), cudaFree(m->dyn_points);
   cudaFree(m->dyn_counts), cudaFree(m->dyn_totals), cudaFree(m->cc_labels), cudaFree(m->cc_sizes), cudaFree(m->cc_stage);
   if (m->dyn_event) cudaEventDestroy(m->dyn_event);
+  if (m->query_event) cudaEventDestroy(m->query_event);
   cudaFree(m->union_list), cudaFree(m->union_list_count);
   if (m->mesh.blocks) freeLayer(&m->mesh);
   cudaFree(m->mesh_v), cudaFree(m->mesh_n), cudaFree(m->mesh_t), cudaFree(m->mesh_c), cudaFree(m->mesh_state);
@@ -3691,6 +3694,183 @@ int32_t nvb_mesh_arena_stats(NvbMapper* m, int64_t out[4]) {
   NVB_CUDA(cudaMemcpy(state, m->mesh_state, sizeof(state), cudaMemcpyDeviceToHost));
   out[1] = state[kArenaUsed], out[2] = state[kArenaLastTotal], out[3] = state[kArenaGarbage];
   return NVB_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------
+// Point queries (nvb_query.cu)
+// ---------------------------------------------------------------------------
+namespace {
+
+constexpr long long kMaxQueryPoints = 1ll << 40;
+
+QueryLayer queryLayerOf(const NvbMapper* m, const DevLayer& L) {
+  QueryLayer q;
+  q.layer = L;
+  q.block_size = m->block_size;
+  q.voxel_size = m->voxel_size;
+  q.voxel_size_inv = voxelSizeInv(m->block_size);
+  return q;
+}
+
+// Orders a query on `qs` between the mappers' work: it runs after everything already enqueued on each mapper (its stream and
+// a pending ESDF wavefront), and each mapper's later work runs after it. Device-side event hops only.
+template <typename Launch>
+int runOrdered(NvbMapper* const* ms, int k, cudaStream_t qs, Launch launch) {
+  for (int i = 0; i < k; i++) {
+    NvbMapper* m = ms[i];
+    if (!m->query_event) NVB_CUDA(cudaEventCreateWithFlags(&m->query_event, cudaEventDisableTiming));
+    if (m->esdf_in_flight) NVB_CUDA(cudaStreamWaitEvent(qs, m->esdf_done, 0));
+    if (m->stream != qs) {
+      NVB_CUDA(cudaEventRecord(m->query_event, m->stream));
+      NVB_CUDA(cudaStreamWaitEvent(qs, m->query_event, 0));
+    }
+  }
+  launch(qs);
+  NVB_CUDA(cudaGetLastError());
+  for (int i = 0; i < k; i++) {
+    NvbMapper* m = ms[i];
+    m->launches++;
+    if (m->stream == qs) continue;
+    NVB_CUDA(cudaEventRecord(m->query_event, qs));
+    NVB_CUDA(cudaStreamWaitEvent(m->stream, m->query_event, 0));
+  }
+  return NVB_OK;
+}
+
+// A per-layer query (nvb_layer_query_voxels, nvb_layer_interpolate) on the mapper's stream. Host buffers are staged on the
+// device and the call returns when the outputs are written back; device buffers are enqueued without synchronising.
+// launch(xyz_dev, out_dev, flags_dev, stream)
+template <typename Launch>
+int runLayerQuery(NvbMapper* m, const float* xyz, int32_t memory, long long n, void* out, size_t out_bytes_per_point,
+                  uint8_t* flags, Launch launch) {
+  NVB_CUDA(cudaSetDevice(m->device));
+  if (memory == NVB_MEM_DEVICE) return runOrdered(&m, 1, m->stream, [&](cudaStream_t st) { launch(xyz, out, flags, st); });
+  float* xyz_dev = nullptr;
+  unsigned char *out_dev = nullptr, *flags_dev = nullptr;
+  auto release = [&]() { cudaFree(xyz_dev), cudaFree(out_dev), cudaFree(flags_dev); };
+  if (cudaMalloc(&xyz_dev, (size_t)n * 3 * sizeof(float)) != cudaSuccess ||
+      cudaMalloc(&out_dev, (size_t)n * out_bytes_per_point) != cudaSuccess || cudaMalloc(&flags_dev, (size_t)n) != cudaSuccess) {
+    release();
+    return fail(NVB_ERR_CUDA, "cudaMalloc of the query's staging buffers failed");
+  }
+  int rc = NVB_OK;
+  cudaError_t e = cudaMemcpyAsync(xyz_dev, xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, m->stream);
+  // the caller's buffer goes down too: the outputs the kernel does not write come back unchanged
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_dev, out, (size_t)n * out_bytes_per_point, cudaMemcpyHostToDevice, m->stream);
+  if (e == cudaSuccess)
+    rc = runOrdered(&m, 1, m->stream, [&](cudaStream_t st) { launch(xyz_dev, out_dev, flags_dev, st); });
+  if (e == cudaSuccess && rc == NVB_OK)
+    e = cudaMemcpyAsync(out, out_dev, (size_t)n * out_bytes_per_point, cudaMemcpyDeviceToHost, m->stream);
+  if (e == cudaSuccess && rc == NVB_OK) e = cudaMemcpyAsync(flags, flags_dev, (size_t)n, cudaMemcpyDeviceToHost, m->stream);
+  if (e == cudaSuccess && rc == NVB_OK) e = cudaStreamSynchronize(m->stream);
+  release();
+  if (rc != NVB_OK) return rc;
+  if (e != cudaSuccess) return fail(NVB_ERR_CUDA, std::string("point query: ") + cudaGetErrorString(e));
+  return NVB_OK;
+}
+
+int checkLayerQueryArgs(NvbMapper* m, const float* xyz, int32_t memory, int64_t n, const void* out, const void* flags) {
+  if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
+  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (n < 0 || n > kMaxQueryPoints) return fail(NVB_ERR_INVALID_ARGUMENT, "bad number of query points");
+  if (n > 0 && (!xyz || !out || !flags)) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  return NVB_OK;
+}
+
+// The layers of a multi-mapper device query (nvb_query_*), all on one device.
+int gatherQueryLayers(NvbMapper* const* mappers, int32_t num_mappers, int32_t layer, int64_t n, const void* in, const void* out,
+                      QueryLayers* q) {
+  if (!mappers || num_mappers < 1) return fail(NVB_ERR_INVALID_ARGUMENT, "no mappers to query");
+  if (num_mappers > kMaxQueryMappers) return fail(NVB_ERR_INVALID_ARGUMENT, "at most 16 mappers per query");
+  if (n < 0 || n > kMaxQueryPoints) return fail(NVB_ERR_INVALID_ARGUMENT, "bad number of query points");
+  if (n > 0 && (!in || !out)) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  q->n = num_mappers;
+  for (int i = 0; i < num_mappers; i++) {
+    NvbMapper* m = mappers[i];
+    if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
+    if (m->device != mappers[0]->device) return fail(NVB_ERR_INVALID_ARGUMENT, "the mappers of one query must share a device");
+    const DevLayer* L = layerOf(m, layer);
+    if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "a mapper of the query has no such layer");
+    q->l[i] = queryLayerOf(m, *L);
+  }
+  return NVB_OK;
+}
+
+int runMapperQuery(NvbMapper* const* mappers, int32_t num_mappers, int64_t n, void* caller_stream,
+                   const std::function<void(cudaStream_t)>& launch) {
+  if (n == 0) return NVB_OK;
+  NVB_CUDA(cudaSetDevice(mappers[0]->device));
+  return runOrdered(mappers, num_mappers, static_cast<cudaStream_t>(caller_stream), launch);
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t nvb_layer_query_voxels(NvbMapper* m, int32_t layer, const float* xyz, int32_t memory, int64_t n, void* out_voxels,
+                               uint8_t* out_success) {
+  int rc = checkLayerQueryArgs(m, xyz, memory, n, out_voxels, out_success);
+  if (rc) return rc;
+  if (layer == NVB_LAYER_MESH) return fail(NVB_ERR_INVALID_ARGUMENT, "the mesh layer has no voxels");
+  DevLayer* L = layerOf(m, layer);
+  if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "unknown layer");
+  if (n == 0) return NVB_OK;
+  const QueryLayer q = queryLayerOf(m, *L);
+  const int voxel_bytes = L->block_bytes / kVpb;
+  return runLayerQuery(m, xyz, memory, n, out_voxels, (size_t)voxel_bytes, out_success,
+                       [&](const float* x, void* o, uint8_t* f, cudaStream_t st) {
+                         launchQueryVoxels(q, voxel_bytes, x, n, o, f, m->num_sms, st);
+                       });
+}
+
+int32_t nvb_layer_interpolate(NvbMapper* m, int32_t layer, const float* xyz, int32_t memory, int64_t n, float* out_values,
+                              uint8_t* out_success) {
+  int rc = checkLayerQueryArgs(m, xyz, memory, n, out_values, out_success);
+  if (rc) return rc;
+  const int kind = layer == NVB_LAYER_TSDF ? kInterpTsdf : layer == NVB_LAYER_ESDF ? kInterpEsdf
+                   : layer == NVB_LAYER_OCCUPANCY ? kInterpOccupancy : -1;
+  DevLayer* L = kind >= 0 ? layerOf(m, layer) : nullptr;
+  if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "interpolation needs the mapper's TSDF, ESDF or occupancy layer");
+  if (n == 0) return NVB_OK;
+  const QueryLayer q = queryLayerOf(m, *L);
+  return runLayerQuery(m, xyz, memory, n, out_values, sizeof(float), out_success,
+                       [&](const float* x, void* o, uint8_t* f, cudaStream_t st) {
+                         launchInterpolate(q, kind, x, n, static_cast<float*>(o), f, m->num_sms, st);
+                       });
+}
+
+int32_t nvb_query_esdf(NvbMapper* const* mappers, int32_t num_mappers, const float* spheres_xyzr, int64_t n,
+                       int32_t with_gradient, float* out, void* caller_stream) {
+  QueryLayers q;
+  int rc = gatherQueryLayers(mappers, num_mappers, NVB_LAYER_ESDF, n, spheres_xyzr, out, &q);
+  if (rc) return rc;
+  return runMapperQuery(mappers, num_mappers, n, caller_stream, [&](cudaStream_t st) {
+    launchQueryEsdf(q, num_mappers > 1, spheres_xyzr, n, with_gradient != 0, out, mappers[0]->num_sms, st);
+  });
+}
+
+int32_t nvb_query_tsdf(NvbMapper* const* mappers, int32_t num_mappers, const float* xyz, int64_t n, float* out,
+                       void* caller_stream) {
+  QueryLayers q;
+  int rc = gatherQueryLayers(mappers, num_mappers, NVB_LAYER_TSDF, n, xyz, out, &q);
+  if (rc) return rc;
+  return runMapperQuery(mappers, num_mappers, n, caller_stream, [&](cudaStream_t st) {
+    launchQueryTsdf(q, num_mappers > 1, xyz, n, out, mappers[0]->num_sms, st);
+  });
+}
+
+int32_t nvb_query_occupancy(NvbMapper* const* mappers, int32_t num_mappers, const float* xyz, int64_t n, float* out,
+                            void* caller_stream) {
+  QueryLayers q;
+  int rc = gatherQueryLayers(mappers, num_mappers, NVB_LAYER_OCCUPANCY, n, xyz, out, &q);
+  if (rc) return rc;
+  // logOddsFromProbability(0), on the host like the mapper's other log-odds constants
+  const float initial = logOddsFromProbability(0.0f);
+  return runMapperQuery(mappers, num_mappers, n, caller_stream, [&](cudaStream_t st) {
+    launchQueryOccupancy(q, num_mappers > 1, initial, xyz, n, out, mappers[0]->num_sms, st);
+  });
 }
 
 }  // extern "C"

@@ -69,6 +69,21 @@ __host__ __device__ __forceinline__ int3 blockIndexFromPosition(float block_size
                    floatToIntRz(floorf(p.z / block_size)));
 }
 
+// 1 / blockSizeToVoxelSize(block_size), evaluated in double and rounded to float (core/internal/impl/indexing_impl.h:41).
+__host__ __device__ __forceinline__ float voxelSizeInv(float block_size) {
+  return (float)(1.0 / (double)(block_size * (1.0f / kVps)));
+}
+
+// getBlockAndVoxelIndexFromPositionInLayer (core/internal/impl/indexing_impl.h:37-49): the block index is floor(p / block_size),
+// the voxel index (p - block_size * b) * voxel_size_inv truncated toward zero and clamped to kVps - 1.
+__host__ __device__ __forceinline__ void blockAndVoxelIndexFromPosition(float block_size, float voxel_size_inv, const Vec3& p,
+                                                                        int3& b, int3& v) {
+  b = blockIndexFromPosition(block_size, p);
+  v.x = min(floatToIntRz((p.x - block_size * (float)b.x) * voxel_size_inv), kVps - 1);
+  v.y = min(floatToIntRz((p.y - block_size * (float)b.y) * voxel_size_inv), kVps - 1);
+  v.z = min(floatToIntRz((p.z - block_size * (float)b.z) * voxel_size_inv), kVps - 1);
+}
+
 // AlignedBox::exteriorDistance(c) of getAABBOfBlock(block_size, idx) (geometry/internal/impl/bounding_boxes_impl.h:55-60,
 // src/geometry/bounding_spheres.cpp:23-31): Eigen's squaredExteriorDistance accumulates the axes in order from 0.
 __host__ __device__ __forceinline__ float blockExteriorDistance(const int idx[3], float block_size, const float c[3]) {
@@ -701,5 +716,31 @@ struct CcArgs {
   int* sizes;               // drows x dcols
 };
 void launchRemoveSmallComponents(const CcArgs& a, int num_sms, cudaStream_t stream);
+
+// nvb_query.cu: point queries (VoxelBlockLayer::getVoxels, interpolation::interpolateOnCPU, nvblox_torch's sdf_query.cu)
+struct QueryLayer {
+  DevLayer layer;
+  float block_size, voxel_size, voxel_size_inv;
+};
+constexpr int kMaxQueryMappers = 16;
+// The mappers of one query, passed by value in the kernel's parameter space: nothing to allocate, free or keep alive while
+// the launch is pending.
+struct QueryLayers {
+  QueryLayer l[kMaxQueryMappers];
+  int n;
+};
+enum QueryInterpKind { kInterpTsdf = 0, kInterpEsdf = 1, kInterpOccupancy = 2 };
+// out: n voxels of voxel_bytes (a multiple of 4) each, written only where found[i] = 1
+void launchQueryVoxels(const QueryLayer& q, int voxel_bytes, const float* xyz, long long n, void* out, unsigned char* found,
+                       int num_sms, cudaStream_t stream);
+void launchInterpolate(const QueryLayer& q, int kind, const float* xyz, long long n, float* out, unsigned char* success,
+                       int num_sms, cudaStream_t stream);
+// q.n == 1 without `multi`: the single-mapper rules
+void launchQueryEsdf(const QueryLayers& q, bool multi, const float* spheres_xyzr, long long n, bool with_gradient, float* out,
+                     int num_sms, cudaStream_t stream);
+void launchQueryTsdf(const QueryLayers& q, bool multi, const float* xyz, long long n, float* out, int num_sms,
+                     cudaStream_t stream);
+void launchQueryOccupancy(const QueryLayers& q, bool multi, float initial_log_odds, const float* xyz, long long n, float* out,
+                          int num_sms, cudaStream_t stream);
 
 }  // namespace nvb

@@ -181,6 +181,89 @@ class _Layer:
         v, _ = self.get_blocks(idx)
         return {tuple(int(c) for c in k): v[i] for i, k in enumerate(idx)}
 
+    def get_voxels(self, points):
+        """VoxelBlockLayer::getVoxels / getVoxelsGPU (map/layer.h:265-295): the voxel holding each point, as stored, and
+        whether its block exists. `points` is an (n, 3) float32 host array -> (structured voxel array, bool array), or a CUDA
+        tensor -> ((n, voxel bytes) uint8 tensor, bool tensor) on its device, ordered after torch's current stream without a
+        host synchronisation; `.cpu().numpy().view(dtype)` of the first gives the structured voxels. Missed voxels are zero."""
+        vb = self._dtype.itemsize
+        if _is_tensor(points):
+            return self._device_query(self._m._L.nvb_layer_query_voxels, points, (vb,), "uint8")
+        pts = _host_points(points)
+        out = np.zeros(pts.shape[0], dtype=self._dtype)
+        ok = np.zeros(pts.shape[0], dtype=np.uint8)
+        check(self._m._L.nvb_layer_query_voxels(self._m._h, self._id, pts.ctypes.data, _lib.NVB_MEM_HOST, pts.shape[0],
+                                                out.ctypes.data, ok.ctypes.data))
+        return out, ok.astype(bool)
+
+    def interpolate(self, points):
+        """interpolation::interpolateOnCPU (interpolation/interpolation_3d.h) on the GPU, for a TSDF (distance), ESDF
+        (unsigned distance in voxels) or occupancy (probability) layer: (values, successes); a failed point has value 0.
+        Host array -> numpy arrays; CUDA tensor -> tensors on its device, as get_voxels."""
+        if _is_tensor(points):
+            return self._device_query(self._m._L.nvb_layer_interpolate, points, (), "float32")
+        pts = _host_points(points)
+        out = np.zeros(pts.shape[0], dtype=np.float32)
+        ok = np.zeros(pts.shape[0], dtype=np.uint8)
+        check(self._m._L.nvb_layer_interpolate(self._m._h, self._id, pts.ctypes.data, _lib.NVB_MEM_HOST, pts.shape[0],
+                                               out.ctypes.data, ok.ctypes.data))
+        return out, ok.astype(bool)
+
+    def _device_query(self, fn, points, shape, dtype):
+        import torch
+        pts = _device_points(points, 3, self._m._device)
+        n = pts.shape[0]
+        out = torch.zeros((n,) + shape, dtype=getattr(torch, dtype), device=pts.device)
+        ok = torch.zeros(n, dtype=torch.uint8, device=pts.device)
+        # No record_stream on the mapper's stream: torch's stream waits for the call, so a later reuse of these tensors' memory
+        # on it is ordered after the call, and nothing is recorded on a stream that closing the mapper destroys.
+        with _on_mapper_stream(self._m, pts.device):
+            check(fn(self._m._h, self._id, pts.data_ptr(), _lib.NVB_MEM_DEVICE, n, out.data_ptr(), ok.data_ptr()))
+        return out, ok.bool()
+
+
+def _is_tensor(a):
+    return hasattr(a, "data_ptr") and hasattr(a, "is_cuda")
+
+
+def _host_points(points):
+    pts = np.ascontiguousarray(points, dtype=np.float32)
+    if pts.ndim != 2 or pts.shape[1] != 3:
+        raise ValueError("points must be an (n, 3) array")
+    return pts
+
+
+def _device_points(t, cols, device, name="points"):
+    """Check a query tensor before anything is enqueued: a float32 (n, cols) CUDA tensor on the mappers' device."""
+    import torch
+    if not _is_tensor(t) or not t.is_cuda:
+        raise ValueError("%s must be a CUDA tensor" % name)
+    if t.dtype != torch.float32:
+        raise ValueError("%s must be float32, not %s" % (name, t.dtype))
+    cols = (cols,) if isinstance(cols, int) else tuple(cols)
+    if t.ndim != 2 or t.shape[1] not in cols:
+        raise ValueError("%s must have shape (n, %s), not %s" % (name, " or ".join(map(str, cols)), tuple(t.shape)))
+    if t.device.index != device:
+        raise ValueError("%s are on cuda:%d, the mapper on cuda:%d" % (name, t.device.index, device))
+    return t.detach().contiguous()
+
+
+class _on_mapper_stream:
+    """Runs a call enqueued on a mapper's stream between torch's current stream and its next work: the mapper's stream waits
+    for what torch enqueued so far, torch's stream waits for the call. Event hops only, no host synchronisation."""
+
+    def __init__(self, mapper, device):
+        import torch
+        self._torch = torch.cuda.current_stream(device)
+        self._ms = torch.cuda.ExternalStream(mapper._L.nvb_mapper_stream(mapper._h), device=device)
+
+    def __enter__(self):
+        self._ms.wait_stream(self._torch)
+
+    def __exit__(self, *exc):
+        self._torch.wait_stream(self._ms)
+        return False
+
 
 class _TsdfIntegrator:
     """ProjectiveTsdfIntegrator parameter surface (projective_tsdf_integrator.h:59-121,
