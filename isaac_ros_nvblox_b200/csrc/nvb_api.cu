@@ -47,6 +47,42 @@ struct StageEvent {
   int stage;
 };
 
+constexpr int kNoFill = -1;
+constexpr bool kKeepContents = true;
+
+// One device allocation of size() elements, freed by the destructor. The mapper's buffers and the temporaries of a single
+// call both use it, so that no return path leaks and no failed allocation leaves a pointer to freed memory behind.
+template <typename T>
+class DeviceArray {
+ public:
+  DeviceArray() = default;
+  DeviceArray(const DeviceArray&) = delete;
+  DeviceArray& operator=(const DeviceArray&) = delete;
+  DeviceArray(DeviceArray&& o) noexcept : p_(o.p_), n_(o.n_) {
+    o.p_ = nullptr;
+    o.n_ = 0;
+  }
+  DeviceArray& operator=(DeviceArray&& o) noexcept {
+    std::swap(p_, o.p_);
+    std::swap(n_, o.n_);
+    return *this;
+  }
+  ~DeviceArray() { cudaFree(p_); }
+
+  T* get() const { return p_; }
+  size_t size() const { return n_; }
+
+  // Makes room for `need` elements by allocating `count` of them (at least `need`); nothing happens when need <= size().
+  // The new allocation is filled with the byte `fill` unless that is kNoFill, and `keep` copies the old elements to its
+  // front. An existing allocation is replaced only once both of the mapper's streams are idle, and freed once the fill
+  // and the copy are done; the new pointer is published last, so after a failure the array still owns the old one.
+  cudaError_t grow(NvbMapper* m, size_t need, size_t count, int fill = kNoFill, bool keep = false);
+
+ private:
+  T* p_ = nullptr;
+  size_t n_ = 0;
+};
+
 }  // namespace
 
 struct NvbMapper {
@@ -76,27 +112,20 @@ struct NvbMapper {
   DevLayer freespace{};    // FreespaceLayer of a NVB_PROJECTIVE_TSDF_WITH_FREESPACE mapper
   DevLayer color{};        // ColorLayer, created by the first nvb_mapper_integrate_color
   NvbColorParams cp{};
-  int4* color_work = nullptr;  // blocks of the last colour frame {x, y, z, colour slot}
-  int color_work_cap = 0;
-  float* color_synth = nullptr;  // sphere-traced synthetic depth
-  size_t color_synth_cap = 0;
-  unsigned char* color_stage = nullptr;  // host colour image / mask staged on the device
-  size_t color_stage_cap = 0;
-  unsigned char* color_mask_stage = nullptr;
-  size_t color_mask_stage_cap = 0;
+  DeviceArray<int4> color_work;  // blocks of the last colour frame {x, y, z, colour slot}
+  DeviceArray<float> color_synth;  // sphere-traced synthetic depth
+  DeviceArray<unsigned char> color_stage;  // host colour image / mask staged on the device
+  DeviceArray<unsigned char> color_mask_stage;
   NvbFreespaceParams fp;
   NvbEsdfSliceParams sp;
   int esdf_mode = 0;                // EsdfMode: 0 unset, 1 3-D, 2 2-D slice (mapper.h:61, src/mapper/mapper.cpp:408-470)
-  unsigned long long* colset = nullptr;
-  size_t colset_n = 0;
-  int* cols = nullptr;
-  int cols_cap = 0;
+  DeviceArray<unsigned long long> colset;
+  DeviceArray<int> cols;
   long long fs_last_update_ms = 0;  // FreespaceIntegrator::last_update_time_ms_ (freespace_integrator.h:171)
-  int* dirty_fs = nullptr;          // the tracker's second consumer (BlocksToUpdateType::kFreespace)
-  int* todo_fs_slots = nullptr;
+  DeviceArray<int> dirty_fs;        // the tracker's second consumer (BlocksToUpdateType::kFreespace)
+  DeviceArray<int> todo_fs_slots;
   bool fs_tracker_initialized = false;
-  int4* fs_work = nullptr;
-  int fs_work_cap = 0;
+  DeviceArray<int4> fs_work;
   int tsdf_count_ub = 0;   // host-side upper bound of *tsdf.count
   int esdf_extra_ub = 0;   // blocks submitted to the ESDF through explicit lists
 
@@ -105,183 +134,151 @@ struct NvbMapper {
   // few KB on the device): a hit skips the raycast and replays the compaction + allocation, which yields the same list in the
   // same order and re-allocates blocks that were deallocated in between, like allocateBlocksWhereRequired does in the reference.
   BlockTensorMap tsdf_tmap;  // TMA descriptor of the TSDF slab (nvb_tsdf.cu)
-  int4* union_list = nullptr;  // nvb_blocks_union's own output list
-  int* union_list_count = nullptr;
-  int union_list_cap = 0;
+  DeviceArray<int4> union_list;  // nvb_blocks_union's own output list
+  DeviceArray<int> union_list_count;
 
-  // Mesh layer (nvb_mesh.cu): header slab + one arena for vertices / normals / triangle indices / colours
+  // Mesh layer (nvb_mesh.cu): header slab + one arena for vertices / normals / triangle indices / colours. An arena of
+  // mesh_t.size() entries holds 3 floats per entry in mesh_v and mesh_n and 4 bytes per entry in mesh_c.
   DevLayer mesh{};
-  float* mesh_v = nullptr;
-  float* mesh_n = nullptr;
-  int* mesh_t = nullptr;
-  unsigned char* mesh_c = nullptr;
-  long long mesh_arena_cap = 0;  // entries
-  float* mesh_alt_v = nullptr;   // the spare arena a repack moves the live segments into (then the two swap)
-  float* mesh_alt_n = nullptr;
-  int* mesh_alt_t = nullptr;
-  unsigned char* mesh_alt_c = nullptr;
-  long long mesh_alt_cap = 0;
-  int* mesh_state = nullptr;     // kArena* ints
-  int* mesh_counts = nullptr;
-  int* mesh_offsets = nullptr;
-  int mesh_list_cap = 0;
-  int* mesh_xyz_dev = nullptr;
-  int mesh_xyz_cap = 0;
-  int* dirty_mesh = nullptr;  // the tracker's third consumer (BlocksToUpdateType::kColorMesh)
-  int* todo_mesh_slots = nullptr;
+  DeviceArray<float> mesh_v;
+  DeviceArray<float> mesh_n;
+  DeviceArray<int> mesh_t;
+  DeviceArray<unsigned char> mesh_c;
+  DeviceArray<float> mesh_alt_v;  // the spare arena a repack moves the live segments into (then the two swap)
+  DeviceArray<float> mesh_alt_n;
+  DeviceArray<int> mesh_alt_t;
+  DeviceArray<unsigned char> mesh_alt_c;
+  DeviceArray<int> mesh_state;  // kArena* ints
+  DeviceArray<int> mesh_counts;
+  DeviceArray<int> mesh_offsets;
+  DeviceArray<int> mesh_xyz_dev;
+  DeviceArray<int> dirty_mesh;  // the tracker's third consumer (BlocksToUpdateType::kColorMesh)
+  DeviceArray<int> todo_mesh_slots;
   bool mesh_tracker_initialized = false;
   NvbMeshParams mp{1e-4f, 1, 5.0f};
   int cache_last_viewpoint = 1;
   // Mapper::do_depth_preprocessing / depth_preprocessing_num_dilations (mapper_params.h:33-42; mapper.cpp:335-352)
   int do_depth_preprocessing = 0;
   int depth_preprocessing_num_dilations = 4;
-  float* pre_depth = nullptr;
-  size_t pre_depth_cap = 0;
+  DeviceArray<float> pre_depth;
   int vc_n = 0;
   float vc_T[2][16];
   NvbCamera vc_cam[2];
   ViewGrid vc_grid[2];
   long long vc_cells[2] = {0, 0};
-  unsigned int* vc_bits[2] = {nullptr, nullptr};
-  size_t vc_bits_cap[2] = {0, 0};
+  DeviceArray<unsigned int> vc_bits[2];
 
   // per-frame scratch
-  unsigned int* bits = nullptr;
-  size_t bits_words_cap = 0;
-  int4* frame_blocks = nullptr;
-  int frame_cap = 0;
-  int* frame_count = nullptr;
-  unsigned long long* tile_state = nullptr;
-  int tile_cap = 0;
-  unsigned int* ticket = nullptr;
+  DeviceArray<unsigned int> bits;
+  DeviceArray<int4> frame_blocks;
+  int* frame_count = nullptr;  // in esdf_ints
+  DeviceArray<unsigned long long> tile_state;
+  DeviceArray<unsigned int> ticket;
   unsigned int ticket_base = 0;
   unsigned int epoch = 0;
-  int* error_dev = nullptr;
+  int* error_dev = nullptr;  // in esdf_ints
 
   // depth / mask staging for host inputs
-  float* depth_stage[kStagingBuffers] = {nullptr, nullptr, nullptr};
-  unsigned char* mask_stage[kStagingBuffers] = {nullptr, nullptr, nullptr};
-  size_t stage_pixels = 0;
+  DeviceArray<float> depth_stage[kStagingBuffers];
+  DeviceArray<unsigned char> mask_stage[kStagingBuffers];
   cudaEvent_t stage_copied[kStagingBuffers];
   cudaEvent_t stage_consumed[kStagingBuffers];
   bool stage_used[kStagingBuffers] = {false, false, false};
   unsigned long long frame_seq = 0;
 
   // tracker
-  int* dirty = nullptr;
-  int* todo_slots = nullptr;
-  int* todo_count = nullptr;
+  DeviceArray<int> dirty;
+  DeviceArray<int> todo_slots;
+  int* todo_count = nullptr;  // in esdf_ints
   bool tracker_initialized = false;
 
   // esdf scratch
-  int4* work = nullptr;
-  int* esdf_ints = nullptr;  // small counters block
-  int* upd_list = nullptr;
-  int* clr_list = nullptr;
-  int* cleared_list = nullptr;
-  int* ring_a = nullptr;
-  int* ring_b = nullptr;
-  int* stamp_a = nullptr;
-  int* stamp_b = nullptr;
-  int* nbr = nullptr;
-  int* nbr27 = nullptr;
-  unsigned char* shadow = nullptr;
-  int shadow_cap = 0;
-  unsigned char* xslab = nullptr;  // exchange-slab wavefront (esdf_persistent == 3): 2 x capacity slots of six faces (7.5 KiB)
-  int* xrec = nullptr;             // ... 2 x CTAs x xseg candidate records of 32 ints ...
+  DeviceArray<int4> work;
+  DeviceArray<int> esdf_ints;  // small counters block
+  DeviceArray<int> upd_list;
+  DeviceArray<int> clr_list;
+  DeviceArray<int> cleared_list;
+  DeviceArray<int> ring_a;
+  DeviceArray<int> ring_b;
+  DeviceArray<int> stamp_a;
+  DeviceArray<int> stamp_b;
+  DeviceArray<int> nbr;
+  DeviceArray<int> nbr27;
+  DeviceArray<unsigned char> shadow;
+  DeviceArray<unsigned char> xslab;  // exchange-slab wavefront (esdf_persistent == 3): 2 x capacity slots of six faces (7.5 KiB)
+  DeviceArray<int> xrec;             // ... 2 x CTAs x xseg candidate records of 32 ints ...
   int xseg = 0;
-  int xseg_grid = 0;               // CTAs of the exchange-slab launch the segments were sized for
-  int* xcounts = nullptr;          // ... and 2 x CTAs count pairs
-  int* cand_stamp = nullptr;
+  int xseg_grid = 0;                 // CTAs of the exchange-slab launch the segments were sized for
+  DeviceArray<int> xcounts;          // ... and 2 x CTAs count pairs
+  DeviceArray<int> cand_stamp;
   // decay integrators
   NvbTsdfDecayParams tdp;
   NvbOccupancyDecayParams odp;
-  int4* dead = nullptr;          // deallocated projective blocks of the last decay call
-  int dead_cap = 0;
-  int* skip_stamp = nullptr;     // per projective slot: == skip_seq -> block excluded from this decay call
-  int skip_cap = 0;
+  DeviceArray<int4> dead;        // deallocated projective blocks of the last decay call
+  DeviceArray<int> skip_stamp;   // per projective slot: == skip_seq -> block excluded from this decay call
   int skip_seq = 0;
-  int* dead_cleared_xyz = nullptr;
-  int dead_cleared_cap = 0;
+  DeviceArray<int> dead_cleared_xyz;
   // map clearing: Mapper::cleared_blocks_ (every clearBlocksInLayers adds to it), ShapeClearer's scratch
   std::set<std::array<int, 3>> cleared_blocks;
-  int4* shape_sel = nullptr;
-  int shape_sel_cap = 0;
-  NvbBoundingShape* shapes_dev = nullptr;
-  int shapes_cap = 0;
+  DeviceArray<int4> shape_sel;
+  DeviceArray<NvbBoundingShape> shapes_dev;
   // ground-plane estimator (nvb_ground.cu): parameters, device scratch, the last result (GroundPlaneEstimator's optionals)
   NvbGroundPlaneParams gp{};
-  unsigned long long* gp_keys = nullptr;  // 2 x gp_blocks_cap: packIndex keys of the TSDF slots, then the sorted keys
-  int* gp_slots = nullptr;                // 2 x gp_blocks_cap: the slots, then the slots in (x, y, z) block-index order
-  int2* gp_counts = nullptr;              // gp_blocks_cap
-  int gp_blocks_cap = 0;
-  void* gp_sort_temp = nullptr;           // the radix sort's scratch
-  size_t gp_sort_temp_bytes = 0;
-  float* gp_fit_stage = nullptr;          // nvb_ransac_fit_plane: host points staged on the device (3 floats each)
-  int gp_fit_stage_cap = 0;
-  int* gp_totals = nullptr;
-  float3* gp_crossings = nullptr;
-  int gp_crossings_cap = 0;
-  float4* gp_candidates = nullptr;
-  int gp_candidates_cap = 0;
-  float4* gp_fit_points = nullptr;  // nvb_ransac_fit_plane's own copy of its points
-  int gp_fit_points_cap = 0;
-  void* gp_states = nullptr;        // curand_init(1234, i, 0) for i < gp_states_n
-  int gp_states_n = 0;
-  float* gp_costs = nullptr;  // per iteration
-  int gp_costs_cap = 0;
-  float4* gp_planes = nullptr;
-  int gp_planes_cap = 0;
-  float* gp_result = nullptr;       // {nx, ny, nz, d, found}
+  DeviceArray<unsigned long long> gp_keys;  // 2 x gp_counts.size(): packIndex keys of the TSDF slots, then the sorted keys
+  DeviceArray<int> gp_slots;                // 2 x gp_counts.size(): the slots, then the slots in (x, y, z) block-index order
+  DeviceArray<int2> gp_counts;
+  DeviceArray<unsigned char> gp_sort_temp;  // the radix sort's scratch
+  DeviceArray<float> gp_fit_stage;          // nvb_ransac_fit_plane: host points staged on the device (3 floats each)
+  DeviceArray<int> gp_totals;
+  DeviceArray<float3> gp_crossings;
+  DeviceArray<float4> gp_candidates;
+  DeviceArray<float4> gp_fit_points;  // nvb_ransac_fit_plane's own copy of its points
+  DeviceArray<unsigned char> gp_states;  // curand_init(1234, i, 0) for each state of ransacStateBytes() bytes
+  DeviceArray<float> gp_costs;  // per iteration
+  DeviceArray<float4> gp_planes;
+  DeviceArray<float> gp_result;     // {nx, ny, nz, d, found}
   bool gp_valid = false;            // crossings and candidates of the last computation are kept
   int gp_num_crossings = 0, gp_num_candidates = 0;
   bool gp_found = false;
   float gp_plane[4] = {0, 0, 0, 0};
   // dynamics detection (nvb_dynamics.cu): the last frame's outputs, sized by pixels; the filter's scratch
-  float* dyn_depth = nullptr;      // staged depth
-  unsigned char* dyn_mask = nullptr;
-  unsigned char* dyn_clean = nullptr;
-  unsigned char* dyn_overlay = nullptr;
-  float* dyn_points = nullptr;
-  int dyn_pixels_cap = 0;
-  int2* dyn_counts = nullptr;
-  int dyn_tiles_cap = 0;
-  int* dyn_totals = nullptr;       // {points, 0}
+  DeviceArray<float> dyn_depth;    // staged depth
+  DeviceArray<unsigned char> dyn_mask;
+  DeviceArray<unsigned char> dyn_clean;
+  DeviceArray<unsigned char> dyn_overlay;
+  DeviceArray<float> dyn_points;
+  DeviceArray<int2> dyn_counts;
+  DeviceArray<int> dyn_totals;     // {points, 0}
   int dyn_rows = 0, dyn_cols = 0;
-  int* cc_labels = nullptr;
-  int* cc_sizes = nullptr;
-  int cc_cap = 0;
-  unsigned char* cc_stage = nullptr;  // host masks staged for the filter (input, then output)
-  int cc_stage_cap = 0;
+  DeviceArray<int> cc_labels;
+  DeviceArray<int> cc_sizes;
+  DeviceArray<unsigned char> cc_stage;  // host masks staged for the filter (input, then output)
   cudaEvent_t dyn_event = nullptr;    // nvb_mapper_wait_for: recorded on this mapper's stream
   cudaEvent_t query_event = nullptr;  // point queries (nvb_query_*): the hand-over between this mapper and the query's stream
   // last integrated view (Mapper::last_posed_depth_image_, mapper.h:830-833), kept when keep_last_view is set
   int keep_last_view = 0;
-  float* last_depth = nullptr;
-  size_t last_depth_cap = 0;
+  DeviceArray<float> last_depth;
   int last_rows = 0, last_cols = 0;
   float last_T_L_C[16];
   NvbCamera last_cam;
   bool has_last_view = false;
-  int* cand_a = nullptr;
-  int* cand_b = nullptr;
+  DeviceArray<int> cand_a;
+  DeviceArray<int> cand_b;
   int ges_switch = 160;
-  int* seed_upd = nullptr;
-  int* seed_clr = nullptr;
+  DeviceArray<int> seed_upd;
+  DeviceArray<int> seed_clr;
   // device-resident merge of block lists (nvb_blocks_union_segments): own scratch, usable on any stream
-  unsigned int* union_bits = nullptr;
-  long long union_bits_cap = 0;      // in bits
-  int* union_state = nullptr;        // AABB, error flag, words in use
-  unsigned int* clr_bits = nullptr;  // to-clear bitmap of the current update (2048 words)
-  unsigned int* psum = nullptr;  // per ESDF slot: box of the block offsets its voxels' parents point into (clear-pass pruning)
+  DeviceArray<unsigned int> union_bits;
+  DeviceArray<int> union_state;           // AABB, error flag, words in use
+  DeviceArray<unsigned int> clr_bits;     // to-clear bitmap of the current update (2048 words)
+  DeviceArray<unsigned int> psum;  // per ESDF slot: box of the block offsets its voxels' parents point into (clear-pass pruning)
   bool prune_default = false;    // esdf_persistent == 3 and not switched off (NVB_CLEAR_PRUNE=0)
   bool prune_ok = false;         // the summaries are upper bounds for every block (only the exchange-slab wavefront keeps them)
   int update_seq = 0;
-  long long* stats = nullptr;
-  unsigned int* barrier = nullptr;
-  unsigned long long* phase_max = nullptr;
-  int* xyz_upload = nullptr;
-  int xyz_upload_cap = 0;
+  DeviceArray<long long> stats;
+  DeviceArray<unsigned int> barrier;
+  DeviceArray<unsigned long long> phase_max;
+  DeviceArray<int> xyz_upload;
 
   // pinned host scratch
   int* h_ints = nullptr;  // [0] frame count, [1] error, [2..] misc, [8], [9] prefetched error words (pinned)
@@ -311,6 +308,29 @@ cudaError_t syncAll(NvbMapper* m) {
   if (m->esdf_stream) e = cudaStreamSynchronize(m->esdf_stream);
   m->esdf_in_flight = false;
   return e;
+}
+
+template <typename T>
+cudaError_t DeviceArray<T>::grow(NvbMapper* m, size_t need, size_t count, int fill, bool keep) {
+  if (need <= n_) return cudaSuccess;
+  count = std::max(count, need);
+  if (p_) {
+    const cudaError_t e = syncAll(m);
+    if (e != cudaSuccess) return e;
+  }
+  T* q = nullptr;
+  cudaError_t e = cudaMalloc(&q, count * sizeof(T));
+  if (e == cudaSuccess && fill != kNoFill) e = cudaMemsetAsync(q, fill, count * sizeof(T), m->stream);
+  if (e == cudaSuccess && keep && n_ > 0) e = cudaMemcpyAsync(q, p_, n_ * sizeof(T), cudaMemcpyDeviceToDevice, m->stream);
+  if (e == cudaSuccess && (fill != kNoFill || keep)) e = cudaStreamSynchronize(m->stream);
+  if (e != cudaSuccess) {
+    cudaFree(q);
+    return e;
+  }
+  cudaFree(p_);
+  p_ = q;
+  n_ = count;
+  return cudaSuccess;
 }
 
 // Device-side join: later work on `stream` waits for the wavefront on `esdf_stream`.
@@ -349,18 +369,6 @@ void freeLayer(DevLayer* L) {
   cudaFree(L->blocks), cudaFree(L->block_index), cudaFree(L->count), cudaFree(L->hash.keys), cudaFree(L->hash.vals);
   cudaFree(L->free_slots), cudaFree(L->free_count);
   *L = DevLayer{};
-}
-
-template <typename T>
-int reallocCopy(T** p, size_t old_n, size_t new_n, bool zero_rest, cudaStream_t stream) {
-  T* q = nullptr;
-  NVB_CUDA(cudaMalloc(&q, new_n * sizeof(T)));
-  if (zero_rest) NVB_CUDA(cudaMemsetAsync(q, 0, new_n * sizeof(T), stream));
-  if (*p && old_n) NVB_CUDA(cudaMemcpyAsync(q, *p, old_n * sizeof(T), cudaMemcpyDeviceToDevice, stream));
-  NVB_CUDA(cudaStreamSynchronize(stream));
-  if (*p) cudaFree(*p);
-  *p = q;
-  return NVB_OK;
 }
 
 // Doubling growth of a layer slab (BlockMemoryPool expansion,
@@ -403,85 +411,61 @@ int growLayer(NvbMapper* m, DevLayer* L, int new_capacity) {
 int allocWaveXRecords(NvbMapper* m, int cap) {
   const int grid = esdfWaveXGrid(m->num_sms, m->esdf_reserved_sms);
   NVB_CUDA(syncAll(m));
-  if (m->xrec) cudaFree(m->xrec);
-  m->xrec = nullptr;
+  m->xrec = DeviceArray<int>();  // released first: the exact size follows the grid down as well as up
   m->xseg = 6 * ((cap + grid - 1) / grid) + 64;
   m->xseg_grid = grid;
-  NVB_CUDA(cudaMalloc(&m->xrec, 2 * (size_t)grid * m->xseg * 32 * sizeof(int)));
+  const size_t n = 2 * (size_t)grid * m->xseg * 32;
+  NVB_CUDA(m->xrec.grow(m, n, n));
   return NVB_OK;
 }
 
-int allocEsdfScratch(NvbMapper* m, int old_cap, int cap) {
-  int rc;
-  if ((rc = reallocCopy(&m->work, 0, (size_t)cap, false, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->upd_list, 0, (size_t)cap, false, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->clr_list, 0, (size_t)cap, false, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->cleared_list, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->ring_a, 0, (size_t)cap, false, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->ring_b, 0, (size_t)cap, false, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->stamp_a, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->stamp_b, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->seed_upd, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->seed_clr, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->psum, 2 * (size_t)old_cap, 2 * (size_t)cap, true, m->stream))) return rc;
+// The ESDF slab's companions, at `cap` slots; the ones that carry state from one update to the next keep their contents.
+int allocEsdfScratch(NvbMapper* m, int cap) {
+  const size_t n = cap;
+  NVB_CUDA(m->work.grow(m, n, n));
+  NVB_CUDA(m->upd_list.grow(m, n, n));
+  NVB_CUDA(m->clr_list.grow(m, n, n));
+  NVB_CUDA(m->cleared_list.grow(m, n, n, 0, kKeepContents));
+  NVB_CUDA(m->ring_a.grow(m, n, n));
+  NVB_CUDA(m->ring_b.grow(m, n, n));
+  NVB_CUDA(m->stamp_a.grow(m, n, n, 0, kKeepContents));
+  NVB_CUDA(m->stamp_b.grow(m, n, n, 0, kKeepContents));
+  NVB_CUDA(m->seed_upd.grow(m, n, n, 0, kKeepContents));
+  NVB_CUDA(m->seed_clr.grow(m, n, n, 0, kKeepContents));
+  NVB_CUDA(m->psum.grow(m, 2 * n, 2 * n, 0, kKeepContents));
   // neighbour table: 0xFE bytes = "unknown" (< -1) for slots that were never linked
-  {
-    int* q = nullptr;
-    NVB_CUDA(cudaMalloc(&q, (size_t)cap * 6 * sizeof(int)));
-    NVB_CUDA(cudaMemsetAsync(q, 0xFE, (size_t)cap * 6 * sizeof(int), m->stream));
-    if (m->nbr && old_cap)
-      NVB_CUDA(cudaMemcpyAsync(q, m->nbr, (size_t)old_cap * 6 * sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
-    NVB_CUDA(syncAll(m));
-    if (m->nbr) cudaFree(m->nbr);
-    m->nbr = q;
-  }
-  {
-    int* q = nullptr;
-    NVB_CUDA(cudaMalloc(&q, (size_t)cap * 27 * sizeof(int)));
-    NVB_CUDA(cudaMemsetAsync(q, 0xFE, (size_t)cap * 27 * sizeof(int), m->stream));
-    if (m->nbr27 && old_cap)
-      NVB_CUDA(cudaMemcpyAsync(q, m->nbr27, (size_t)old_cap * 27 * sizeof(int), cudaMemcpyDeviceToDevice, m->stream));
-    NVB_CUDA(syncAll(m));
-    if (m->nbr27) cudaFree(m->nbr27);
-    m->nbr27 = q;
-  }
-  if ((rc = reallocCopy(&m->cand_stamp, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->cand_a, 0, (size_t)cap, false, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->cand_b, 0, (size_t)cap, false, m->stream))) return rc;
+  NVB_CUDA(m->nbr.grow(m, 6 * n, 6 * n, 0xFE, kKeepContents));
+  NVB_CUDA(m->nbr27.grow(m, 27 * n, 27 * n, 0xFE, kKeepContents));
+  NVB_CUDA(m->cand_stamp.grow(m, n, n, 0, kKeepContents));
+  NVB_CUDA(m->cand_a.grow(m, n, n));
+  NVB_CUDA(m->cand_b.grow(m, n, n));
   if (m->esdf_persistent == 2) {
     // gather-emulate-sweep wavefront: second ESDF slab (contents only live inside one launch)
-    if (m->shadow) cudaFree(m->shadow);
-    m->shadow = nullptr;
-    NVB_CUDA(cudaMalloc(&m->shadow, (size_t)cap * kEsdfBlockBytes));
-    m->shadow_cap = cap;
+    NVB_CUDA(m->shadow.grow(m, n * kEsdfBlockBytes, n * kEsdfBlockBytes));
   }
   if (m->esdf_persistent == 3) {
     // exchange-slab wavefront: two slabs by ring parity + the candidate records (contents only live inside one launch)
-    NVB_CUDA(syncAll(m));
-    if (m->xslab) cudaFree(m->xslab);
-    m->xslab = nullptr;
-    NVB_CUDA(cudaMalloc(&m->xslab, esdfWaveXSlabBytes(cap)));
+    NVB_CUDA(m->xslab.grow(m, esdfWaveXSlabBytes(cap), esdfWaveXSlabBytes(cap)));
     int rc;
     if ((rc = allocWaveXRecords(m, cap))) return rc;
-    if (!m->xcounts) {
-      NVB_CUDA(cudaMalloc(&m->xcounts, esdfWaveXFlagBytes()));
-      NVB_CUDA(cudaMemsetAsync(m->xcounts, 0, esdfWaveXFlagBytes(), m->stream));
-    }
+    const size_t flags = esdfWaveXFlagBytes() / sizeof(int);
+    NVB_CUDA(m->xcounts.grow(m, flags, flags, 0));
   }
   return NVB_OK;
 }
 
-int allocTsdfSide(NvbMapper* m, int old_cap, int cap) {
-  int rc;
-  if ((rc = reallocCopy(&m->dirty, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-  if ((rc = reallocCopy(&m->todo_slots, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
+// The tracker's arrays follow the projective slab's capacity and keep their contents.
+int allocTsdfSide(NvbMapper* m, int cap) {
+  const size_t n = cap;
+  NVB_CUDA(m->dirty.grow(m, n, n, 0, kKeepContents));
+  NVB_CUDA(m->todo_slots.grow(m, n, n, 0, kKeepContents));
   if (m->projective_layer_type == NVB_PROJECTIVE_TSDF_WITH_FREESPACE) {
-    if ((rc = reallocCopy(&m->dirty_fs, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-    if ((rc = reallocCopy(&m->todo_fs_slots, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
+    NVB_CUDA(m->dirty_fs.grow(m, n, n, 0, kKeepContents));
+    NVB_CUDA(m->todo_fs_slots.grow(m, n, n, 0, kKeepContents));
   }
-  if (m->dirty_mesh) {
-    if ((rc = reallocCopy(&m->dirty_mesh, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
-    if ((rc = reallocCopy(&m->todo_mesh_slots, (size_t)old_cap, (size_t)cap, true, m->stream))) return rc;
+  if (m->dirty_mesh.get()) {
+    NVB_CUDA(m->dirty_mesh.grow(m, n, n, 0, kKeepContents));
+    NVB_CUDA(m->todo_mesh_slots.grow(m, n, n, 0, kKeepContents));
   }
   return NVB_OK;
 }
@@ -499,34 +483,34 @@ EsdfCtx makeEsdfCtx(NvbMapper* m) {
   c.tsdf = m->tsdf, c.esdf = m->esdf;
   c.freespace = m->freespace;
   c.use_freespace = m->projective_layer_type == NVB_PROJECTIVE_TSDF_WITH_FREESPACE ? 1 : 0;
-  c.work = m->work;
-  c.work_count = m->esdf_ints + kWorkCount;
-  c.upd_list = m->upd_list, c.upd_count = m->esdf_ints + kUpdCount;
-  c.clr_list = m->clr_list, c.clr_count = m->esdf_ints + kClrCount;
-  c.clr_aabb = m->esdf_ints + kClrAabb;
-  c.cleared_list = m->cleared_list, c.cleared_count = m->esdf_ints + kClearedCount;
-  c.ring_a = m->ring_a, c.ring_b = m->ring_b;
-  c.ring_count = m->esdf_ints + kRingCount;
-  c.tail_state = m->esdf_ints + kTailState;
-  c.stamp_a = m->stamp_a, c.stamp_b = m->stamp_b;
-  c.ring_id = m->esdf_ints + kRingId;
-  c.nbr = m->nbr, c.seed_upd = m->seed_upd, c.seed_clr = m->seed_clr;
-  c.clr_bits = m->clr_bits;
-  c.psum = m->psum, c.prune = (m->prune_ok && m->esdf_persistent == 3) ? 1 : 0;
-  c.nbr27 = m->nbr27, c.shadow = m->shadow, c.cand_stamp = m->cand_stamp;
-  c.xslab = m->xslab, c.xrec = m->xrec, c.xtail = m->esdf_ints + kXTail, c.xseg = m->xseg, c.xcounts = m->xcounts;
+  c.work = m->work.get();
+  c.work_count = m->esdf_ints.get() + kWorkCount;
+  c.upd_list = m->upd_list.get(), c.upd_count = m->esdf_ints.get() + kUpdCount;
+  c.clr_list = m->clr_list.get(), c.clr_count = m->esdf_ints.get() + kClrCount;
+  c.clr_aabb = m->esdf_ints.get() + kClrAabb;
+  c.cleared_list = m->cleared_list.get(), c.cleared_count = m->esdf_ints.get() + kClearedCount;
+  c.ring_a = m->ring_a.get(), c.ring_b = m->ring_b.get();
+  c.ring_count = m->esdf_ints.get() + kRingCount;
+  c.tail_state = m->esdf_ints.get() + kTailState;
+  c.stamp_a = m->stamp_a.get(), c.stamp_b = m->stamp_b.get();
+  c.ring_id = m->esdf_ints.get() + kRingId;
+  c.nbr = m->nbr.get(), c.seed_upd = m->seed_upd.get(), c.seed_clr = m->seed_clr.get();
+  c.clr_bits = m->clr_bits.get();
+  c.psum = m->psum.get(), c.prune = (m->prune_ok && m->esdf_persistent == 3) ? 1 : 0;
+  c.nbr27 = m->nbr27.get(), c.shadow = m->shadow.get(), c.cand_stamp = m->cand_stamp.get();
+  c.xslab = m->xslab.get(), c.xrec = m->xrec.get(), c.xtail = m->esdf_ints.get() + kXTail, c.xseg = m->xseg, c.xcounts = m->xcounts.get();
   c.xsplit_min_k = m->esdf_split_min_k;
-  c.ges_counts = m->esdf_ints + kGesCounts;
-  c.cand_a = m->cand_a, c.cand_b = m->cand_b, c.ges_switch = m->ges_switch;
-  c.colset_keys = m->colset, c.colset_mask = m->colset_n ? (unsigned int)(m->colset_n - 1) : 0u;
-  c.cols = m->cols, c.cols_count = m->esdf_ints + kColsCount;
-  c.dead_cleared_xyz = m->dead_cleared_xyz;
-  c.dead_cleared_count = m->dead_cleared_xyz ? m->esdf_ints + kDeadClearedCount : nullptr;
-  c.cleared_seq = m->esdf_ints + kClearedSeq;
+  c.ges_counts = m->esdf_ints.get() + kGesCounts;
+  c.cand_a = m->cand_a.get(), c.cand_b = m->cand_b.get(), c.ges_switch = m->ges_switch;
+  c.colset_keys = m->colset.get(), c.colset_mask = m->colset.size() ? (unsigned int)(m->colset.size() - 1) : 0u;
+  c.cols = m->cols.get(), c.cols_count = m->esdf_ints.get() + kColsCount;
+  c.dead_cleared_xyz = m->dead_cleared_xyz.get();
+  c.dead_cleared_count = m->dead_cleared_xyz.get() ? m->esdf_ints.get() + kDeadClearedCount : nullptr;
+  c.cleared_seq = m->esdf_ints.get() + kClearedSeq;
   c.update_seq = m->update_seq;
-  c.barrier = m->barrier;
-  c.phase_max = m->phase_max;
-  c.stats = m->stats;
+  c.barrier = m->barrier.get();
+  c.phase_max = m->phase_max.get();
+  c.stats = m->stats.get();
   c.error = m->error_dev;
   // esdf_integrator.cu:693-696, 672-676
   const float max_esdf_distance_vox = m->ep.max_esdf_distance_m / m->voxel_size;
@@ -675,10 +659,9 @@ int ensureTsdfCapacity(NvbMapper* m, long long new_cells) {
   long long cap = m->tsdf.capacity;
   while (cap < (long long)count + new_cells) cap *= 2;
   if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "TSDF layer would exceed 2^28 blocks");
-  const int old = m->tsdf.capacity;
   int rc = growLayer(m, &m->tsdf, (int)cap);
   if (rc) return rc;
-  return allocTsdfSide(m, old, (int)cap);
+  return allocTsdfSide(m, (int)cap);
 }
 
 // The explicit-list entry points are synchronous: afterwards the real fill level of the ESDF slab is known and replaces
@@ -696,52 +679,29 @@ int ensureEsdfCapacity(NvbMapper* m, long long needed_total) {
   long long cap = m->esdf.capacity;
   while (cap < needed_total) cap *= 2;
   if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "ESDF layer would exceed 2^28 blocks");
-  const int old = m->esdf.capacity;
   int rc = growLayer(m, &m->esdf, (int)cap);
   if (rc) return rc;
-  return allocEsdfScratch(m, old, (int)cap);
+  return allocEsdfScratch(m, (int)cap);
 }
 
 int ensureFrameScratch(NvbMapper* m, const ViewGrid& g) {
-  if ((size_t)g.num_words > m->bits_words_cap) {
-    NVB_CUDA(syncAll(m));
-    const size_t cap = (size_t)(1.5 * g.num_words) + 64;  // kBufferExpansionFactor, view_calculator_impl.cuh:159
-    if (m->bits) cudaFree(m->bits);
-    NVB_CUDA(cudaMalloc(&m->bits, cap * sizeof(unsigned int)));
-    NVB_CUDA(cudaMemsetAsync(m->bits, 0, cap * sizeof(unsigned int), m->stream));
-    m->bits_words_cap = cap;
-  }
-  if (g.linear_size > m->frame_cap) {
-    NVB_CUDA(syncAll(m));
-    const int cap = (int)std::min<long long>((long long)(1.5 * g.linear_size) + 64, 0x7fffffff);
-    if (m->frame_blocks) cudaFree(m->frame_blocks);
-    NVB_CUDA(cudaMalloc(&m->frame_blocks, (size_t)cap * sizeof(int4)));
-    m->frame_cap = cap;
-  }
-  const int tiles = compactNumTiles(g);
-  if (tiles > m->tile_cap) {
-    NVB_CUDA(syncAll(m));
-    const int cap = tiles * 2;
-    if (m->tile_state) cudaFree(m->tile_state);
-    NVB_CUDA(cudaMalloc(&m->tile_state, (size_t)cap * sizeof(unsigned long long)));
-    NVB_CUDA(cudaMemsetAsync(m->tile_state, 0, (size_t)cap * sizeof(unsigned long long), m->stream));
-    m->tile_cap = cap;
-  }
+  const size_t words = g.num_words;
+  NVB_CUDA(m->bits.grow(m, words, (size_t)(1.5 * words) + 64, 0));  // kBufferExpansionFactor, view_calculator_impl.cuh:159
+  const size_t cells = g.linear_size;
+  NVB_CUDA(m->frame_blocks.grow(m, cells, (size_t)std::min<long long>((long long)(1.5 * cells) + 64, 0x7fffffff)));
+  const size_t tiles = compactNumTiles(g);
+  NVB_CUDA(m->tile_state.grow(m, tiles, 2 * tiles, 0));
   return NVB_OK;
 }
 
 int ensureStaging(NvbMapper* m, size_t pixels) {
-  if (pixels <= m->stage_pixels) return NVB_OK;
-  NVB_CUDA(syncAll(m));
+  if (pixels <= m->mask_stage[kStagingBuffers - 1].size()) return NVB_OK;  // the last buffer a growth replaces
   NVB_CUDA(cudaStreamSynchronize(m->copy_stream));
   for (int k = 0; k < kStagingBuffers; k++) {
-    if (m->depth_stage[k]) cudaFree(m->depth_stage[k]);
-    if (m->mask_stage[k]) cudaFree(m->mask_stage[k]);
-    NVB_CUDA(cudaMalloc(&m->depth_stage[k], pixels * sizeof(float)));
-    NVB_CUDA(cudaMalloc(&m->mask_stage[k], pixels));
+    NVB_CUDA(m->depth_stage[k].grow(m, pixels, pixels));
+    NVB_CUDA(m->mask_stage[k].grow(m, pixels, pixels));
     m->stage_used[k] = false;
   }
-  m->stage_pixels = pixels;
   return NVB_OK;
 }
 
@@ -872,14 +832,14 @@ int enqueueFrame(NvbMapper* m, const float* depth, const unsigned char* mask, in
     if ((rc = ensureStaging(m, pixels))) return rc;
     stage_slot = (int)(m->frame_seq % kStagingBuffers);
     if (m->stage_used[stage_slot]) NVB_CUDA(cudaStreamWaitEvent(m->copy_stream, m->stage_consumed[stage_slot], 0));
-    NVB_CUDA(cudaMemcpyAsync(m->depth_stage[stage_slot], depth, pixels * sizeof(float), cudaMemcpyHostToDevice,
+    NVB_CUDA(cudaMemcpyAsync(m->depth_stage[stage_slot].get(), depth, pixels * sizeof(float), cudaMemcpyHostToDevice,
                              m->copy_stream));
     if (mask)
-      NVB_CUDA(cudaMemcpyAsync(m->mask_stage[stage_slot], mask, pixels, cudaMemcpyHostToDevice, m->copy_stream));
+      NVB_CUDA(cudaMemcpyAsync(m->mask_stage[stage_slot].get(), mask, pixels, cudaMemcpyHostToDevice, m->copy_stream));
     NVB_CUDA(cudaEventRecord(m->stage_copied[stage_slot], m->copy_stream));
     NVB_CUDA(cudaStreamWaitEvent(m->stream, m->stage_copied[stage_slot], 0));
-    depth_dev = m->depth_stage[stage_slot];
-    mask_dev = mask ? m->mask_stage[stage_slot] : nullptr;
+    depth_dev = m->depth_stage[stage_slot].get();
+    mask_dev = mask ? m->mask_stage[stage_slot].get() : nullptr;
   }
   m->frame_seq++;
   if (integrate && m->do_depth_preprocessing) {
@@ -888,27 +848,16 @@ int enqueueFrame(NvbMapper* m, const float* depth, const unsigned char* mask, in
     // CHECK_GE(rows, 3), CHECK_GE(cols, 3) (src/sensors/depth_preprocessing.cpp:64-65)
     if (rows < 3 || cols < 3) return fail(NVB_ERR_INVALID_ARGUMENT, "depth preprocessing needs an image of at least 3x3");
     const size_t pixels = (size_t)rows * cols;
-    if (m->pre_depth_cap < pixels) {
-      NVB_CUDA(syncAll(m));
-      if (m->pre_depth) cudaFree(m->pre_depth);
-      m->pre_depth = nullptr, m->pre_depth_cap = 0;
-      NVB_CUDA(cudaMalloc(&m->pre_depth, pixels * sizeof(float)));
-      m->pre_depth_cap = pixels;
-    }
-    launchDilateInvalid(depth_dev, m->pre_depth, rows, cols, m->depth_preprocessing_num_dilations, kInvalidDepthThreshold,
+    NVB_CUDA(m->pre_depth.grow(m, pixels, pixels));
+    launchDilateInvalid(depth_dev, m->pre_depth.get(), rows, cols, m->depth_preprocessing_num_dilations, kInvalidDepthThreshold,
                         kInvalidDepthValue, m->stream);
     m->launches++;
-    depth_dev = m->pre_depth;
+    depth_dev = m->pre_depth.get();
   }
   if (integrate && m->keep_last_view) {
     const size_t pixels = (size_t)rows * cols;
-    if (m->last_depth_cap < pixels) {
-      NVB_CUDA(syncAll(m));
-      if (m->last_depth) cudaFree(m->last_depth);
-      NVB_CUDA(cudaMalloc(&m->last_depth, pixels * sizeof(float)));
-      m->last_depth_cap = pixels;
-    }
-    NVB_CUDA(cudaMemcpyAsync(m->last_depth, depth_dev, pixels * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
+    NVB_CUDA(m->last_depth.grow(m, pixels, pixels));
+    NVB_CUDA(cudaMemcpyAsync(m->last_depth.get(), depth_dev, pixels * sizeof(float), cudaMemcpyDeviceToDevice, m->stream));
     m->last_rows = rows, m->last_cols = cols, m->last_cam = *cam, m->has_last_view = true;
     memcpy(m->last_T_L_C, T_L_C_cm, sizeof(m->last_T_L_C));
   }
@@ -916,27 +865,23 @@ int enqueueFrame(NvbMapper* m, const float* depth, const unsigned char* mask, in
   beginStage(m, 0);
   if (cache_hit >= 0) {
     // the cached view bitset instead of a raycast
-    NVB_CUDA(cudaMemcpyAsync(m->bits, m->vc_bits[cache_hit], (size_t)grid.num_words * sizeof(unsigned int), cudaMemcpyDeviceToDevice,
+    NVB_CUDA(cudaMemcpyAsync(m->bits.get(), m->vc_bits[cache_hit].get(), (size_t)grid.num_words * sizeof(unsigned int), cudaMemcpyDeviceToDevice,
                              m->stream));
   } else {
     launchViewRaycast(depth_dev, rows, cols, T_L_C, *cam, block_size, trunc_m, max_dist, m->tp.raycast_subsampling,
-                      grid, m->bits, m->stream);
+                      grid, m->bits.get(), m->stream);
     m->launches++;
     if (integrate && m->cache_last_viewpoint) {
       // ViewpointCache::storeResultInCache (view_calculator_impl.h:157-174): newest first, the oldest of two is dropped
       if (m->vc_n == 2) m->vc_n = 1;
       if (m->vc_n == 1) {
-        std::swap(m->vc_bits[0], m->vc_bits[1]), std::swap(m->vc_bits_cap[0], m->vc_bits_cap[1]);
+        std::swap(m->vc_bits[0], m->vc_bits[1]);
         memcpy(m->vc_T[1], m->vc_T[0], sizeof(m->vc_T[0]));
         m->vc_cam[1] = m->vc_cam[0], m->vc_grid[1] = m->vc_grid[0], m->vc_cells[1] = m->vc_cells[0];
       }
-      if (m->vc_bits_cap[0] < (size_t)grid.num_words) {
-        NVB_CUDA(syncAll(m));
-        if (m->vc_bits[0]) cudaFree(m->vc_bits[0]);
-        m->vc_bits_cap[0] = (size_t)(1.5 * grid.num_words) + 64;
-        NVB_CUDA(cudaMalloc(&m->vc_bits[0], m->vc_bits_cap[0] * sizeof(unsigned int)));
-      }
-      NVB_CUDA(cudaMemcpyAsync(m->vc_bits[0], m->bits, (size_t)grid.num_words * sizeof(unsigned int), cudaMemcpyDeviceToDevice,
+      const size_t words = grid.num_words;
+      NVB_CUDA(m->vc_bits[0].grow(m, words, (size_t)(1.5 * words) + 64));
+      NVB_CUDA(cudaMemcpyAsync(m->vc_bits[0].get(), m->bits.get(), (size_t)grid.num_words * sizeof(unsigned int), cudaMemcpyDeviceToDevice,
                                m->stream));
       memcpy(m->vc_T[0], T_L_C_cm, sizeof(m->vc_T[0]));
       m->vc_cam[0] = *cam, m->vc_grid[0] = grid, m->vc_cells[0] = cells;
@@ -947,33 +892,33 @@ int enqueueFrame(NvbMapper* m, const float* depth, const unsigned char* mask, in
 
   beginStage(m, 1);
   CompactArgs ca{};
-  ca.bits = m->bits;
+  ca.bits = m->bits.get();
   ca.grid = grid;
-  ca.frame_blocks = m->frame_blocks;
+  ca.frame_blocks = m->frame_blocks.get();
   ca.frame_count = m->frame_count;
-  ca.tile_state = m->tile_state;
-  ca.ticket = m->ticket;
+  ca.tile_state = m->tile_state.get();
+  ca.ticket = m->ticket.get();
   ca.ticket_base = m->ticket_base;
   ca.epoch = ++m->epoch;
   ca.allocate = integrate ? 1 : 0;
   ca.layer = m->tsdf;
   ca.error = m->error_dev;
-  ca.dirty = (integrate && m->tracker_initialized) ? m->dirty : nullptr;
-  ca.todo_slots = m->todo_slots;
+  ca.dirty = (integrate && m->tracker_initialized) ? m->dirty.get() : nullptr;
+  ca.todo_slots = m->todo_slots.get();
   ca.todo_count = m->todo_count;
-  ca.dirty2 = (integrate && m->dirty_fs && m->fs_tracker_initialized) ? m->dirty_fs : nullptr;
-  ca.todo2_slots = m->todo_fs_slots;
-  ca.todo2_count = m->esdf_ints + kTodoFsCount;
-  ca.dirty3 = (integrate && m->dirty_mesh && m->mesh_tracker_initialized) ? m->dirty_mesh : nullptr;
-  ca.todo3_slots = m->todo_mesh_slots;
-  ca.todo3_count = m->esdf_ints + kTodoMeshCount;
+  ca.dirty2 = (integrate && m->dirty_fs.get() && m->fs_tracker_initialized) ? m->dirty_fs.get() : nullptr;
+  ca.todo2_slots = m->todo_fs_slots.get();
+  ca.todo2_count = m->esdf_ints.get() + kTodoFsCount;
+  ca.dirty3 = (integrate && m->dirty_mesh.get() && m->mesh_tracker_initialized) ? m->dirty_mesh.get() : nullptr;
+  ca.todo3_slots = m->todo_mesh_slots.get();
+  ca.todo3_count = m->esdf_ints.get() + kTodoMeshCount;
   launchCompactAllocate(ca, m->stream);
   if (compactUsesTickets(grid)) m->ticket_base += (unsigned int)compactNumTiles(grid);
   endStage(m);
   m->launches++;
 
   if (!integrate) {
-    launchClearBits(m->bits, grid.num_words, m->stream);
+    launchClearBits(m->bits.get(), grid.num_words, m->stream);
     m->launches++;
   }
   if (integrate) {
@@ -997,16 +942,16 @@ int enqueueFrame(NvbMapper* m, const float* depth, const unsigned char* mask, in
       o.occupied_half_width_m = m->op.occupied_region_half_width_m;
       o.min_log_odds = logOddsFromProbability(0.01f);
       o.max_log_odds = logOddsFromProbability(0.99f);
-      launchOccupancyIntegrate(m->frame_blocks, m->frame_count, m->tsdf.blocks, depth_dev, mask_dev, mask_mode, rows,
-                               cols, T_C_L, *cam, p, o, m->num_sms, m->bits, grid.num_words, m->stream);
+      launchOccupancyIntegrate(m->frame_blocks.get(), m->frame_count, m->tsdf.blocks, depth_dev, mask_dev, mask_mode, rows,
+                               cols, T_C_L, *cam, p, o, m->num_sms, m->bits.get(), grid.num_words, m->stream);
     } else {
       // the slab's tensor descriptor follows reallocations (growLayer) by being re-encoded when base or capacity changed
       if (tsdfUseTma() && (m->tsdf_tmap.base != m->tsdf.blocks || m->tsdf_tmap.capacity != m->tsdf.capacity)) {
         if (encodeBlockTensorMap(&m->tsdf_tmap, m->tsdf.blocks, m->tsdf.capacity, kTsdfBlockBytes))
           return fail(NVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the TSDF slab");
       }
-      launchTsdfIntegrate(m->frame_blocks, m->frame_count, m->tsdf.blocks, depth_dev, mask_dev, mask_mode, rows, cols,
-                          T_C_L, *cam, p, m->num_sms, m->bits, grid.num_words, tsdfUseTma() ? &m->tsdf_tmap : nullptr, m->stream);
+      launchTsdfIntegrate(m->frame_blocks.get(), m->frame_count, m->tsdf.blocks, depth_dev, mask_dev, mask_mode, rows, cols,
+                          T_C_L, *cam, p, m->num_sms, m->bits.get(), grid.num_words, tsdfUseTma() ? &m->tsdf_tmap : nullptr, m->stream);
     }
     endStage(m);
     m->launches++;
@@ -1052,11 +997,11 @@ int readFrameList(NvbMapper* m, int32_t* out_xyz, int32_t cap, int32_t* out_coun
   int want = 0;
   if (out_xyz && cap > 0 && m->h_list) {
     want = std::min<long long>(std::min<long long>(cap, kHostListCap), (long long)m->last_frame_n * 3 / 2 + 512);
-    want = std::min(want, m->frame_cap);
+    want = (int)std::min<size_t>(want, m->frame_blocks.size());
   }
   NVB_CUDA(cudaMemcpyAsync(m->h_ints, m->frame_count, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   if (want > 0)
-    NVB_CUDA(cudaMemcpyAsync(m->h_list, m->frame_blocks, (size_t)want * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(m->h_list, m->frame_blocks.get(), (size_t)want * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
   int rc = enqueueErrorCopies(m);
   if (rc) return rc;
   NVB_CUDA(syncAll(m));
@@ -1069,7 +1014,7 @@ int readFrameList(NvbMapper* m, int32_t* out_xyz, int32_t cap, int32_t* out_coun
     std::vector<int4> tmp;
     if (k > want) {  // the frame has more blocks than the speculative prefix: one more copy
       tmp.resize((size_t)k);
-      NVB_CUDA(cudaMemcpy(tmp.data(), m->frame_blocks, (size_t)k * sizeof(int4), cudaMemcpyDeviceToHost));
+      NVB_CUDA(cudaMemcpy(tmp.data(), m->frame_blocks.get(), (size_t)k * sizeof(int4), cudaMemcpyDeviceToHost));
       src = tmp.data();
     }
     for (int i = 0; i < k; i++) out_xyz[3 * i] = src[i].x, out_xyz[3 * i + 1] = src[i].y, out_xyz[3 * i + 2] = src[i].z;
@@ -1097,20 +1042,14 @@ int enqueueEsdf(NvbMapper* m, const int* in_xyz_dev, int n_explicit, bool from_t
   if ((rc = ensureEsdfCapacity(m, (long long)std::min(m->tsdf_count_ub, m->tsdf.capacity) + m->esdf_extra_ub))) return rc;
   if (slice) {
     // column set + column list sized to the projective layer
-    const size_t want = (size_t)nextPow2(2ll * std::max(m->tsdf.capacity, upper));
-    if (m->colset_n < want || m->cols_cap < std::max(m->tsdf.capacity, upper)) {
-      NVB_CUDA(syncAll(m));
-      if (m->colset) cudaFree(m->colset);
-      if (m->cols) cudaFree(m->cols);
-      NVB_CUDA(cudaMalloc(&m->colset, want * sizeof(unsigned long long)));
-      m->colset_n = want;
-      m->cols_cap = std::max(m->tsdf.capacity, upper);
-      NVB_CUDA(cudaMalloc(&m->cols, (size_t)m->cols_cap * 2 * sizeof(int)));
-    }
+    const size_t columns = std::max(m->tsdf.capacity, upper);
+    const size_t want = (size_t)nextPow2(2ll * columns);
+    NVB_CUDA(m->colset.grow(m, want, want));
+    NVB_CUDA(m->cols.grow(m, 2 * columns, 2 * columns));
   }
   m->update_seq++;
   EsdfCtx c = makeEsdfCtx(m);
-  c.tracker_dirty = from_tracker ? m->dirty : nullptr;
+  c.tracker_dirty = from_tracker ? m->dirty.get() : nullptr;
   c.tracker_todo_count = from_tracker ? m->todo_count : nullptr;
   if (slice) {
     // getBlockAndVoxelIndexFrom1DPositionInLayer (core/internal/impl/indexing_impl.h:105-115), on the host like the
@@ -1136,11 +1075,11 @@ int enqueueEsdf(NvbMapper* m, const int* in_xyz_dev, int n_explicit, bool from_t
   cudaError_t e;
   auto allocAndMark = [&](cudaStream_t st) {
     if (slice) {
-      launchEsdfSliceAllocateAndMark(c, from_tracker ? nullptr : in_xyz_dev, from_tracker ? m->todo_slots : nullptr,
+      launchEsdfSliceAllocateAndMark(c, from_tracker ? nullptr : in_xyz_dev, from_tracker ? m->todo_slots.get() : nullptr,
                                      from_tracker ? m->todo_count : nullptr, from_tracker ? upper : n_explicit, m->num_sms, st);
       m->launches += 3;
     } else {
-      if (from_tracker) launchEsdfAllocate(c, nullptr, m->todo_slots, m->todo_count, upper, st);
+      if (from_tracker) launchEsdfAllocate(c, nullptr, m->todo_slots.get(), m->todo_count, upper, st);
       else launchEsdfAllocate(c, in_xyz_dev, nullptr, nullptr, n_explicit, st);
       launchEsdfMark(c, upper, m->num_sms, st);
       m->launches += 2;
@@ -1301,24 +1240,19 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   if (m->projective_layer_type == NVB_PROJECTIVE_TSDF_WITH_FREESPACE &&
       (rc = allocLayer(&m->freespace, tcap, kFreespaceBlockBytes, m->stream)))
     return rc;
-  if ((rc = allocTsdfSide(m, 0, tcap))) return rc;
-  if ((rc = allocEsdfScratch(m, 0, ecap))) return rc;
-  NVB_CUDA(cudaMalloc(&m->esdf_ints, kNumInts * sizeof(int)));
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints, 0, kNumInts * sizeof(int), m->stream));
+  if ((rc = allocTsdfSide(m, tcap))) return rc;
+  if ((rc = allocEsdfScratch(m, ecap))) return rc;
+  NVB_CUDA(m->esdf_ints.grow(m, kNumInts, kNumInts, 0));
   const int one = 1;
-  NVB_CUDA(cudaMemcpyAsync(m->esdf_ints + kRingId, &one, sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  m->todo_count = m->esdf_ints + kTodoCount;
-  m->frame_count = m->esdf_ints + kFrameCount;
-  m->error_dev = m->esdf_ints + kError;
-  NVB_CUDA(cudaMalloc(&m->clr_bits, 2048 * sizeof(unsigned int)));
-  NVB_CUDA(cudaMalloc(&m->stats, 16 * sizeof(long long)));
-  NVB_CUDA(cudaMemsetAsync(m->stats, 0, 16 * sizeof(long long), m->stream));
-  NVB_CUDA(cudaMalloc(&m->phase_max, 4000 * sizeof(unsigned long long)));
-  NVB_CUDA(cudaMemsetAsync(m->phase_max, 0, 4000 * sizeof(unsigned long long), m->stream));
-  NVB_CUDA(cudaMalloc(&m->barrier, 64));
-  NVB_CUDA(cudaMemsetAsync(m->barrier, 0, 64, m->stream));
-  NVB_CUDA(cudaMalloc(&m->ticket, 64));
-  NVB_CUDA(cudaMemsetAsync(m->ticket, 0, 64, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(m->esdf_ints.get() + kRingId, &one, sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  m->todo_count = m->esdf_ints.get() + kTodoCount;
+  m->frame_count = m->esdf_ints.get() + kFrameCount;
+  m->error_dev = m->esdf_ints.get() + kError;
+  NVB_CUDA(m->clr_bits.grow(m, 2048, 2048));
+  NVB_CUDA(m->stats.grow(m, 16, 16, 0));
+  NVB_CUDA(m->phase_max.grow(m, 4000, 4000, 0));
+  NVB_CUDA(m->barrier.grow(m, 16, 16, 0));  // 64 bytes
+  NVB_CUDA(m->ticket.grow(m, 16, 16, 0));   // 64 bytes
   NVB_CUDA(cudaMallocHost(&m->h_ints, 64 * sizeof(int)));
   memset(m->h_ints, 0, 64 * sizeof(int));
   NVB_CUDA(cudaMallocHost(&m->h_list, (size_t)kHostListCap * sizeof(int4)));
@@ -1375,41 +1309,16 @@ void nvb_mapper_destroy(NvbMapper* m) {
   freeLayer(&m->tsdf), freeLayer(&m->esdf);
   if (m->freespace.blocks) freeLayer(&m->freespace);
   if (m->color.blocks) freeLayer(&m->color);
-  cudaFree(m->color_work), cudaFree(m->color_synth), cudaFree(m->color_stage), cudaFree(m->color_mask_stage);
-  cudaFree(m->dirty_fs), cudaFree(m->todo_fs_slots), cudaFree(m->fs_work), cudaFree(m->colset), cudaFree(m->cols);
-  cudaFree(m->bits), cudaFree(m->frame_blocks), cudaFree(m->tile_state), cudaFree(m->ticket);
   for (int k = 0; k < kStagingBuffers; k++) {
-    cudaFree(m->depth_stage[k]), cudaFree(m->mask_stage[k]);
     cudaEventDestroy(m->stage_copied[k]), cudaEventDestroy(m->stage_consumed[k]);
   }
-  cudaFree(m->dirty), cudaFree(m->todo_slots);
-  cudaFree(m->work), cudaFree(m->esdf_ints), cudaFree(m->upd_list), cudaFree(m->clr_list), cudaFree(m->cleared_list);
-  cudaFree(m->ring_a), cudaFree(m->ring_b), cudaFree(m->stamp_a), cudaFree(m->stamp_b);
-  cudaFree(m->nbr), cudaFree(m->seed_upd), cudaFree(m->seed_clr), cudaFree(m->psum);
-  cudaFree(m->nbr27), cudaFree(m->shadow), cudaFree(m->cand_stamp), cudaFree(m->cand_a), cudaFree(m->cand_b);
-  cudaFree(m->xslab), cudaFree(m->xrec), cudaFree(m->xcounts);
-  cudaFree(m->dead), cudaFree(m->skip_stamp), cudaFree(m->dead_cleared_xyz), cudaFree(m->last_depth);
-  cudaFree(m->shape_sel), cudaFree(m->shapes_dev);
-  cudaFree(m->gp_keys), cudaFree(m->gp_sort_temp), cudaFree(m->gp_fit_stage);
-  cudaFree(m->gp_slots), cudaFree(m->gp_counts), cudaFree(m->gp_totals), cudaFree(m->gp_crossings), cudaFree(m->gp_candidates);
-  cudaFree(m->gp_fit_points), cudaFree(m->gp_states), cudaFree(m->gp_costs), cudaFree(m->gp_planes), cudaFree(m->gp_result);
-  cudaFree(m->pre_depth);
-  cudaFree(m->dyn_depth), cudaFree(m->dyn_mask), cudaFree(m->dyn_clean), cudaFree(m->dyn_overlay), cudaFree(m->dyn_points);
-  cudaFree(m->dyn_counts), cudaFree(m->dyn_totals), cudaFree(m->cc_labels), cudaFree(m->cc_sizes), cudaFree(m->cc_stage);
   if (m->dyn_event) cudaEventDestroy(m->dyn_event);
   if (m->query_event) cudaEventDestroy(m->query_event);
-  cudaFree(m->union_list), cudaFree(m->union_list_count);
   if (m->mesh.blocks) freeLayer(&m->mesh);
-  cudaFree(m->mesh_v), cudaFree(m->mesh_n), cudaFree(m->mesh_t), cudaFree(m->mesh_c), cudaFree(m->mesh_state);
-  cudaFree(m->mesh_alt_v), cudaFree(m->mesh_alt_n), cudaFree(m->mesh_alt_t), cudaFree(m->mesh_alt_c);
-  cudaFree(m->mesh_counts), cudaFree(m->mesh_offsets), cudaFree(m->mesh_xyz_dev), cudaFree(m->dirty_mesh), cudaFree(m->todo_mesh_slots);
-  cudaFree(m->clr_bits), cudaFree(m->union_bits), cudaFree(m->union_state);
-  cudaFree(m->vc_bits[0]), cudaFree(m->vc_bits[1]);
-  cudaFree(m->stats), cudaFree(m->barrier), cudaFree(m->phase_max), cudaFree(m->xyz_upload);
   cudaFreeHost(m->h_ints), cudaFreeHost(m->h_count_ring), cudaFreeHost(m->h_list);
   for (int k = 0; k < kCountRing; k++) cudaEventDestroy(m->count_events[k]);
   cudaStreamDestroy(m->stream), cudaStreamDestroy(m->copy_stream);
-  delete m;
+  delete m;  // the device buffers free themselves
 }
 
 int32_t nvb_mapper_clear(NvbMapper* m) {
@@ -1429,17 +1338,17 @@ int32_t nvb_mapper_clear(NvbMapper* m) {
     NVB_CUDA(cudaMemsetAsync(L->free_count, 0, sizeof(int), m->stream));
     launchFillU64(L->hash.keys, kEmptyKey, (size_t)L->hash.mask + 1, m->stream);
   }
-  NVB_CUDA(cudaMemsetAsync(m->dirty, 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->dirty.get(), 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
   NVB_CUDA(cudaMemsetAsync(m->todo_count, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints + kClearedCount, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints + kClearedSeq, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints + kDeadClearedCount, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->seed_upd, 0, (size_t)m->esdf.capacity * sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->seed_clr, 0, (size_t)m->esdf.capacity * sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->psum, 0, 2 * (size_t)m->esdf.capacity * sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kClearedCount, 0, sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kClearedSeq, 0, sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kDeadClearedCount, 0, sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->seed_upd.get(), 0, (size_t)m->esdf.capacity * sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->seed_clr.get(), 0, (size_t)m->esdf.capacity * sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->psum.get(), 0, 2 * (size_t)m->esdf.capacity * sizeof(int), m->stream));
   m->prune_ok = m->prune_default;  // an empty layer: every summary is exact again
-  NVB_CUDA(cudaMemsetAsync(m->nbr, 0xFE, (size_t)m->esdf.capacity * 6 * sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->nbr27, 0xFE, (size_t)m->esdf.capacity * 27 * sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->nbr.get(), 0xFE, (size_t)m->esdf.capacity * 6 * sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->nbr27.get(), 0xFE, (size_t)m->esdf.capacity * 27 * sizeof(int), m->stream));
   NVB_CUDA(cudaMemsetAsync(m->error_dev, 0, sizeof(int), m->stream));
   m->tracker_initialized = false;
   m->fs_tracker_initialized = false;
@@ -1449,14 +1358,14 @@ int32_t nvb_mapper_clear(NvbMapper* m) {
     NVB_CUDA(cudaMemsetAsync(m->mesh.count, 0, sizeof(int), m->stream));
     NVB_CUDA(cudaMemsetAsync(m->mesh.free_count, 0, sizeof(int), m->stream));
     launchFillU64(m->mesh.hash.keys, kEmptyKey, (size_t)m->mesh.hash.mask + 1, m->stream);
-    NVB_CUDA(cudaMemsetAsync(m->mesh_state, 0, kArenaInts * sizeof(int), m->stream));
-    NVB_CUDA(cudaMemsetAsync(m->esdf_ints + kTodoMeshCount, 0, sizeof(int), m->stream));
-    NVB_CUDA(cudaMemsetAsync(m->dirty_mesh, 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
+    NVB_CUDA(cudaMemsetAsync(m->mesh_state.get(), 0, kArenaInts * sizeof(int), m->stream));
+    NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kTodoMeshCount, 0, sizeof(int), m->stream));
+    NVB_CUDA(cudaMemsetAsync(m->dirty_mesh.get(), 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
   }
   m->esdf_mode = 0;
   m->fs_last_update_ms = 0;
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints + kTodoFsCount, 0, sizeof(int), m->stream));
-  if (m->dirty_fs) NVB_CUDA(cudaMemsetAsync(m->dirty_fs, 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kTodoFsCount, 0, sizeof(int), m->stream));
+  if (m->dirty_fs.get()) NVB_CUDA(cudaMemsetAsync(m->dirty_fs.get(), 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
   m->has_last_view = false;
   m->tsdf_count_ub = 0, m->tsdf_count_confirmed = 0, m->esdf_extra_ub = 0;
   m->cells_cum = 0, m->confirmed_cum = 0;
@@ -1565,21 +1474,10 @@ int32_t nvb_mapper_get_occupancy_decay_params(const NvbMapper* m, NvbOccupancyDe
 namespace {
 // The dead list (projective capacity) and the ESDF side's dead-cleared list (ESDF capacity) of a deallocation.
 int ensureRemovalScratch(NvbMapper* m) {
-  if (m->dead_cap < m->tsdf.capacity) {
-    if (m->dead) cudaFree(m->dead);
-    NVB_CUDA(cudaMalloc(&m->dead, (size_t)m->tsdf.capacity * sizeof(int4)));
-    m->dead_cap = m->tsdf.capacity;
-  }
-  if (m->dead_cleared_cap < m->esdf.capacity) {
-    int* q = nullptr;
-    NVB_CUDA(cudaMalloc(&q, (size_t)m->esdf.capacity * 3 * sizeof(int)));
-    if (m->dead_cleared_xyz) {
-      NVB_CUDA(cudaMemcpy(q, m->dead_cleared_xyz, (size_t)m->dead_cleared_cap * 3 * sizeof(int), cudaMemcpyDeviceToDevice));
-      cudaFree(m->dead_cleared_xyz);
-    }
-    m->dead_cleared_xyz = q;
-    m->dead_cleared_cap = m->esdf.capacity;
-  }
+  const size_t dead = m->tsdf.capacity;
+  NVB_CUDA(m->dead.grow(m, dead, dead));
+  const size_t cleared = 3 * (size_t)m->esdf.capacity;
+  NVB_CUDA(m->dead_cleared_xyz.grow(m, cleared, cleared, kNoFill, kKeepContents));
   return NVB_OK;
 }
 
@@ -1588,7 +1486,7 @@ int ensureRemovalScratch(NvbMapper* m) {
 // the freespace, colour and mesh twins go, every touched hash is rebuilt without them, and the indices join
 // cleared_blocks_. `removed` receives the dead list. The tracker is the caller's.
 int removeDeadBlocks(NvbMapper* m, int n_dead, std::vector<int4>* removed) {
-  const int* dead_count = m->esdf_ints + kDeadCount;
+  const int* dead_count = m->esdf_ints.get() + kDeadCount;
   EsdfCtx c = makeEsdfCtx(m);
   if (m->esdf_mode == 2) {
     c.slice_mode = 1;
@@ -1597,23 +1495,23 @@ int removeDeadBlocks(NvbMapper* m, int n_dead, std::vector<int4>* removed) {
     c.slice_max_bz = (int)std::floor(m->sp.slice_max_height_m / m->block_size);
     c.slice_out_bz = (int)std::floor(m->sp.slice_height_m / m->block_size);
   }
-  launchEsdfRemoveBlocks(c, m->dead, dead_count, n_dead, m->stream);
+  launchEsdfRemoveBlocks(c, m->dead.get(), dead_count, n_dead, m->stream);
   // Voxels of other blocks may keep parents inside the removed blocks: the reference clears them when they happen to be
   // candidates of a later clear pass, which the per-block parent boxes cannot tell. No pruning from here on.
   m->prune_ok = false;
   std::vector<DevLayer*> touched = {&m->tsdf, &m->esdf};
   if (m->freespace.blocks) {
-    launchRemoveBlocks(m->freespace, m->dead, dead_count, n_dead, m->stream);
+    launchRemoveBlocks(m->freespace, m->dead.get(), dead_count, n_dead, m->stream);
     touched.push_back(&m->freespace);
   }
   if (m->color.blocks) {
-    launchRemoveBlocks(m->color, m->dead, dead_count, n_dead, m->stream);
+    launchRemoveBlocks(m->color, m->dead.get(), dead_count, n_dead, m->stream);
     touched.push_back(&m->color);
   }
   // ColorMeshLayer::clearBlocksAsync (Mapper::clearBlocksInLayers, src/mapper/mapper.cpp:552-557): the arena segments
   // of the removed headers are no longer referenced and are dropped by the next arena repack
   if (m->mesh.blocks) {
-    launchRemoveBlocks(m->mesh, m->dead, dead_count, n_dead, m->stream);
+    launchRemoveBlocks(m->mesh, m->dead.get(), dead_count, n_dead, m->stream);
     touched.push_back(&m->mesh);
   }
   for (DevLayer* L : touched) {
@@ -1627,7 +1525,7 @@ int removeDeadBlocks(NvbMapper* m, int n_dead, std::vector<int4>* removed) {
   m->launches += 6;
   // cleared_blocks_.insert (mapper.cpp:631-633)
   removed->resize((size_t)n_dead);
-  NVB_CUDA(cudaMemcpyAsync(removed->data(), m->dead, (size_t)n_dead * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(removed->data(), m->dead.get(), (size_t)n_dead * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   for (const int4& d : *removed) m->cleared_blocks.insert({d.y, d.z, d.w});
   return NVB_OK;
@@ -1662,12 +1560,7 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
   // scratch sized to the layer
   int rc = ensureRemovalScratch(m);
   if (rc) return rc;
-  if (m->skip_cap < P.capacity) {
-    if (m->skip_stamp) cudaFree(m->skip_stamp);
-    NVB_CUDA(cudaMalloc(&m->skip_stamp, (size_t)P.capacity * sizeof(int)));
-    NVB_CUDA(cudaMemsetAsync(m->skip_stamp, 0, (size_t)P.capacity * sizeof(int), m->stream));
-    m->skip_cap = P.capacity;
-  }
+  NVB_CUDA(m->skip_stamp.grow(m, P.capacity, P.capacity, 0));
   DecayArgs a{};
   a.layer = P;
   a.occupancy = occupancy ? 1 : 0;
@@ -1691,15 +1584,15 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
   }
   // block exclusion
   std::vector<int> excl;
-  int* excl_dev = nullptr;
+  DeviceArray<int> excl_dev;
   if (exclusion && exclusion->num_excluded_blocks > 0) {
     const int ne = exclusion->num_excluded_blocks;
-    NVB_CUDA(cudaMalloc(&excl_dev, (size_t)ne * 3 * sizeof(int)));
-    NVB_CUDA(cudaMemcpyAsync(excl_dev, exclusion->excluded_blocks_xyz_host, (size_t)ne * 3 * sizeof(int), cudaMemcpyHostToDevice,
+    NVB_CUDA(excl_dev.grow(m, (size_t)ne * 3, (size_t)ne * 3));
+    NVB_CUDA(cudaMemcpyAsync(excl_dev.get(), exclusion->excluded_blocks_xyz_host, (size_t)ne * 3 * sizeof(int), cudaMemcpyHostToDevice,
                              m->stream));
     m->skip_seq++;
-    launchMarkSkipped(P, excl_dev, ne, m->skip_stamp, m->skip_seq, m->stream);
-    a.skip_stamp = m->skip_stamp;
+    launchMarkSkipped(P, excl_dev.get(), ne, m->skip_stamp.get(), m->skip_seq, m->stream);
+    a.skip_stamp = m->skip_stamp.get();
     a.skip_seq = m->skip_seq;
   }
   if (exclusion && exclusion->has_exclusion_sphere && exclusion->exclusion_radius_m * exclusion->exclusion_radius_m > 0.0f) {
@@ -1708,34 +1601,32 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
     a.r2 = exclusion->exclusion_radius_m * exclusion->exclusion_radius_m;
   }
   // view exclusion
-  float* depth_tmp = nullptr;
+  DeviceArray<float> depth_tmp;
   if (depth) {
     const float* depth_dev = depth;
     if (depth_memory == NVB_MEM_HOST) {
-      NVB_CUDA(cudaMalloc(&depth_tmp, (size_t)rows * cols * sizeof(float)));
-      NVB_CUDA(cudaMemcpyAsync(depth_tmp, depth, (size_t)rows * cols * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-      depth_dev = depth_tmp;
+      NVB_CUDA(depth_tmp.grow(m, (size_t)rows * cols, (size_t)rows * cols));
+      NVB_CUDA(cudaMemcpyAsync(depth_tmp.get(), depth, (size_t)rows * cols * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+      depth_dev = depth_tmp.get();
     }
     a.depth = depth_dev, a.rows = rows, a.cols = cols;
     a.T_C_L = invertRigid(rigidFromColMajor(T_L_C));
     a.cam = *cam;
   }
-  a.dead = m->dead;
-  a.dead_count = m->esdf_ints + kDeadCount;
-  a.tracker_dirty = m->dirty;
+  a.dead = m->dead.get();
+  a.dead_count = m->esdf_ints.get() + kDeadCount;
+  a.tracker_dirty = m->dirty.get();
   NVB_CUDA(cudaMemsetAsync(a.dead_count, 0, sizeof(int), m->stream));
   launchDecay(a, m->num_sms, m->stream);
   m->launches++;
   int n_dead = 0;
   NVB_CUDA(cudaMemcpyAsync(&n_dead, a.dead_count, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  if (depth_tmp) cudaFree(depth_tmp);
-  if (excl_dev) cudaFree(excl_dev);
   if (n_dead > 0) {
     std::vector<int4> removed;
     if ((rc = removeDeadBlocks(m, n_dead, &removed))) return rc;
-    if (m->dirty_fs) NVB_CUDA(cudaMemsetAsync(m->dirty_fs, 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
-    if (m->dirty_mesh) NVB_CUDA(cudaMemsetAsync(m->dirty_mesh, 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
+    if (m->dirty_fs.get()) NVB_CUDA(cudaMemsetAsync(m->dirty_fs.get(), 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
+    if (m->dirty_mesh.get()) NVB_CUDA(cudaMemsetAsync(m->dirty_mesh.get(), 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
     if (out_count) *out_count = n_dead;
     if (removed_xyz_host && cap > 0) {
       const int k = std::min(n_dead, (int)cap);
@@ -1748,8 +1639,8 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
   m->fs_tracker_initialized = false;
   m->mesh_tracker_initialized = false;
   NVB_CUDA(cudaMemsetAsync(m->todo_count, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints + kTodoFsCount, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints + kTodoMeshCount, 0, sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kTodoFsCount, 0, sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kTodoMeshCount, 0, sizeof(int), m->stream));
   NVB_CUDA(syncAll(m));
   return checkDeviceError(m);
 }
@@ -1788,20 +1679,15 @@ int freespaceUpdateImpl(NvbMapper* m, const int* in_xyz_dev, int n_explicit, lon
   int upper = in_xyz_dev ? n_explicit : std::min(m->tsdf_count_ub, m->tsdf.capacity);
   if (!in_xyz_dev) pollCounts(m), upper = std::min(m->tsdf_count_ub, m->tsdf.capacity);
   if (upper < 1) upper = 1;
-  if (m->fs_work_cap < upper) {
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    if (m->fs_work) cudaFree(m->fs_work);
-    NVB_CUDA(cudaMalloc(&m->fs_work, (size_t)upper * 2 * sizeof(int4)));
-    m->fs_work_cap = upper * 2;
-  }
+  NVB_CUDA(m->fs_work.grow(m, upper, 2 * (size_t)upper));
   FreespaceArgs a{};
   a.tsdf = m->tsdf, a.fs = m->freespace;
   if (in_xyz_dev) {
     a.in_xyz = in_xyz_dev, a.n_explicit = n_explicit;
   } else {
-    a.todo_slots = m->todo_fs_slots, a.todo_count = m->esdf_ints + kTodoFsCount, a.tracker_dirty = m->dirty_fs;
+    a.todo_slots = m->todo_fs_slots.get(), a.todo_count = m->esdf_ints.get() + kTodoFsCount, a.tracker_dirty = m->dirty_fs.get();
   }
-  a.work = m->fs_work, a.work_count = m->esdf_ints + kFsWorkCount, a.error = m->error_dev;
+  a.work = m->fs_work.get(), a.work_count = m->esdf_ints.get() + kFsWorkCount, a.error = m->error_dev;
   a.max_tsdf_distance_for_occupancy_m = m->fp.max_tsdf_distance_for_occupancy_m;
   a.max_unobserved_ms = m->fp.max_unobserved_to_keep_consecutive_occupancy_ms;
   a.min_free_ms = m->fp.min_duration_since_occupied_for_freespace_ms;
@@ -1814,13 +1700,13 @@ int freespaceUpdateImpl(NvbMapper* m, const int* in_xyz_dev, int n_explicit, lon
   a.p.half_voxel_size = m->block_size * (0.5f / kVps);
   a.p.max_integration_distance_m = max_view_distance_m > 0.0f ? max_view_distance_m : FLT_MAX;
   a.p.truncation_distance_m = truncation_distance_m > 0.0f ? truncation_distance_m : FLT_MAX;
-  float* depth_tmp = nullptr;
+  DeviceArray<float> depth_tmp;
   if (depth) {
     const float* depth_dev = depth;
     if (memory == NVB_MEM_HOST) {
-      NVB_CUDA(cudaMalloc(&depth_tmp, (size_t)rows * cols * sizeof(float)));
-      NVB_CUDA(cudaMemcpyAsync(depth_tmp, depth, (size_t)rows * cols * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-      depth_dev = depth_tmp;
+      NVB_CUDA(depth_tmp.grow(m, (size_t)rows * cols, (size_t)rows * cols));
+      NVB_CUDA(cudaMemcpyAsync(depth_tmp.get(), depth, (size_t)rows * cols * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+      depth_dev = depth_tmp.get();
     }
     a.depth = depth_dev, a.rows = rows, a.cols = cols;
     a.T_C_L = invertRigid(rigidFromColMajor(T_L_C));
@@ -1830,7 +1716,6 @@ int freespaceUpdateImpl(NvbMapper* m, const int* in_xyz_dev, int n_explicit, lon
   m->launches += 2;
   m->fs_last_update_ms = now_ms;
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  if (depth_tmp) cudaFree(depth_tmp);
   return checkDeviceError(m);
 }
 }  // namespace
@@ -1847,7 +1732,7 @@ int32_t nvb_mapper_update_freespace(NvbMapper* m, int64_t update_time_ms, const 
   }
   NVB_CUDA(cudaSetDevice(m->device));
   if (!m->fs_tracker_initialized || update_full_layer) {
-    launchTodoAll(m->tsdf, m->dirty_fs, m->todo_fs_slots, m->esdf_ints + kTodoFsCount, m->stream);
+    launchTodoAll(m->tsdf, m->dirty_fs.get(), m->todo_fs_slots.get(), m->esdf_ints.get() + kTodoFsCount, m->stream);
     m->launches++;
     m->fs_tracker_initialized = true;
   }
@@ -1881,14 +1766,12 @@ int32_t nvb_freespace_update_blocks(NvbMapper* m, const int32_t* blocks_xyz_host
   std::sort(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x != b.x ? a.x < b.x : (a.y != b.y ? a.y < b.y : a.z < b.z); });
   v.erase(std::unique(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x == b.x && a.y == b.y && a.z == b.z; }), v.end());
   num_blocks = (int)v.size();
-  int* xyz_dev = nullptr;
-  NVB_CUDA(cudaMalloc(&xyz_dev, (size_t)num_blocks * 3 * sizeof(int)));
-  NVB_CUDA(cudaMemcpyAsync(xyz_dev, v.data(), (size_t)num_blocks * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  DeviceArray<int> xyz_dev;
+  NVB_CUDA(xyz_dev.grow(m, (size_t)num_blocks * 3, (size_t)num_blocks * 3));
+  NVB_CUDA(cudaMemcpyAsync(xyz_dev.get(), v.data(), (size_t)num_blocks * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  const int rc = freespaceUpdateImpl(m, xyz_dev, num_blocks, update_time_ms, depth, depth_memory, rows, cols, T_L_C, cam,
-                                     max_view_distance_m, truncation_distance_m);
-  cudaFree(xyz_dev);
-  return rc;
+  return freespaceUpdateImpl(m, xyz_dev.get(), num_blocks, update_time_ms, depth, depth_memory, rows, cols, T_L_C, cam,
+                             max_view_distance_m, truncation_distance_m);
 }
 
 int32_t nvb_mapper_decay_exclude_last_view(NvbMapper* m, const NvbDecayExclusion* exclusion, int32_t* removed_xyz_host,
@@ -1897,7 +1780,7 @@ int32_t nvb_mapper_decay_exclude_last_view(NvbMapper* m, const NvbDecayExclusion
   if (!m->keep_last_view) return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper was created without keep_last_view");
   if (!m->has_last_view)  // "Last view not set for sensor type. Decaying all voxels" (mapper_impl.h:200-203)
     return nvb_mapper_decay(m, exclusion, nullptr, 0, 0, 0, nullptr, nullptr, removed_xyz_host, cap, out_count);
-  return nvb_mapper_decay(m, exclusion, m->last_depth, NVB_MEM_DEVICE, m->last_rows, m->last_cols, m->last_T_L_C,
+  return nvb_mapper_decay(m, exclusion, m->last_depth.get(), NVB_MEM_DEVICE, m->last_rows, m->last_cols, m->last_T_L_C,
                           &m->last_cam, removed_xyz_host, cap, out_count);
 }
 
@@ -1910,25 +1793,25 @@ int32_t nvb_mapper_clear_outside_radius(NvbMapper* m, const float center[3], flo
   int rc = ensureRemovalScratch(m);
   if (rc) return rc;
   // getBlocksOutsideRadius over the projective layer's blocks (TSDF for kTsdf / kTsdfWithFreespace, occupancy for kOccupancy)
-  int* dead_count = m->esdf_ints + kDeadCount;
+  int* dead_count = m->esdf_ints.get() + kDeadCount;
   NVB_CUDA(cudaMemsetAsync(dead_count, 0, sizeof(int), m->stream));
-  launchSelectOutsideRadius(m->tsdf, center, radius, m->block_size, m->dead, dead_count, m->stream);
+  launchSelectOutsideRadius(m->tsdf, center, radius, m->block_size, m->dead.get(), dead_count, m->stream);
   m->launches++;
   int n = 0;
   NVB_CUDA(cudaMemcpyAsync(&n, dead_count, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   if (n == 0) return checkDeviceError(m);
   // {Tsdf,Occupancy}Layer::clearBlocksAsync
-  launchRemoveBlocks(m->tsdf, m->dead, dead_count, n, m->stream);
+  launchRemoveBlocks(m->tsdf, m->dead.get(), dead_count, n, m->stream);
   // BlocksToUpdateTracker::removeClearedBlocksFromTracking: out of every initialised consumer's list; no switch to
   // update-all (unlike the decay)
-  launchTrackerDropDead(m->dead, dead_count, n, m->dirty, m->dirty_fs, m->dirty_mesh, m->stream);
+  launchTrackerDropDead(m->dead.get(), dead_count, n, m->dirty.get(), m->dirty_fs.get(), m->dirty_mesh.get(), m->stream);
   m->launches += 2;
-  if (m->tracker_initialized) launchDropDeadSlots(m->tsdf, m->todo_slots, m->todo_count, m->stream), m->launches++;
-  if (m->dirty_fs && m->fs_tracker_initialized)
-    launchDropDeadSlots(m->tsdf, m->todo_fs_slots, m->esdf_ints + kTodoFsCount, m->stream), m->launches++;
-  if (m->dirty_mesh && m->mesh_tracker_initialized)
-    launchDropDeadSlots(m->tsdf, m->todo_mesh_slots, m->esdf_ints + kTodoMeshCount, m->stream), m->launches++;
+  if (m->tracker_initialized) launchDropDeadSlots(m->tsdf, m->todo_slots.get(), m->todo_count, m->stream), m->launches++;
+  if (m->dirty_fs.get() && m->fs_tracker_initialized)
+    launchDropDeadSlots(m->tsdf, m->todo_fs_slots.get(), m->esdf_ints.get() + kTodoFsCount, m->stream), m->launches++;
+  if (m->dirty_mesh.get() && m->mesh_tracker_initialized)
+    launchDropDeadSlots(m->tsdf, m->todo_mesh_slots.get(), m->esdf_ints.get() + kTodoMeshCount, m->stream), m->launches++;
   std::vector<int4> removed;
   if ((rc = removeDeadBlocks(m, n, &removed))) return rc;
   if (out_count) *out_count = n;
@@ -1948,33 +1831,24 @@ int clearShapesImpl(NvbMapper* m, DevLayer* L, int voxel_kind, bool track, const
   if (num_shapes == 0 || !L) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));  // an update_esdf_async may still be reading the layer
-  if (m->shape_sel_cap < L->capacity) {
-    if (m->shape_sel) cudaFree(m->shape_sel);
-    m->shape_sel = nullptr;
-    NVB_CUDA(cudaMalloc(&m->shape_sel, ((size_t)L->capacity + 1) * sizeof(int4)));
-    m->shape_sel_cap = L->capacity;
-  }
-  if (m->shapes_cap < num_shapes) {
-    if (m->shapes_dev) cudaFree(m->shapes_dev);
-    m->shapes_dev = nullptr;
-    NVB_CUDA(cudaMalloc(&m->shapes_dev, (size_t)num_shapes * sizeof(NvbBoundingShape)));
-    m->shapes_cap = num_shapes;
-  }
-  NVB_CUDA(cudaMemcpyAsync(m->shapes_dev, shapes, (size_t)num_shapes * sizeof(NvbBoundingShape), cudaMemcpyHostToDevice,
+  const size_t sel = (size_t)L->capacity + 1;  // the count, then the list
+  NVB_CUDA(m->shape_sel.grow(m, sel, sel));
+  NVB_CUDA(m->shapes_dev.grow(m, num_shapes, num_shapes));
+  NVB_CUDA(cudaMemcpyAsync(m->shapes_dev.get(), shapes, (size_t)num_shapes * sizeof(NvbBoundingShape), cudaMemcpyHostToDevice,
                            m->stream));
   ShapeClearArgs a{};
   a.layer = *L;
   a.voxel_kind = voxel_kind;
-  a.shapes = m->shapes_dev, a.num_shapes = num_shapes;
+  a.shapes = m->shapes_dev.get(), a.num_shapes = num_shapes;
   a.block_size = m->block_size;
-  a.sel_count = reinterpret_cast<int*>(m->shape_sel);
-  a.sel = m->shape_sel + 1;
+  a.sel_count = reinterpret_cast<int*>(m->shape_sel.get());
+  a.sel = m->shape_sel.get() + 1;
   if (track) {
-    if (m->tracker_initialized) a.dirty = m->dirty, a.todo_slots = m->todo_slots, a.todo_count = m->todo_count;
-    if (m->dirty_fs && m->fs_tracker_initialized)
-      a.dirty2 = m->dirty_fs, a.todo2_slots = m->todo_fs_slots, a.todo2_count = m->esdf_ints + kTodoFsCount;
-    if (m->dirty_mesh && m->mesh_tracker_initialized)
-      a.dirty3 = m->dirty_mesh, a.todo3_slots = m->todo_mesh_slots, a.todo3_count = m->esdf_ints + kTodoMeshCount;
+    if (m->tracker_initialized) a.dirty = m->dirty.get(), a.todo_slots = m->todo_slots.get(), a.todo_count = m->todo_count;
+    if (m->dirty_fs.get() && m->fs_tracker_initialized)
+      a.dirty2 = m->dirty_fs.get(), a.todo2_slots = m->todo_fs_slots.get(), a.todo2_count = m->esdf_ints.get() + kTodoFsCount;
+    if (m->dirty_mesh.get() && m->mesh_tracker_initialized)
+      a.dirty3 = m->dirty_mesh.get(), a.todo3_slots = m->todo_mesh_slots.get(), a.todo3_count = m->esdf_ints.get() + kTodoMeshCount;
   }
   NVB_CUDA(cudaMemsetAsync(a.sel_count, 0, sizeof(int), m->stream));
   launchShapeSelect(a, m->stream);
@@ -2096,16 +1970,16 @@ int32_t nvb_mapper_mark_unobserved_free_inside_radius(NvbMapper* m, const float 
   a.block_size = m->block_size;
   a.trunc_m = m->tp.truncation_distance_vox * m->voxel_size;  // get_truncation_distance_m(layer->voxel_size())
   a.error = m->error_dev;
-  if (m->tracker_initialized) a.dirty = m->dirty, a.todo_slots = m->todo_slots, a.todo_count = m->todo_count;
-  if (m->dirty_fs && m->fs_tracker_initialized)
-    a.dirty2 = m->dirty_fs, a.todo2_slots = m->todo_fs_slots, a.todo2_count = m->esdf_ints + kTodoFsCount;
-  if (m->dirty_mesh && m->mesh_tracker_initialized)
-    a.dirty3 = m->dirty_mesh, a.todo3_slots = m->todo_mesh_slots, a.todo3_count = m->esdf_ints + kTodoMeshCount;
-  int4* out_dev = nullptr;
-  NVB_CUDA(cudaMalloc(&out_dev, ((size_t)cells + 1) * sizeof(int4)));
-  a.out = out_dev + 1;
-  a.out_count = reinterpret_cast<int*>(out_dev);
-  NVB_CUDA(cudaMemsetAsync(out_dev, 0, sizeof(int4), m->stream));
+  if (m->tracker_initialized) a.dirty = m->dirty.get(), a.todo_slots = m->todo_slots.get(), a.todo_count = m->todo_count;
+  if (m->dirty_fs.get() && m->fs_tracker_initialized)
+    a.dirty2 = m->dirty_fs.get(), a.todo2_slots = m->todo_fs_slots.get(), a.todo2_count = m->esdf_ints.get() + kTodoFsCount;
+  if (m->dirty_mesh.get() && m->mesh_tracker_initialized)
+    a.dirty3 = m->dirty_mesh.get(), a.todo3_slots = m->todo_mesh_slots.get(), a.todo3_count = m->esdf_ints.get() + kTodoMeshCount;
+  DeviceArray<int4> out_dev;
+  NVB_CUDA(out_dev.grow(m, (size_t)cells + 1, (size_t)cells + 1));
+  a.out = out_dev.get() + 1;
+  a.out_count = reinterpret_cast<int*>(out_dev.get());
+  NVB_CUDA(cudaMemsetAsync(out_dev.get(), 0, sizeof(int4), m->stream));
   launchMarkFreeSphere(a, m->num_sms, m->stream);
   m->launches++;
   int n = 0;
@@ -2120,7 +1994,6 @@ int32_t nvb_mapper_mark_unobserved_free_inside_radius(NvbMapper* m, const float 
     for (int i = 0; i < k; i++)
       updated_xyz_host[3 * i] = tmp[i].x, updated_xyz_host[3 * i + 1] = tmp[i].y, updated_xyz_host[3 * i + 2] = tmp[i].z;
   }
-  cudaFree(out_dev);
   return checkDeviceError(m);
 }
 
@@ -2188,12 +2061,7 @@ int ensureColorLayer(NvbMapper* m) {
   } else if (m->color.capacity < m->tsdf.capacity) {
     if ((rc = growLayer(m, &m->color, m->tsdf.capacity))) return rc;
   }
-  if (m->color_work_cap < m->tsdf.capacity) {
-    NVB_CUDA(syncAll(m));
-    if (m->color_work) cudaFree(m->color_work);
-    NVB_CUDA(cudaMalloc(&m->color_work, (size_t)m->tsdf.capacity * sizeof(int4)));
-    m->color_work_cap = m->tsdf.capacity;
-  }
+  NVB_CUDA(m->color_work.grow(m, m->tsdf.capacity, m->tsdf.capacity));
   return NVB_OK;
 }
 
@@ -2216,24 +2084,14 @@ int fillTracerArgs(NvbMapper* m, ColorArgs* a, const float* T_L_C_cm, const NvbC
   a->max_ray_len = m->cp.sphere_tracer_maximum_ray_length_m;
   a->eps_m = m->cp.sphere_tracer_surface_distance_epsilon_vox * m->voxel_size;
   const size_t need = (size_t)a->drows * a->dcols;
-  if (m->color_synth_cap < need) {
-    NVB_CUDA(syncAll(m));
-    if (m->color_synth) cudaFree(m->color_synth);
-    NVB_CUDA(cudaMalloc(&m->color_synth, need * sizeof(float)));
-    m->color_synth_cap = need;
-  }
-  a->synth = m->color_synth;
+  NVB_CUDA(m->color_synth.grow(m, need, need));
+  a->synth = m->color_synth.get();
   return NVB_OK;
 }
 
-int stageBytes(NvbMapper* m, unsigned char** buf, size_t* cap, const unsigned char* host, size_t bytes) {
-  if (*cap < bytes) {
-    NVB_CUDA(syncAll(m));
-    if (*buf) cudaFree(*buf);
-    NVB_CUDA(cudaMalloc(buf, bytes));
-    *cap = bytes;
-  }
-  NVB_CUDA(cudaMemcpyAsync(*buf, host, bytes, cudaMemcpyHostToDevice, m->stream));
+int stageBytes(NvbMapper* m, DeviceArray<unsigned char>* buf, const unsigned char* host, size_t bytes) {
+  NVB_CUDA(buf->grow(m, bytes, bytes));
+  NVB_CUDA(cudaMemcpyAsync(buf->get(), host, bytes, cudaMemcpyHostToDevice, m->stream));
   return NVB_OK;
 }
 }  // namespace
@@ -2316,20 +2174,20 @@ int32_t nvb_mapper_integrate_color(NvbMapper* m, const uint8_t* color, const uin
     w_old /= total, w_new /= total;
     a.w_old_h = roundThroughHalf(w_old), a.w_new_h = roundThroughHalf(w_new);
   }
-  a.work = m->color_work;
-  a.work_count = m->esdf_ints + kColorWorkCount;
+  a.work = m->color_work.get();
+  a.work_count = m->esdf_ints.get() + kColorWorkCount;
   a.error = m->error_dev;
   a.rows = rows, a.cols = cols;
   a.depth_subsample = rows / a.drows;  // projective_integrator_impl.cuh:320
   if (a.depth_subsample <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "the colour image is smaller than the synthetic depth image");
   a.mask_mode = mask_mode;
   if (memory == NVB_MEM_HOST) {
-    if ((rc = stageBytes(m, &m->color_stage, &m->color_stage_cap, color, (size_t)rows * cols * 3))) return rc;
-    a.color_image = m->color_stage;
+    if ((rc = stageBytes(m, &m->color_stage, color, (size_t)rows * cols * 3))) return rc;
+    a.color_image = m->color_stage.get();
     a.mask = nullptr;
     if (mask) {
-      if ((rc = stageBytes(m, &m->color_mask_stage, &m->color_mask_stage_cap, mask, (size_t)rows * cols))) return rc;
-      a.mask = m->color_mask_stage;
+      if ((rc = stageBytes(m, &m->color_mask_stage, mask, (size_t)rows * cols))) return rc;
+      a.mask = m->color_mask_stage.get();
     }
   } else {
     a.color_image = color, a.mask = mask;
@@ -2351,16 +2209,16 @@ int32_t nvb_mapper_integrate_color(NvbMapper* m, const uint8_t* color, const uin
 int32_t nvb_mapper_last_color_blocks(NvbMapper* m, int32_t* out_xyz_host, int32_t cap, int32_t* out_count) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
   if (out_count) *out_count = 0;
-  if (!m->color.blocks || !m->color_work) return NVB_OK;
+  if (!m->color.blocks || !m->color_work.get()) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   int n = 0;
-  NVB_CUDA(cudaMemcpyAsync(&n, m->esdf_ints + kColorWorkCount, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(&n, m->esdf_ints.get() + kColorWorkCount, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   if (out_count) *out_count = n;
   if (out_xyz_host && cap > 0 && n > 0) {
     const int k = std::min(n, (int)cap);
     std::vector<int4> tmp((size_t)k);
-    NVB_CUDA(cudaMemcpyAsync(tmp.data(), m->color_work, (size_t)k * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(tmp.data(), m->color_work.get(), (size_t)k * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
     NVB_CUDA(cudaStreamSynchronize(m->stream));
     for (int i = 0; i < k; i++)
       out_xyz_host[3 * i] = tmp[i].x, out_xyz_host[3 * i + 1] = tmp[i].y, out_xyz_host[3 * i + 2] = tmp[i].z;
@@ -2383,7 +2241,7 @@ int32_t nvb_mapper_update_esdf_async(NvbMapper* m, int32_t update_full_layer) {
   if (!m->tracker_initialized || update_full_layer) {
     // First query of the tracker, or UpdateFullLayer::kYes: every TSDF block
     // (map/blocks_to_update_tracker.cpp:107-124, src/mapper/mapper.cpp:523-537).
-    launchTodoAll(m->tsdf, m->dirty, m->todo_slots, m->todo_count, m->stream);
+    launchTodoAll(m->tsdf, m->dirty.get(), m->todo_slots.get(), m->todo_count, m->stream);
     m->launches++;
     m->tracker_initialized = true;
   }
@@ -2417,17 +2275,12 @@ int32_t nvb_esdf_integrate_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, 
   for (const K& k : v)
     if (!indexInRange(k.x, k.y, k.z)) return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
   const int n = (int)v.size();
-  if (n > m->xyz_upload_cap) {
-    NVB_CUDA(syncAll(m));
-    if (m->xyz_upload) cudaFree(m->xyz_upload);
-    NVB_CUDA(cudaMalloc(&m->xyz_upload, (size_t)n * 2 * 3 * sizeof(int)));
-    m->xyz_upload_cap = n * 2;
-  }
+  NVB_CUDA(m->xyz_upload.grow(m, 3 * (size_t)n, 6 * (size_t)n));
   // Stream-ordered upload: a blocking cudaMemcpy from pageable memory may return before the DMA has landed,
   // and the mapper's stream is non-blocking (not ordered against the legacy default stream).
-  NVB_CUDA(cudaMemcpyAsync(m->xyz_upload, v.data(), (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(m->xyz_upload.get(), v.data(), (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));  // v is pageable and about to go out of scope
-  int rc = enqueueEsdf(m, m->xyz_upload, n, false);
+  int rc = enqueueEsdf(m, m->xyz_upload.get(), n, false);
   if (rc) return rc;
   if ((rc = nvb_mapper_synchronize(m))) return rc;
   return tightenEsdfBound(m);
@@ -2467,7 +2320,7 @@ static int32_t updateEsdfSliceImpl(NvbMapper* m, const float* plane, int32_t upd
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
   NVB_CUDA(cudaSetDevice(m->device));
   if (!m->tracker_initialized || update_full_layer) {
-    launchTodoAll(m->tsdf, m->dirty, m->todo_slots, m->todo_count, m->stream);
+    launchTodoAll(m->tsdf, m->dirty.get(), m->todo_slots.get(), m->todo_count, m->stream);
     m->launches++;
     m->tracker_initialized = true;
   }
@@ -2493,15 +2346,10 @@ static int32_t integrateSliceBlocksImpl(NvbMapper* m, const float* plane, const 
   for (int i = 0; i < num_blocks; i++)
     if (!indexInRange(blocks_xyz_host[3 * i], blocks_xyz_host[3 * i + 1], blocks_xyz_host[3 * i + 2]))
       return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
-  if (num_blocks > m->xyz_upload_cap) {
-    NVB_CUDA(syncAll(m));
-    if (m->xyz_upload) cudaFree(m->xyz_upload);
-    NVB_CUDA(cudaMalloc(&m->xyz_upload, (size_t)num_blocks * 2 * 3 * sizeof(int)));
-    m->xyz_upload_cap = num_blocks * 2;
-  }
-  NVB_CUDA(cudaMemcpyAsync(m->xyz_upload, blocks_xyz_host, (size_t)num_blocks * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(m->xyz_upload.grow(m, 3 * (size_t)num_blocks, 6 * (size_t)num_blocks));
+  NVB_CUDA(cudaMemcpyAsync(m->xyz_upload.get(), blocks_xyz_host, (size_t)num_blocks * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  int rc = enqueueEsdf(m, m->xyz_upload, num_blocks, false, true, plane);
+  int rc = enqueueEsdf(m, m->xyz_upload.get(), num_blocks, false, true, plane);
   if (rc) return rc;
   if ((rc = nvb_mapper_synchronize(m))) return rc;
   return tightenEsdfBound(m);
@@ -2531,55 +2379,31 @@ int32_t nvb_mapper_get_ground_plane_params(const NvbMapper* m, NvbGroundPlanePar
 }  // extern "C"
 
 namespace {
-// Grows a device array to at least n elements (contents not kept).
-template <typename T>
-int ensureDevice(T** p, int* cap, long long n) {
-  if (*cap >= n) return NVB_OK;
-  const long long want = std::max(n, 2ll * *cap);
-  if (*p) cudaFree(*p);
-  *p = nullptr;
-  *cap = 0;
-  NVB_CUDA(cudaMalloc(p, (size_t)want * sizeof(T)));
-  *cap = (int)want;
-  return NVB_OK;
-}
-
 // RansacPlaneFitter::fit on n points already on the device (float4); the generator states of new iterations are made
 // once and kept.
 int ransacFit(NvbMapper* m, const float4* pts, int n, int iterations, float threshold, float plane[4], int* found) {
   *found = 0;
   if (n < 3) return NVB_OK;  // "We need at least three points to form a plane"
-  if (iterations > m->gp_states_n) {
-    // The existing states are kept; the new array replaces them only once it is complete (no leak on failure).
-    void* st = nullptr;
-    NVB_CUDA(cudaMalloc(&st, (size_t)iterations * ransacStateBytes()));
-    cudaError_t e = cudaSuccess;
-    if (m->gp_states_n)
-      e = cudaMemcpyAsync(st, m->gp_states, (size_t)m->gp_states_n * ransacStateBytes(), cudaMemcpyDeviceToDevice, m->stream);
-    if (e == cudaSuccess) {
-      launchRansacInit(st, m->gp_states_n, iterations, m->stream);
-      m->launches++;
-      e = cudaStreamSynchronize(m->stream);
-    }
-    if (e != cudaSuccess) {
-      cudaFree(st);
-      return fail(NVB_ERR_CUDA, std::string("RANSAC generator states: ") + cudaGetErrorString(e));
-    }
-    cudaFree(m->gp_states);
-    m->gp_states = st;
-    m->gp_states_n = iterations;
+  const size_t have = m->gp_states.size() / ransacStateBytes();
+  if ((size_t)iterations > have) {
+    const size_t bytes = (size_t)iterations * ransacStateBytes();
+    NVB_CUDA(m->gp_states.grow(m, bytes, bytes, kNoFill, kKeepContents));
+    launchRansacInit(m->gp_states.get(), (int)have, iterations, m->stream);
+    m->launches++;
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
   }
-  int rc = ensureDevice(&m->gp_costs, &m->gp_costs_cap, iterations);
-  if (!rc) rc = ensureDevice(&m->gp_planes, &m->gp_planes_cap, iterations);
-  if (rc) return rc;
-  if (!m->gp_result) NVB_CUDA(cudaMalloc(&m->gp_result, 5 * sizeof(float)));
+  const size_t it = iterations;
+  NVB_CUDA(m->gp_costs.grow(m, it, std::max(it, 2 * m->gp_costs.size())));
+  NVB_CUDA(m->gp_planes.grow(m, it, std::max(it, 2 * m->gp_planes.size())));
+  NVB_CUDA(m->gp_result.grow(m, 5, 5));
   // A/B switch for measurements: the reference's launch shape (256-thread CTAs, points read from global memory)
   const char* e = getenv("NVB_RANSAC_REFERENCE_SHAPE");
   const bool reference_shape = e && atoi(e) == 1;
-  launchRansacFit(pts, n, iterations, threshold, m->gp_states, m->gp_costs, m->gp_planes, m->gp_result, reference_shape, m->stream);
+  launchRansacFit(pts, n, iterations, threshold, m->gp_states.get(), m->gp_costs.get(), m->gp_planes.get(), m->gp_result.get(),
+                  reference_shape, m->stream);
   m->launches += 2;
   float out[5];
-  NVB_CUDA(cudaMemcpyAsync(out, m->gp_result, sizeof(out), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(out, m->gp_result.get(), sizeof(out), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   int f = 0;
   std::memcpy(&f, &out[4], sizeof(int));
@@ -2613,53 +2437,43 @@ int32_t nvb_mapper_compute_ground_plane(NvbMapper* m, float plane[4], int32_t* f
   if (hw == 0) return NVB_OK;  // "tsdf_layer.numBlocks() == 0"
   // The slots below the high-water mark in (x, y, z) block-index order, sorted on the device; free slots sort last and
   // count nothing (a layer whose slots are all free gives no crossings, hence no plane, like an empty one).
-  if (hw > m->gp_blocks_cap) {
-    const int cap = std::max(hw, 2 * m->gp_blocks_cap);
-    int dummy = 0, rc = ensureDevice(&m->gp_keys, &dummy, 2ll * cap);
-    if (!rc) dummy = 0, rc = ensureDevice(&m->gp_slots, &dummy, 2ll * cap);
-    if (!rc) dummy = 0, rc = ensureDevice(&m->gp_counts, &dummy, cap);
-    if (rc) {
-      m->gp_blocks_cap = 0;
-      return rc;
-    }
-    m->gp_blocks_cap = cap;
-  }
+  const size_t blocks = hw;
+  const size_t cap = std::max(blocks, 2 * m->gp_counts.size());
+  NVB_CUDA(m->gp_keys.grow(m, 2 * blocks, 2 * cap));
+  NVB_CUDA(m->gp_slots.grow(m, 2 * blocks, 2 * cap));
+  NVB_CUDA(m->gp_counts.grow(m, blocks, cap));
   const size_t temp_bytes = groundSortTempBytes(hw);
-  if (temp_bytes > m->gp_sort_temp_bytes) {
-    cudaFree(m->gp_sort_temp);
-    m->gp_sort_temp = nullptr;
-    m->gp_sort_temp_bytes = 0;
-    NVB_CUDA(cudaMalloc(&m->gp_sort_temp, temp_bytes));
-    m->gp_sort_temp_bytes = temp_bytes;
-  }
+  NVB_CUDA(m->gp_sort_temp.grow(m, temp_bytes, temp_bytes));
   int rc = NVB_OK;
-  if (!m->gp_totals) NVB_CUDA(cudaMalloc(&m->gp_totals, 2 * sizeof(int)));
-  NVB_CUDA(launchGroundSortBlocks(m->tsdf, hw, m->gp_keys, m->gp_slots, m->gp_sort_temp, m->gp_sort_temp_bytes, m->stream));
+  NVB_CUDA(m->gp_totals.grow(m, 2, 2));
+  NVB_CUDA(launchGroundSortBlocks(m->tsdf, hw, m->gp_keys.get(), m->gp_slots.get(), m->gp_sort_temp.get(), m->gp_sort_temp.size(),
+                                  m->stream));
   m->launches += 2;
   GroundExtractArgs a{};
   a.tsdf = m->tsdf;
-  a.slots = m->gp_slots + hw, a.num_blocks = hw;
-  a.counts = m->gp_counts, a.totals = m->gp_totals;
+  a.slots = m->gp_slots.get() + hw, a.num_blocks = hw;
+  a.counts = m->gp_counts.get(), a.totals = m->gp_totals.get();
   a.block_size = m->block_size, a.voxel_size = m->voxel_size;
   a.min_tsdf_weight = m->gp.min_tsdf_weight;
   a.min_z = m->gp.ground_points_candidates_min_z_m, a.max_z = m->gp.ground_points_candidates_max_z_m;
   launchGroundCount(a, m->stream);
   m->launches += 2;
   int totals[2];
-  NVB_CUDA(cudaMemcpyAsync(totals, m->gp_totals, sizeof(totals), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(totals, m->gp_totals.get(), sizeof(totals), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   // "Maximum number of crossings reached." (tsdf_zero_crossings_extractor.cu:126-131)
   if (totals[0] >= m->gp.max_crossings) return checkDeviceError(m);
-  if ((rc = ensureDevice(&m->gp_crossings, &m->gp_crossings_cap, std::max(totals[0], 1)))) return rc;
-  if ((rc = ensureDevice(&m->gp_candidates, &m->gp_candidates_cap, std::max(totals[1], 1)))) return rc;
-  a.crossings = m->gp_crossings, a.candidates = m->gp_candidates;
+  const size_t crossings = std::max(totals[0], 1), candidates = std::max(totals[1], 1);
+  NVB_CUDA(m->gp_crossings.grow(m, crossings, std::max(crossings, 2 * m->gp_crossings.size())));
+  NVB_CUDA(m->gp_candidates.grow(m, candidates, std::max(candidates, 2 * m->gp_candidates.size())));
+  a.crossings = m->gp_crossings.get(), a.candidates = m->gp_candidates.get();
   launchGroundEmit(a, m->stream);
   m->launches++;
   m->gp_valid = true;
   m->gp_num_crossings = totals[0], m->gp_num_candidates = totals[1];
   int f = 0;
   float pl[4];
-  if ((rc = ransacFit(m, m->gp_candidates, totals[1], m->gp.num_ransac_iterations, m->gp.ransac_distance_threshold_m, pl, &f))) {
+  if ((rc = ransacFit(m, m->gp_candidates.get(), totals[1], m->gp.num_ransac_iterations, m->gp.ransac_distance_threshold_m, pl, &f))) {
     groundReset(m);
     return rc;
   }
@@ -2693,11 +2507,11 @@ int32_t nvb_mapper_ground_plane_points(NvbMapper* m, int32_t which, float* xyz, 
   if (!xyz || k == 0) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   if (which == NVB_GROUND_POINTS_CROSSINGS) {
-    NVB_CUDA(cudaMemcpyAsync(xyz, m->gp_crossings, (size_t)k * sizeof(float3), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(xyz, m->gp_crossings.get(), (size_t)k * sizeof(float3), cudaMemcpyDeviceToHost, m->stream));
     NVB_CUDA(cudaStreamSynchronize(m->stream));
   } else {
     std::vector<float4> c((size_t)k);
-    NVB_CUDA(cudaMemcpyAsync(c.data(), m->gp_candidates, (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(c.data(), m->gp_candidates.get(), (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, m->stream));
     NVB_CUDA(cudaStreamSynchronize(m->stream));
     for (int i = 0; i < k; i++) xyz[3 * i] = c[i].x, xyz[3 * i + 1] = c[i].y, xyz[3 * i + 2] = c[i].z;
   }
@@ -2713,19 +2527,20 @@ int32_t nvb_ransac_fit_plane(NvbMapper* m, const float* points, int32_t memory, 
   *found = 0;
   if (n < 3) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
-  int rc = ensureDevice(&m->gp_fit_points, &m->gp_fit_points_cap, n);
-  if (rc) return rc;
+  const size_t points_n = n;
+  NVB_CUDA(m->gp_fit_points.grow(m, points_n, std::max(points_n, 2 * m->gp_fit_points.size())));
   const float* src = points;
   if (memory == NVB_MEM_HOST) {
     // staged on the device for the packing kernel, in a buffer kept by the mapper
-    if ((rc = ensureDevice(&m->gp_fit_stage, &m->gp_fit_stage_cap, 3ll * n))) return rc;
-    NVB_CUDA(cudaMemcpyAsync(m->gp_fit_stage, points, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    src = m->gp_fit_stage;
+    NVB_CUDA(m->gp_fit_stage.grow(m, 3 * points_n, std::max(3 * points_n, 2 * m->gp_fit_stage.size())));
+    NVB_CUDA(cudaMemcpyAsync(m->gp_fit_stage.get(), points, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    src = m->gp_fit_stage.get();
   }
-  launchPackPoints(src, n, m->gp_fit_points, m->stream);
+  launchPackPoints(src, n, m->gp_fit_points.get(), m->stream);
   m->launches++;
   int f = 0;
-  if ((rc = ransacFit(m, m->gp_fit_points, n, num_ransac_iterations, ransac_distance_threshold_m, plane, &f))) return rc;
+  int rc;
+  if ((rc = ransacFit(m, m->gp_fit_points.get(), n, num_ransac_iterations, ransac_distance_threshold_m, plane, &f))) return rc;
   *found = f;
   return checkDeviceError(m);
 }
@@ -2736,32 +2551,17 @@ namespace {
 constexpr long long kMaxDynamicsPixels = 1ll << 28;  // 3-byte overlay and 12-byte points per pixel stay below 2^32
 
 // Grows the detector's per-pixel buffers (nothing is kept: the next call rewrites them). Growing synchronises first, so
-// that no pending kernel, and no consumer ordered behind this stream, still reads the old buffers.
+// that no pending kernel, and no consumer ordered behind this mapper's streams, still reads the old buffers.
 int ensureDynamicsBuffers(NvbMapper* m, int pixels) {
-  const int tiles = dynamicsNumTiles(pixels);
-  if (pixels > m->dyn_pixels_cap) {
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(m->dyn_depth), cudaFree(m->dyn_mask), cudaFree(m->dyn_clean), cudaFree(m->dyn_overlay), cudaFree(m->dyn_points);
-    m->dyn_depth = nullptr, m->dyn_mask = m->dyn_clean = m->dyn_overlay = nullptr, m->dyn_points = nullptr;
-    m->dyn_pixels_cap = 0;
-    NVB_CUDA(cudaMalloc(&m->dyn_depth, (size_t)pixels * sizeof(float)));
-    NVB_CUDA(cudaMalloc(&m->dyn_mask, (size_t)pixels));
-    NVB_CUDA(cudaMalloc(&m->dyn_clean, (size_t)pixels));
-    NVB_CUDA(cudaMalloc(&m->dyn_overlay, (size_t)pixels * 3));
-    NVB_CUDA(cudaMalloc(&m->dyn_points, (size_t)pixels * 3 * sizeof(float)));
-    m->dyn_pixels_cap = pixels;
-  }
-  if (tiles > m->dyn_tiles_cap) {
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(m->dyn_counts);
-    m->dyn_counts = nullptr, m->dyn_tiles_cap = 0;
-    NVB_CUDA(cudaMalloc(&m->dyn_counts, (size_t)tiles * sizeof(int2)));
-    m->dyn_tiles_cap = tiles;
-  }
-  if (!m->dyn_totals) {
-    NVB_CUDA(cudaMalloc(&m->dyn_totals, 2 * sizeof(int)));
-    NVB_CUDA(cudaMemsetAsync(m->dyn_totals, 0, 2 * sizeof(int), m->stream));
-  }
+  const size_t n = pixels;
+  NVB_CUDA(m->dyn_depth.grow(m, n, n));
+  NVB_CUDA(m->dyn_mask.grow(m, n, n));
+  NVB_CUDA(m->dyn_clean.grow(m, n, n));
+  NVB_CUDA(m->dyn_overlay.grow(m, 3 * n, 3 * n));
+  NVB_CUDA(m->dyn_points.grow(m, 3 * n, 3 * n));
+  const size_t tiles = dynamicsNumTiles(pixels);
+  NVB_CUDA(m->dyn_counts.grow(m, tiles, tiles));
+  NVB_CUDA(m->dyn_totals.grow(m, 2, 2, 0));
   return NVB_OK;
 }
 
@@ -2790,17 +2590,17 @@ int32_t nvb_mapper_compute_dynamics(NvbMapper* m, const float* depth, int32_t me
   const int pixels = rows * cols;
   if ((rc = ensureDynamicsBuffers(m, pixels))) return rc;
   // The freespace layer is written on `stream` only (nvb_mapper_update_freespace); the detection follows it there.
-  NVB_CUDA(cudaMemcpyAsync(m->dyn_depth, depth, (size_t)pixels * sizeof(float),
+  NVB_CUDA(cudaMemcpyAsync(m->dyn_depth.get(), depth, (size_t)pixels * sizeof(float),
                            memory == NVB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, m->stream));
   DynamicsArgs a{};
-  a.depth = m->dyn_depth, a.rows = rows, a.cols = cols;
+  a.depth = m->dyn_depth.get(), a.rows = rows, a.cols = cols;
   a.T_L_C = rigidFromColMajor(T_L_C);
   a.cam = *cam;
   a.fs = m->freespace;
   a.block_size = m->block_size;
   a.voxel_size_inv = (float)(1.0 / (double)(m->block_size * (1.0f / kVps)));  // 1.0 / blockSizeToVoxelSize(block_size)
-  a.mask = m->dyn_mask, a.overlay = m->dyn_overlay, a.counts = m->dyn_counts, a.points = m->dyn_points;
-  launchDynamicsDetect(a, m->dyn_totals, m->stream);
+  a.mask = m->dyn_mask.get(), a.overlay = m->dyn_overlay.get(), a.counts = m->dyn_counts.get(), a.points = m->dyn_points.get();
+  launchDynamicsDetect(a, m->dyn_totals.get(), m->stream);
   m->launches += 3;
   m->dyn_rows = rows, m->dyn_cols = cols;
   return NVB_OK;
@@ -2827,34 +2627,21 @@ int32_t nvb_mapper_remove_small_components(NvbMapper* m, const uint8_t* mask_in,
   CcArgs a{};
   a.rows = rows, a.cols = cols, a.drows = rows / 2, a.dcols = cols / 2;
   a.min_size = threshold / 4;  // size_threshold / (kDownScaleFactor * kDownScaleFactor)
-  const int down = std::max(a.drows * a.dcols, 1);
-  if (down > m->cc_cap) {
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(m->cc_labels), cudaFree(m->cc_sizes);
-    m->cc_labels = m->cc_sizes = nullptr, m->cc_cap = 0;
-    const int cap = std::max(down, 2 * m->cc_cap);
-    NVB_CUDA(cudaMalloc(&m->cc_labels, (size_t)cap * sizeof(int)));
-    NVB_CUDA(cudaMalloc(&m->cc_sizes, (size_t)cap * sizeof(int)));
-    m->cc_cap = cap;
-  }
-  a.labels = m->cc_labels, a.sizes = m->cc_sizes;
+  const size_t down = std::max(a.drows * a.dcols, 1);
+  NVB_CUDA(m->cc_labels.grow(m, down, std::max(down, 2 * m->cc_labels.size())));
+  NVB_CUDA(m->cc_sizes.grow(m, down, std::max(down, 2 * m->cc_sizes.size())));
+  a.labels = m->cc_labels.get(), a.sizes = m->cc_sizes.get();
   if (memory == NVB_MEM_HOST) {
-    if (pixels > m->cc_stage_cap) {
-      NVB_CUDA(cudaStreamSynchronize(m->stream));
-      cudaFree(m->cc_stage);
-      m->cc_stage = nullptr, m->cc_stage_cap = 0;
-      NVB_CUDA(cudaMalloc(&m->cc_stage, (size_t)pixels));
-      m->cc_stage_cap = pixels;
-    }
-    NVB_CUDA(cudaMemcpyAsync(m->cc_stage, mask_in, (size_t)pixels, cudaMemcpyHostToDevice, m->stream));
-    a.in = m->cc_stage, a.out = m->cc_stage;
+    NVB_CUDA(m->cc_stage.grow(m, pixels, pixels));
+    NVB_CUDA(cudaMemcpyAsync(m->cc_stage.get(), mask_in, (size_t)pixels, cudaMemcpyHostToDevice, m->stream));
+    a.in = m->cc_stage.get(), a.out = m->cc_stage.get();
   } else {
     a.in = mask_in, a.out = mask_out;
   }
   launchRemoveSmallComponents(a, m->num_sms, m->stream);
   m->launches += a.drows > 0 && a.dcols > 0 ? 4 : 1;
   if (memory == NVB_MEM_HOST) {
-    NVB_CUDA(cudaMemcpyAsync(mask_out, m->cc_stage, (size_t)pixels, cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(mask_out, m->cc_stage.get(), (size_t)pixels, cudaMemcpyDeviceToHost, m->stream));
     NVB_CUDA(cudaStreamSynchronize(m->stream));
   }
   return NVB_OK;
@@ -2865,7 +2652,7 @@ int32_t nvb_mapper_dynamic_mask(NvbMapper* m, uint8_t* out, int32_t memory, int3
   if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
   *rows = m->dyn_rows, *cols = m->dyn_cols;
   NVB_CUDA(cudaSetDevice(m->device));
-  return copyDynamicsOut(m, out, m->dyn_mask, (size_t)m->dyn_rows * m->dyn_cols, memory);
+  return copyDynamicsOut(m, out, m->dyn_mask.get(), (size_t)m->dyn_rows * m->dyn_cols, memory);
 }
 
 int32_t nvb_mapper_dynamic_overlay(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols) {
@@ -2873,27 +2660,27 @@ int32_t nvb_mapper_dynamic_overlay(NvbMapper* m, uint8_t* out, int32_t memory, i
   if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
   *rows = m->dyn_rows, *cols = m->dyn_cols;
   NVB_CUDA(cudaSetDevice(m->device));
-  return copyDynamicsOut(m, out, m->dyn_overlay, (size_t)m->dyn_rows * m->dyn_cols * 3, memory);
+  return copyDynamicsOut(m, out, m->dyn_overlay.get(), (size_t)m->dyn_rows * m->dyn_cols * 3, memory);
 }
 
 int32_t nvb_mapper_dynamic_points(NvbMapper* m, float* xyz, int32_t memory, int32_t cap, int32_t* out_count) {
   if (!m || !out_count) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
   *out_count = 0;
-  if (!m->dyn_totals) return NVB_OK;  // never computed
+  if (!m->dyn_totals.get()) return NVB_OK;  // never computed
   NVB_CUDA(cudaSetDevice(m->device));
   int n = 0;
-  NVB_CUDA(cudaMemcpyAsync(&n, m->dyn_totals, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(&n, m->dyn_totals.get(), sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   *out_count = n;
   const int k = std::min(n, std::max(cap, 0));
-  return copyDynamicsOut(m, xyz, m->dyn_points, (size_t)k * 3 * sizeof(float), memory);
+  return copyDynamicsOut(m, xyz, m->dyn_points.get(), (size_t)k * 3 * sizeof(float), memory);
 }
 
 int32_t nvb_mapper_dynamics_device_buffers(NvbMapper* m, NvbDynamicsBuffers* out) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  out->depth = m->dyn_depth, out->mask = m->dyn_mask, out->cleaned_mask = m->dyn_clean, out->overlay = m->dyn_overlay;
-  out->points = m->dyn_points, out->num_points = m->dyn_totals;
+  out->depth = m->dyn_depth.get(), out->mask = m->dyn_mask.get(), out->cleaned_mask = m->dyn_clean.get(), out->overlay = m->dyn_overlay.get();
+  out->points = m->dyn_points.get(), out->num_points = m->dyn_totals.get();
   out->rows = m->dyn_rows, out->cols = m->dyn_cols;
   return NVB_OK;
 }
@@ -2915,7 +2702,7 @@ int32_t nvb_esdf_slice_aabb(NvbMapper* m, float slice_height_m, float aabb_out[6
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   const int zb = (int)std::floor(slice_height_m / m->block_size);
-  int* box_dev = m->esdf_ints + kGesCounts;  // four scratch ints (the wavefront is idle)
+  int* box_dev = m->esdf_ints.get() + kGesCounts;  // four scratch ints (the wavefront is idle)
   const int init[4] = {INT32_MAX, INT32_MAX, INT32_MIN, INT32_MIN};
   NVB_CUDA(cudaMemcpyAsync(box_dev, init, sizeof(init), cudaMemcpyHostToDevice, m->stream));
   launchSliceAabb(m->esdf, zb, box_dev, m->stream);
@@ -2948,17 +2735,17 @@ int32_t nvb_esdf_slice_distance_image_in_aabb(NvbMapper* m, float slice_height_m
   *rows_out = rows, *cols_out = cols;
   const long long npix = (long long)rows * cols;
   if (npix <= 0 || (!image_host && !grid_host) || cap_pixels <= 0) return NVB_OK;
-  float* img_dev = nullptr;
-  signed char* grid_dev = nullptr;
-  if (image_host) NVB_CUDA(cudaMalloc(&img_dev, (size_t)npix * sizeof(float)));
-  if (grid_host) NVB_CUDA(cudaMalloc(&grid_dev, (size_t)npix));
-  launchSliceImage(m->esdf, bs, aabb[0], aabb[1], slice_height_m, unobserved_value, rows, cols, img_dev, grid_dev, m->stream);
+  DeviceArray<float> img_dev;
+  DeviceArray<signed char> grid_dev;
+  if (image_host) NVB_CUDA(img_dev.grow(m, npix, npix));
+  if (grid_host) NVB_CUDA(grid_dev.grow(m, npix, npix));
+  launchSliceImage(m->esdf, bs, aabb[0], aabb[1], slice_height_m, unobserved_value, rows, cols, img_dev.get(), grid_dev.get(),
+                   m->stream);
   m->launches++;
   const size_t k = (size_t)std::min<long long>(npix, cap_pixels);
-  if (image_host) NVB_CUDA(cudaMemcpyAsync(image_host, img_dev, k * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
-  if (grid_host) NVB_CUDA(cudaMemcpyAsync(grid_host, grid_dev, k, cudaMemcpyDeviceToHost, m->stream));
+  if (image_host) NVB_CUDA(cudaMemcpyAsync(image_host, img_dev.get(), k * sizeof(float), cudaMemcpyDeviceToHost, m->stream));
+  if (grid_host) NVB_CUDA(cudaMemcpyAsync(grid_host, grid_dev.get(), k, cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  cudaFree(img_dev), cudaFree(grid_dev);
   return NVB_OK;
 }
 
@@ -3022,23 +2809,16 @@ int32_t nvb_blocks_union(NvbMapper* m, const int32_t* xyz_dev, int32_t n, const 
   scratch.linear_size = 0;  // bitset + tile state only
   if ((rc = ensureFrameScratch(m, scratch))) return rc;
   const int need = std::min(n, g.linear_size);
-  if (need > m->union_list_cap) {
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    if (m->union_list) cudaFree(m->union_list);
-    m->union_list = nullptr, m->union_list_cap = 0;
-    const int cap2 = (int)std::min<long long>((long long)(1.5 * need) + 64, 0x7fffffff);
-    NVB_CUDA(cudaMalloc(&m->union_list, (size_t)cap2 * sizeof(int4)));
-    m->union_list_cap = cap2;
-  }
-  if (!m->union_list_count) NVB_CUDA(cudaMalloc(&m->union_list_count, sizeof(int)));
-  launchMarkList(xyz_dev, n, g, m->bits, m->stream);
+  NVB_CUDA(m->union_list.grow(m, need, (size_t)std::min<long long>((long long)(1.5 * need) + 64, 0x7fffffff)));
+  NVB_CUDA(m->union_list_count.grow(m, 1, 1));
+  launchMarkList(xyz_dev, n, g, m->bits.get(), m->stream);
   CompactArgs ca{};
-  ca.bits = m->bits;
+  ca.bits = m->bits.get();
   ca.grid = g;
-  ca.frame_blocks = m->union_list;
-  ca.frame_count = m->union_list_count;
-  ca.tile_state = m->tile_state;
-  ca.ticket = m->ticket;
+  ca.frame_blocks = m->union_list.get();
+  ca.frame_count = m->union_list_count.get();
+  ca.tile_state = m->tile_state.get();
+  ca.ticket = m->ticket.get();
   ca.ticket_base = m->ticket_base;
   ca.epoch = ++m->epoch;
   ca.allocate = 0;
@@ -3046,11 +2826,11 @@ int32_t nvb_blocks_union(NvbMapper* m, const int32_t* xyz_dev, int32_t n, const 
   ca.error = m->error_dev;
   launchCompactAllocate(ca, m->stream);
   if (compactUsesTickets(g)) m->ticket_base += (unsigned int)compactNumTiles(g);
-  launchClearBits(m->bits, g.num_words, m->stream);
-  if (out_xyz_dev && cap > 0) launchUnpackList(m->union_list, m->union_list_count, out_xyz_dev, cap, m->stream);
+  launchClearBits(m->bits.get(), g.num_words, m->stream);
+  if (out_xyz_dev && cap > 0) launchUnpackList(m->union_list.get(), m->union_list_count.get(), out_xyz_dev, cap, m->stream);
   m->launches += 4;
   if (out_count_host) {
-    NVB_CUDA(cudaMemcpyAsync(m->h_ints, m->union_list_count, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(m->h_ints, m->union_list_count.get(), sizeof(int), cudaMemcpyDeviceToHost, m->stream));
     NVB_CUDA(cudaStreamSynchronize(m->stream));
     *out_count_host = m->h_ints[0];
   }
@@ -3060,8 +2840,8 @@ int32_t nvb_blocks_union(NvbMapper* m, const int32_t* xyz_dev, int32_t n, const 
 int32_t nvb_mapper_append_frame_blocks(NvbMapper* m, int32_t* segment_dev, int32_t cap_entries) {
   if (!m || !segment_dev || cap_entries <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   NVB_CUDA(cudaSetDevice(m->device));
-  if (!m->frame_blocks) return NVB_OK;  // no frame integrated yet
-  launchAppendFrame(m->frame_blocks, m->frame_count, segment_dev, cap_entries, m->error_dev, m->stream);
+  if (!m->frame_blocks.get()) return NVB_OK;  // no frame integrated yet
+  launchAppendFrame(m->frame_blocks.get(), m->frame_count, segment_dev, cap_entries, m->error_dev, m->stream);
   m->launches++;
   return NVB_OK;
 }
@@ -3072,16 +2852,12 @@ int32_t nvb_blocks_union_segments(NvbMapper* m, const int32_t* segments_dev, int
       segment_stride_ints < 1 + 3 * cap_entries)
     return fail(NVB_ERR_INVALID_ARGUMENT, "bad argument");
   NVB_CUDA(cudaSetDevice(m->device));
-  if (!m->union_bits) {
-    // 2^28 cells = 32 MiB of bits: a union AABB of e.g. 1024 x 1024 x 256 blocks (410 m x 410 m x 102 m at 5 cm voxels)
-    m->union_bits_cap = 1ll << 28;
-    NVB_CUDA(cudaMalloc(&m->union_bits, (size_t)(m->union_bits_cap / 8)));
-    NVB_CUDA(cudaMemset(m->union_bits, 0, (size_t)(m->union_bits_cap / 8)));
-    NVB_CUDA(cudaMalloc(&m->union_state, 8 * sizeof(int)));
-    NVB_CUDA(cudaMemset(m->union_state, 0, 8 * sizeof(int)));
-  }
-  launchUnionSegments(segments_dev, num_segments, segment_stride_ints, cap_entries, m->union_state, m->union_bits, m->union_bits_cap,
-                      out_xyz_dev, out_cap, out_count_dev, stream ? (cudaStream_t)stream : m->stream);
+  // 2^28 cells = 32 MiB of bits: a union AABB of e.g. 1024 x 1024 x 256 blocks (410 m x 410 m x 102 m at 5 cm voxels)
+  constexpr long long kUnionCells = 1ll << 28;
+  NVB_CUDA(m->union_bits.grow(m, kUnionCells / 32, kUnionCells / 32, 0));
+  NVB_CUDA(m->union_state.grow(m, 8, 8, 0));
+  launchUnionSegments(segments_dev, num_segments, segment_stride_ints, cap_entries, m->union_state.get(), m->union_bits.get(),
+                      kUnionCells, out_xyz_dev, out_cap, out_count_dev, stream ? (cudaStream_t)stream : m->stream);
   m->launches += 5;
   return NVB_OK;
 }
@@ -3090,10 +2866,10 @@ int32_t nvb_blocks_union_status(NvbMapper* m, int32_t* out_error) {
   if (!m || !out_error) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   NVB_CUDA(cudaSetDevice(m->device));
   *out_error = 0;
-  if (m->union_state) {
+  if (m->union_state.get()) {
     NVB_CUDA(cudaDeviceSynchronize());
     int st[8];
-    NVB_CUDA(cudaMemcpy(st, m->union_state, sizeof(st), cudaMemcpyDeviceToHost));
+    NVB_CUDA(cudaMemcpy(st, m->union_state.get(), sizeof(st), cudaMemcpyDeviceToHost));
     *out_error = st[6];
   }
   return NVB_OK;
@@ -3111,7 +2887,7 @@ int32_t nvb_mapper_set_esdf_reserved_sms(NvbMapper* m, int32_t reserved_sms) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
   if (reserved_sms < 0 || reserved_sms > 64) return fail(NVB_ERR_INVALID_ARGUMENT, "reserved_sms must be in [0, 64]");
   m->esdf_reserved_sms = reserved_sms;
-  if (m->xrec && esdfWaveXGrid(m->num_sms, reserved_sms) != m->xseg_grid) return allocWaveXRecords(m, m->esdf.capacity);
+  if (m->xrec.get() && esdfWaveXGrid(m->num_sms, reserved_sms) != m->xseg_grid) return allocWaveXRecords(m, m->esdf.capacity);
   return NVB_OK;
 }
 int32_t nvb_mapper_get_esdf_reserved_sms(const NvbMapper* m) { return m ? m->esdf_reserved_sms : 0; }
@@ -3237,18 +3013,17 @@ int32_t nvb_layer_get_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
   if (n <= 0) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
-  int* xyz_dev = nullptr;
-  unsigned char *out_dev = nullptr, *found_dev = nullptr;
-  NVB_CUDA(cudaMalloc(&xyz_dev, (size_t)n * 3 * sizeof(int)));
-  NVB_CUDA(cudaMalloc(&out_dev, (size_t)n * L->block_bytes));
-  NVB_CUDA(cudaMalloc(&found_dev, (size_t)n));
-  NVB_CUDA(cudaMemcpyAsync(xyz_dev, xyz_host, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  launchGatherBlocks(*L, xyz_dev, n, out_dev, found_dev, m->stream);
+  DeviceArray<int> xyz_dev;
+  DeviceArray<unsigned char> out_dev, found_dev;
+  NVB_CUDA(xyz_dev.grow(m, (size_t)n * 3, (size_t)n * 3));
+  NVB_CUDA(out_dev.grow(m, (size_t)n * L->block_bytes, (size_t)n * L->block_bytes));
+  NVB_CUDA(found_dev.grow(m, n, n));
+  NVB_CUDA(cudaMemcpyAsync(xyz_dev.get(), xyz_host, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  launchGatherBlocks(*L, xyz_dev.get(), n, out_dev.get(), found_dev.get(), m->stream);
   m->launches++;
-  NVB_CUDA(cudaMemcpyAsync(out_host, out_dev, (size_t)n * L->block_bytes, cudaMemcpyDeviceToHost, m->stream));
-  if (found_host) NVB_CUDA(cudaMemcpyAsync(found_host, found_dev, (size_t)n, cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(out_host, out_dev.get(), (size_t)n * L->block_bytes, cudaMemcpyDeviceToHost, m->stream));
+  if (found_host) NVB_CUDA(cudaMemcpyAsync(found_host, found_dev.get(), (size_t)n, cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(syncAll(m));
-  cudaFree(xyz_dev), cudaFree(out_dev), cudaFree(found_dev);
   return NVB_OK;
 }
 
@@ -3272,24 +3047,23 @@ int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
   }
   L = layerOf(m, layer);
   NVB_CUDA(syncAll(m));
-  int* xyz_dev = nullptr;
-  unsigned char* in_dev = nullptr;
-  NVB_CUDA(cudaMalloc(&xyz_dev, (size_t)n * 3 * sizeof(int)));
-  NVB_CUDA(cudaMalloc(&in_dev, (size_t)n * L->block_bytes));
-  NVB_CUDA(cudaMemcpyAsync(xyz_dev, xyz_host, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  NVB_CUDA(cudaMemcpyAsync(in_dev, in_host, (size_t)n * L->block_bytes, cudaMemcpyHostToDevice, m->stream));
-  launchScatterBlocks(*L, xyz_dev, n, in_dev, m->error_dev, m->stream);
+  DeviceArray<int> xyz_dev;
+  DeviceArray<unsigned char> in_dev;
+  NVB_CUDA(xyz_dev.grow(m, (size_t)n * 3, (size_t)n * 3));
+  NVB_CUDA(in_dev.grow(m, (size_t)n * L->block_bytes, (size_t)n * L->block_bytes));
+  NVB_CUDA(cudaMemcpyAsync(xyz_dev.get(), xyz_host, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(in_dev.get(), in_host, (size_t)n * L->block_bytes, cudaMemcpyHostToDevice, m->stream));
+  launchScatterBlocks(*L, xyz_dev.get(), n, in_dev.get(), m->error_dev, m->stream);
   m->launches++;
   if (layer == NVB_LAYER_ESDF) m->prune_ok = false;  // voxels written from outside: the parent boxes are no longer bounds
   NVB_CUDA(syncAll(m));
-  cudaFree(xyz_dev), cudaFree(in_dev);
   if (layer == NVB_LAYER_TSDF) {
     // the tracker is told like after an integration: a later updateEsdf must see these blocks
     m->tracker_initialized = false;
   } else {
     // blocks created outside the ESDF update path are not linked: forget the neighbour table,
     // it is re-resolved lazily through the hash
-    NVB_CUDA(cudaMemsetAsync(m->nbr, 0xFE, (size_t)m->esdf.capacity * 6 * sizeof(int), m->stream));
+    NVB_CUDA(cudaMemsetAsync(m->nbr.get(), 0xFE, (size_t)m->esdf.capacity * 6 * sizeof(int), m->stream));
     NVB_CUDA(cudaStreamSynchronize(m->stream));
   }
   return checkDeviceError(m);
@@ -3326,7 +3100,7 @@ int32_t nvb_mapper_last_esdf_stats(NvbMapper* m, int64_t out[8]) {
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   long long tmp[8];
-  NVB_CUDA(cudaMemcpy(tmp, m->stats, sizeof(tmp), cudaMemcpyDeviceToHost));
+  NVB_CUDA(cudaMemcpy(tmp, m->stats.get(), sizeof(tmp), cudaMemcpyDeviceToHost));
   for (int i = 0; i < 8; i++) out[i] = tmp[i];
   return NVB_OK;
 }
@@ -3336,7 +3110,7 @@ int32_t nvb_mapper_esdf_time_split(NvbMapper* m, int64_t out[4]) {
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   long long tmp[5];
-  NVB_CUDA(cudaMemcpy(tmp, m->stats + 8, sizeof(tmp), cudaMemcpyDeviceToHost));
+  NVB_CUDA(cudaMemcpy(tmp, m->stats.get() + 8, sizeof(tmp), cudaMemcpyDeviceToHost));
   for (int i = 0; i < 4; i++) out[i] = tmp[i];
   out[0] = tmp[0];
   // [1]+[2] are CTA 0's own work; tmp[4] is the sum over phases of the slowest CTA's work: report it in [1]
@@ -3350,7 +3124,7 @@ int32_t nvb_mapper_esdf_clear_blocks_read(NvbMapper* m, int64_t* out) {
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   long long v = 0;
-  NVB_CUDA(cudaMemcpy(&v, m->stats + 13, sizeof(v), cudaMemcpyDeviceToHost));
+  NVB_CUDA(cudaMemcpy(&v, m->stats.get() + 13, sizeof(v), cudaMemcpyDeviceToHost));
   *out = v;
   return NVB_OK;
 }
@@ -3360,7 +3134,7 @@ int32_t nvb_mapper_esdf_split_stats(NvbMapper* m, int64_t out[2]) {
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   long long tmp[2];
-  NVB_CUDA(cudaMemcpy(tmp, m->stats + 14, sizeof(tmp), cudaMemcpyDeviceToHost));
+  NVB_CUDA(cudaMemcpy(tmp, m->stats.get() + 14, sizeof(tmp), cudaMemcpyDeviceToHost));
   out[0] = tmp[0], out[1] = tmp[1];
   return NVB_OK;
 }
@@ -3370,7 +3144,7 @@ int32_t nvb_mapper_debug_phase_max(NvbMapper* m, int64_t* out, int32_t cap) {
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   if (cap > 4000) cap = 4000;
-  NVB_CUDA(cudaMemcpy(out, m->phase_max, (size_t)cap * sizeof(long long), cudaMemcpyDeviceToHost));
+  NVB_CUDA(cudaMemcpy(out, m->phase_max.get(), (size_t)cap * sizeof(long long), cudaMemcpyDeviceToHost));
   return NVB_OK;
 }
 
@@ -3409,11 +3183,9 @@ int ensureMeshLayer(NvbMapper* m) {
   int rc;
   if (!m->mesh.blocks) {
     if ((rc = allocLayer(&m->mesh, m->tsdf.capacity, kMeshHeaderBytes, m->stream))) return rc;
-    NVB_CUDA(cudaMalloc(&m->mesh_state, kArenaInts * sizeof(int)));
-    NVB_CUDA(cudaMemsetAsync(m->mesh_state, 0, kArenaInts * sizeof(int), m->stream));
-    NVB_CUDA(cudaMalloc(&m->dirty_mesh, (size_t)m->tsdf.capacity * sizeof(int)));
-    NVB_CUDA(cudaMemsetAsync(m->dirty_mesh, 0, (size_t)m->tsdf.capacity * sizeof(int), m->stream));
-    NVB_CUDA(cudaMalloc(&m->todo_mesh_slots, (size_t)m->tsdf.capacity * sizeof(int)));
+    NVB_CUDA(m->mesh_state.grow(m, kArenaInts, kArenaInts, 0));
+    NVB_CUDA(m->dirty_mesh.grow(m, m->tsdf.capacity, m->tsdf.capacity, 0));
+    NVB_CUDA(m->todo_mesh_slots.grow(m, m->tsdf.capacity, m->tsdf.capacity));
   } else if (m->mesh.capacity < m->tsdf.capacity) {
     if ((rc = growLayer(m, &m->mesh, m->tsdf.capacity))) return rc;
   }
@@ -3423,10 +3195,10 @@ int ensureMeshLayer(NvbMapper* m) {
 MeshCtx makeMeshCtx(NvbMapper* m) {
   MeshCtx c{};
   c.tsdf = m->tsdf, c.color = m->color, c.mesh = m->mesh;
-  c.vertices = m->mesh_v, c.normals = m->mesh_n, c.triangles = m->mesh_t, c.colors_raw = m->mesh_c;
-  c.colors = reinterpret_cast<uchar4*>(m->mesh_c);
-  c.arena_state = m->mesh_state;
-  c.counts = m->mesh_counts, c.offsets = m->mesh_offsets;
+  c.vertices = m->mesh_v.get(), c.normals = m->mesh_n.get(), c.triangles = m->mesh_t.get(), c.colors_raw = m->mesh_c.get();
+  c.colors = reinterpret_cast<uchar4*>(m->mesh_c.get());
+  c.arena_state = m->mesh_state.get();
+  c.counts = m->mesh_counts.get(), c.offsets = m->mesh_offsets.get();
   c.block_size = m->block_size, c.voxel_size = m->voxel_size;
   c.min_weight = m->mp.min_weight, c.cutoff_distance_m = m->mp.cutoff_distance_vox * m->voxel_size;
   c.weld = m->mp.weld_vertices ? 1 : 0;
@@ -3441,43 +3213,36 @@ int repackMeshArena(NvbMapper* m, long long need) {
   int nslots = 0;
   NVB_CUDA(cudaMemcpy(&nslots, m->mesh.count, sizeof(int), cudaMemcpyDeviceToHost));
   nslots = std::min(nslots, m->mesh.capacity);
-  int* sizes = nullptr;
-  int* new_off = nullptr;
-  NVB_CUDA(cudaMalloc(&sizes, ((size_t)nslots + 1) * sizeof(int)));
-  NVB_CUDA(cudaMalloc(&new_off, ((size_t)nslots + 1) * sizeof(int)));
+  DeviceArray<int> sizes, new_off;
+  NVB_CUDA(sizes.grow(m, (size_t)nslots + 1, (size_t)nslots + 1));
+  NVB_CUDA(new_off.grow(m, (size_t)nslots + 1, (size_t)nslots + 1));
   MeshCtx c = makeMeshCtx(m);
-  launchMeshCompactSizes(c, nslots, sizes, m->stream);
+  launchMeshCompactSizes(c, nslots, sizes.get(), m->stream);
   std::vector<int> h((size_t)nslots + 1, 0), o((size_t)nslots + 1, 0);
-  NVB_CUDA(cudaMemcpyAsync(h.data(), sizes, (size_t)nslots * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(h.data(), sizes.get(), (size_t)nslots * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   long long live = 0;
   for (int i = 0; i < nslots; i++) o[i] = (int)live, live += h[i];
   // at least half of the arena is free behind the live data after a repack: with an update re-emitting ~1/5 of the live
   // vertices, that is several updates between repacks
-  long long cap = std::max<long long>(m->mesh_arena_cap, 1 << 20);
+  long long cap = std::max<long long>(m->mesh_t.size(), 1 << 20);
   while (cap < 2 * (live + need)) cap *= 2;
-  if (cap > 0x7fffffffll) {
-    cudaFree(sizes), cudaFree(new_off);
-    return fail(NVB_ERR_CAPACITY, "mesh arena beyond 2^31 vertices");
-  }
-  // the spare arena of the previous repack is reused when it has the right size (no cudaMalloc in the steady state)
-  if (m->mesh_alt_cap != cap) {
-    cudaFree(m->mesh_alt_v), cudaFree(m->mesh_alt_n), cudaFree(m->mesh_alt_t), cudaFree(m->mesh_alt_c);
-    m->mesh_alt_v = m->mesh_alt_n = nullptr, m->mesh_alt_t = nullptr, m->mesh_alt_c = nullptr, m->mesh_alt_cap = 0;
-    NVB_CUDA(cudaMalloc(&m->mesh_alt_v, (size_t)cap * 12));
-    NVB_CUDA(cudaMalloc(&m->mesh_alt_n, (size_t)cap * 12));
-    NVB_CUDA(cudaMalloc(&m->mesh_alt_t, (size_t)cap * 4));
-    NVB_CUDA(cudaMalloc(&m->mesh_alt_c, (size_t)cap * 4));
-    m->mesh_alt_cap = cap;
-  }
-  NVB_CUDA(cudaMemcpyAsync(new_off, o.data(), (size_t)nslots * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  if (m->mesh_v) launchMeshCompactMove(c, nslots, new_off, m->mesh_alt_v, m->mesh_alt_n, m->mesh_alt_t, m->mesh_alt_c, m->num_sms, m->stream);
+  if (cap > 0x7fffffffll) return fail(NVB_ERR_CAPACITY, "mesh arena beyond 2^31 vertices");
+  // The spare arena is the one the previous repack moved out of, never larger than `cap`: when it has the right size it
+  // is reused (no cudaMalloc in the steady state).
+  NVB_CUDA(m->mesh_alt_v.grow(m, 3 * cap, 3 * cap));
+  NVB_CUDA(m->mesh_alt_n.grow(m, 3 * cap, 3 * cap));
+  NVB_CUDA(m->mesh_alt_t.grow(m, cap, cap));
+  NVB_CUDA(m->mesh_alt_c.grow(m, 4 * cap, 4 * cap));
+  NVB_CUDA(cudaMemcpyAsync(new_off.get(), o.data(), (size_t)nslots * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  if (m->mesh_v.get())
+    launchMeshCompactMove(c, nslots, new_off.get(), m->mesh_alt_v.get(), m->mesh_alt_n.get(), m->mesh_alt_t.get(),
+                          m->mesh_alt_c.get(), m->num_sms, m->stream);
   const int state[kArenaInts] = {(int)live, 0, (int)live, 0};
-  NVB_CUDA(cudaMemcpyAsync(m->mesh_state, state, sizeof(state), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(m->mesh_state.get(), state, sizeof(state), cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  cudaFree(sizes), cudaFree(new_off);
   std::swap(m->mesh_v, m->mesh_alt_v), std::swap(m->mesh_n, m->mesh_alt_n), std::swap(m->mesh_t, m->mesh_alt_t);
-  std::swap(m->mesh_c, m->mesh_alt_c), std::swap(m->mesh_arena_cap, m->mesh_alt_cap);
+  std::swap(m->mesh_c, m->mesh_alt_c);
   m->launches += 2;
   return NVB_OK;
 }
@@ -3486,25 +3251,19 @@ int repackMeshArena(NvbMapper* m, long long need) {
 int meshUpdateImpl(NvbMapper* m, const int* xyz_dev, const int* slots_dev, const int* count_dev, int upper, bool color) {
   int rc;
   if (upper <= 0) return NVB_OK;
-  if (m->mesh_list_cap < upper) {
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(m->mesh_counts), cudaFree(m->mesh_offsets);
-    m->mesh_counts = m->mesh_offsets = nullptr;
-    const int cap = std::max(upper, 2 * m->mesh_list_cap);
-    NVB_CUDA(cudaMalloc(&m->mesh_counts, (size_t)cap * sizeof(int)));
-    NVB_CUDA(cudaMalloc(&m->mesh_offsets, (size_t)cap * sizeof(int)));
-    m->mesh_list_cap = cap;
-  }
+  const size_t list = upper;
+  NVB_CUDA(m->mesh_counts.grow(m, list, std::max(list, 2 * m->mesh_counts.size())));
+  NVB_CUDA(m->mesh_offsets.grow(m, list, std::max(list, 2 * m->mesh_offsets.size())));
   MeshCtx c = makeMeshCtx(m);
   c.in_xyz = xyz_dev, c.in_slots = slots_dev, c.in_count_dev = count_dev, c.in_count_host = upper;
-  c.tracker_dirty = slots_dev ? m->dirty_mesh : nullptr;
+  c.tracker_dirty = slots_dev ? m->dirty_mesh.get() : nullptr;
   launchMeshCount(c, upper, m->num_sms, m->stream);
   m->launches += 2;
   // the one number the host needs: does the update fit behind the arena's fill level?
   int state[kArenaInts];
-  NVB_CUDA(cudaMemcpyAsync(state, m->mesh_state, sizeof(state), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(state, m->mesh_state.get(), sizeof(state), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  if ((long long)state[kArenaLastBase] + state[kArenaLastTotal] > m->mesh_arena_cap) {
+  if ((long long)state[kArenaLastBase] + state[kArenaLastTotal] > (long long)m->mesh_t.size()) {
     if ((rc = repackMeshArena(m, state[kArenaLastTotal]))) return rc;
     c = makeMeshCtx(m);
     c.in_xyz = xyz_dev, c.in_slots = slots_dev, c.in_count_dev = count_dev, c.in_count_host = upper;
@@ -3533,15 +3292,9 @@ int uploadMeshList(NvbMapper* m, const int32_t* xyz_host, int n, int* out_unique
   std::sort(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x != b.x ? a.x < b.x : (a.y != b.y ? a.y < b.y : a.z < b.z); });
   v.erase(std::unique(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x == b.x && a.y == b.y && a.z == b.z; }), v.end());
   const int u = (int)v.size();
-  if (m->mesh_xyz_cap < u) {
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    cudaFree(m->mesh_xyz_dev);
-    m->mesh_xyz_dev = nullptr;
-    const int cap = std::max(u, 2 * m->mesh_xyz_cap);
-    NVB_CUDA(cudaMalloc(&m->mesh_xyz_dev, (size_t)cap * 3 * sizeof(int)));
-    m->mesh_xyz_cap = cap;
-  }
-  NVB_CUDA(cudaMemcpyAsync(m->mesh_xyz_dev, v.data(), (size_t)u * sizeof(K3), cudaMemcpyHostToDevice, m->stream));
+  const size_t ints = 3 * (size_t)u;
+  NVB_CUDA(m->mesh_xyz_dev.grow(m, ints, std::max(ints, 2 * m->mesh_xyz_dev.size())));
+  NVB_CUDA(cudaMemcpyAsync(m->mesh_xyz_dev.get(), v.data(), (size_t)u * sizeof(K3), cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));  // v dies with this scope
   *out_unique = u;
   return NVB_OK;
@@ -3578,13 +3331,13 @@ int32_t nvb_mapper_update_mesh(NvbMapper* m, int32_t update_full_layer) {
   pollCounts(m);
   const int upper = std::min(m->tsdf_count_ub, m->tsdf.capacity);
   if (!m->mesh_tracker_initialized || update_full_layer) {
-    launchTodoAll(m->tsdf, m->dirty_mesh, m->todo_mesh_slots, m->esdf_ints + kTodoMeshCount, m->stream);
+    launchTodoAll(m->tsdf, m->dirty_mesh.get(), m->todo_mesh_slots.get(), m->esdf_ints.get() + kTodoMeshCount, m->stream);
     m->launches++;
     m->mesh_tracker_initialized = true;
   }
   // integrateBlocksGPU + updateAppearance over the tracker's blocks, then markBlocksAsUpdated (mapper.cpp:385-395)
-  if ((rc = meshUpdateImpl(m, nullptr, m->todo_mesh_slots, m->esdf_ints + kTodoMeshCount, upper, true))) return rc;
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints + kTodoMeshCount, 0, sizeof(int), m->stream));
+  if ((rc = meshUpdateImpl(m, nullptr, m->todo_mesh_slots.get(), m->esdf_ints.get() + kTodoMeshCount, upper, true))) return rc;
+  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kTodoMeshCount, 0, sizeof(int), m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   return checkDeviceError(m);
 }
@@ -3599,7 +3352,7 @@ int32_t nvb_mesh_integrate_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, 
   if (num_blocks == 0) return NVB_OK;  // (:73-75)
   int u = 0;
   if ((rc = uploadMeshList(m, blocks_xyz_host, num_blocks, &u))) return rc;
-  if ((rc = meshUpdateImpl(m, m->mesh_xyz_dev, nullptr, nullptr, u, update_color != 0))) return rc;
+  if ((rc = meshUpdateImpl(m, m->mesh_xyz_dev.get(), nullptr, nullptr, u, update_color != 0))) return rc;
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   return checkDeviceError(m);
 }
@@ -3610,11 +3363,11 @@ int32_t nvb_mesh_update_color(NvbMapper* m, const int32_t* blocks_xyz_host, int3
   NVB_CUDA(cudaSetDevice(m->device));
   int rc;
   if ((rc = ensureMeshLayer(m))) return rc;
-  if (num_blocks == 0 || !m->mesh_v) return NVB_OK;
+  if (num_blocks == 0 || !m->mesh_v.get()) return NVB_OK;
   int u = 0;
   if ((rc = uploadMeshList(m, blocks_xyz_host, num_blocks, &u))) return rc;
   MeshCtx c = makeMeshCtx(m);
-  c.in_xyz = m->mesh_xyz_dev, c.in_count_host = u;
+  c.in_xyz = m->mesh_xyz_dev.get(), c.in_count_host = u;
   launchMeshColor(c, u, m->num_sms, m->stream);
   m->launches++;
   NVB_CUDA(cudaStreamSynchronize(m->stream));
@@ -3628,15 +3381,14 @@ int32_t nvb_mesh_block_sizes(NvbMapper* m, const int32_t* blocks_xyz_host, int32
   for (int i = 0; i < 3 * num_blocks; i++) sizes_out[i] = -1;
   if (!m->mesh.blocks) return NVB_OK;
   NVB_CUDA(syncAll(m));
-  int* dev = nullptr;
-  NVB_CUDA(cudaMalloc(&dev, (size_t)num_blocks * 7 * sizeof(int)));  // headers[4n] (int4-aligned) | xyz[3n]
-  int* xyz_dev = dev + 4 * (size_t)num_blocks;
+  DeviceArray<int> dev;  // headers[4n] (int4-aligned) | xyz[3n]
+  NVB_CUDA(dev.grow(m, (size_t)num_blocks * 7, (size_t)num_blocks * 7));
+  int* xyz_dev = dev.get() + 4 * (size_t)num_blocks;
   NVB_CUDA(cudaMemcpy(xyz_dev, blocks_xyz_host, (size_t)num_blocks * 3 * sizeof(int), cudaMemcpyHostToDevice));
-  launchMeshHeaders(makeMeshCtx(m), xyz_dev, num_blocks, dev, m->stream);
+  launchMeshHeaders(makeMeshCtx(m), xyz_dev, num_blocks, dev.get(), m->stream);
   std::vector<int> h((size_t)num_blocks * 4);
-  NVB_CUDA(cudaMemcpyAsync(h.data(), dev, h.size() * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(h.data(), dev.get(), h.size() * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  cudaFree(dev);
   for (int i = 0; i < num_blocks; i++)
     if (h[4 * i] >= 0) sizes_out[3 * i] = h[4 * i + 1], sizes_out[3 * i + 1] = h[4 * i + 2], sizes_out[3 * i + 2] = h[4 * i + 3];
   return NVB_OK;
@@ -3649,49 +3401,47 @@ int32_t nvb_mesh_get_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   const size_t n = (size_t)num_blocks;
-  int* dev = nullptr;  // headers[4n] (int4-aligned) | xyz[3n] | dst[3n]
-  NVB_CUDA(cudaMalloc(&dev, n * 10 * sizeof(int)));
-  NVB_CUDA(cudaMemcpy(dev + 4 * n, blocks_xyz_host, n * 3 * sizeof(int), cudaMemcpyHostToDevice));
+  DeviceArray<int> dev;  // headers[4n] (int4-aligned) | xyz[3n] | dst[3n]
+  NVB_CUDA(dev.grow(m, n * 10, n * 10));
+  NVB_CUDA(cudaMemcpy(dev.get() + 4 * n, blocks_xyz_host, n * 3 * sizeof(int), cudaMemcpyHostToDevice));
   MeshCtx c = makeMeshCtx(m);
-  launchMeshHeaders(c, dev + 4 * n, num_blocks, dev, m->stream);
+  launchMeshHeaders(c, dev.get() + 4 * n, num_blocks, dev.get(), m->stream);
   std::vector<int> h(n * 4), dst(n * 3);
-  NVB_CUDA(cudaMemcpyAsync(h.data(), dev, h.size() * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(h.data(), dev.get(), h.size() * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   long long tv = 0, tt = 0, tc = 0;
   for (size_t i = 0; i < n; i++) {
     dst[3 * i] = (int)tv, dst[3 * i + 1] = (int)tt, dst[3 * i + 2] = (int)tc;
     if (h[4 * i] >= 0) tv += h[4 * i + 1], tt += h[4 * i + 2], tc += h[4 * i + 3];
   }
-  if (tv > caps[0] || tt > caps[1] || tc > caps[2]) {
-    cudaFree(dev);
+  if (tv > caps[0] || tt > caps[1] || tc > caps[2])
     return fail(NVB_ERR_CAPACITY, "output buffers smaller than the listed mesh blocks");
-  }
-  float *pv = nullptr, *pn = nullptr;
-  int* pt = nullptr;
-  unsigned char* pc = nullptr;
-  NVB_CUDA(cudaMalloc(&pv, std::max<size_t>(1, (size_t)tv * 12)));
-  NVB_CUDA(cudaMalloc(&pn, std::max<size_t>(1, (size_t)tv * 12)));
-  NVB_CUDA(cudaMalloc(&pt, std::max<size_t>(1, (size_t)tt * 4)));
-  NVB_CUDA(cudaMalloc(&pc, std::max<size_t>(1, (size_t)tc * 4)));
-  NVB_CUDA(cudaMemcpyAsync(dev + 7 * n, dst.data(), n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  launchMeshPack(c, dev, dev + 7 * n, num_blocks, pv, pn, pt, pc, m->num_sms, m->stream);
-  if (vertices_out && tv) NVB_CUDA(cudaMemcpyAsync(vertices_out, pv, (size_t)tv * 12, cudaMemcpyDeviceToHost, m->stream));
-  if (normals_out && tv) NVB_CUDA(cudaMemcpyAsync(normals_out, pn, (size_t)tv * 12, cudaMemcpyDeviceToHost, m->stream));
-  if (triangles_out && tt) NVB_CUDA(cudaMemcpyAsync(triangles_out, pt, (size_t)tt * 4, cudaMemcpyDeviceToHost, m->stream));
-  if (colors_out && tc) NVB_CUDA(cudaMemcpyAsync(colors_out, pc, (size_t)tc * 4, cudaMemcpyDeviceToHost, m->stream));
+  // 3 floats per vertex and normal, one int per triangle index, 4 bytes per colour; at least one element each
+  DeviceArray<float> pv, pn;
+  DeviceArray<int> pt;
+  DeviceArray<unsigned char> pc;
+  NVB_CUDA(pv.grow(m, std::max<size_t>(1, (size_t)tv * 3), std::max<size_t>(1, (size_t)tv * 3)));
+  NVB_CUDA(pn.grow(m, std::max<size_t>(1, (size_t)tv * 3), std::max<size_t>(1, (size_t)tv * 3)));
+  NVB_CUDA(pt.grow(m, std::max<size_t>(1, (size_t)tt), std::max<size_t>(1, (size_t)tt)));
+  NVB_CUDA(pc.grow(m, std::max<size_t>(1, (size_t)tc * 4), std::max<size_t>(1, (size_t)tc * 4)));
+  NVB_CUDA(cudaMemcpyAsync(dev.get() + 7 * n, dst.data(), n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  launchMeshPack(c, dev.get(), dev.get() + 7 * n, num_blocks, pv.get(), pn.get(), pt.get(), pc.get(), m->num_sms, m->stream);
+  if (vertices_out && tv) NVB_CUDA(cudaMemcpyAsync(vertices_out, pv.get(), (size_t)tv * 12, cudaMemcpyDeviceToHost, m->stream));
+  if (normals_out && tv) NVB_CUDA(cudaMemcpyAsync(normals_out, pn.get(), (size_t)tv * 12, cudaMemcpyDeviceToHost, m->stream));
+  if (triangles_out && tt) NVB_CUDA(cudaMemcpyAsync(triangles_out, pt.get(), (size_t)tt * 4, cudaMemcpyDeviceToHost, m->stream));
+  if (colors_out && tc) NVB_CUDA(cudaMemcpyAsync(colors_out, pc.get(), (size_t)tc * 4, cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  cudaFree(dev), cudaFree(pv), cudaFree(pn), cudaFree(pt), cudaFree(pc);
   return NVB_OK;
 }
 
 int32_t nvb_mesh_arena_stats(NvbMapper* m, int64_t out[4]) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  out[0] = m->mesh_arena_cap, out[1] = out[2] = out[3] = 0;
+  out[0] = (int64_t)m->mesh_t.size(), out[1] = out[2] = out[3] = 0;
   if (!m->mesh.blocks) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   int state[kArenaInts];
-  NVB_CUDA(cudaMemcpy(state, m->mesh_state, sizeof(state), cudaMemcpyDeviceToHost));
+  NVB_CUDA(cudaMemcpy(state, m->mesh_state.get(), sizeof(state), cudaMemcpyDeviceToHost));
   out[1] = state[kArenaUsed], out[2] = state[kArenaLastTotal], out[3] = state[kArenaGarbage];
   return NVB_OK;
 }
@@ -3747,27 +3497,20 @@ int runLayerQuery(NvbMapper* m, const float* xyz, int32_t memory, long long n, v
                   uint8_t* flags, Launch launch) {
   NVB_CUDA(cudaSetDevice(m->device));
   if (memory == NVB_MEM_DEVICE) return runOrdered(&m, 1, m->stream, [&](cudaStream_t st) { launch(xyz, out, flags, st); });
-  float* xyz_dev = nullptr;
-  unsigned char *out_dev = nullptr, *flags_dev = nullptr;
-  auto release = [&]() { cudaFree(xyz_dev), cudaFree(out_dev), cudaFree(flags_dev); };
-  if (cudaMalloc(&xyz_dev, (size_t)n * 3 * sizeof(float)) != cudaSuccess ||
-      cudaMalloc(&out_dev, (size_t)n * out_bytes_per_point) != cudaSuccess || cudaMalloc(&flags_dev, (size_t)n) != cudaSuccess) {
-    release();
-    return fail(NVB_ERR_CUDA, "cudaMalloc of the query's staging buffers failed");
-  }
-  int rc = NVB_OK;
-  cudaError_t e = cudaMemcpyAsync(xyz_dev, xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, m->stream);
+  const size_t out_bytes = (size_t)n * out_bytes_per_point;
+  DeviceArray<float> xyz_dev;
+  DeviceArray<unsigned char> out_dev, flags_dev;
+  NVB_CUDA(xyz_dev.grow(m, (size_t)n * 3, (size_t)n * 3));
+  NVB_CUDA(out_dev.grow(m, out_bytes, out_bytes));
+  NVB_CUDA(flags_dev.grow(m, n, n));
+  NVB_CUDA(cudaMemcpyAsync(xyz_dev.get(), xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
   // the caller's buffer goes down too: the outputs the kernel does not write come back unchanged
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out_dev, out, (size_t)n * out_bytes_per_point, cudaMemcpyHostToDevice, m->stream);
-  if (e == cudaSuccess)
-    rc = runOrdered(&m, 1, m->stream, [&](cudaStream_t st) { launch(xyz_dev, out_dev, flags_dev, st); });
-  if (e == cudaSuccess && rc == NVB_OK)
-    e = cudaMemcpyAsync(out, out_dev, (size_t)n * out_bytes_per_point, cudaMemcpyDeviceToHost, m->stream);
-  if (e == cudaSuccess && rc == NVB_OK) e = cudaMemcpyAsync(flags, flags_dev, (size_t)n, cudaMemcpyDeviceToHost, m->stream);
-  if (e == cudaSuccess && rc == NVB_OK) e = cudaStreamSynchronize(m->stream);
-  release();
-  if (rc != NVB_OK) return rc;
-  if (e != cudaSuccess) return fail(NVB_ERR_CUDA, std::string("point query: ") + cudaGetErrorString(e));
+  NVB_CUDA(cudaMemcpyAsync(out_dev.get(), out, out_bytes, cudaMemcpyHostToDevice, m->stream));
+  const int rc = runOrdered(&m, 1, m->stream, [&](cudaStream_t st) { launch(xyz_dev.get(), out_dev.get(), flags_dev.get(), st); });
+  if (rc) return rc;
+  NVB_CUDA(cudaMemcpyAsync(out, out_dev.get(), out_bytes, cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(flags, flags_dev.get(), (size_t)n, cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
   return NVB_OK;
 }
 

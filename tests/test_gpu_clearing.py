@@ -322,6 +322,10 @@ def test_layer_clear_shapes_occupancy_and_color(gpu):
     touched = occ.m.occupancy_layer().clear_shapes(_gpu_shapes(shapes))
     assert np.array_equal(touched, _arr(cr.clear_shapes(occ.o, shapes, "occupancy"))) and len(touched) > 0
     _assert_occ_equal(occ.m.occupancy_layer().as_dict(), occ.o.occupancy_layer())
+    more = _shapes(40) + [cr.Sphere((0.0, 0.0, 1.0), 1.0)]  # a longer list on the same mapper: the shape buffer grows
+    touched = occ.m.occupancy_layer().clear_shapes(_gpu_shapes(more))
+    assert np.array_equal(touched, _arr(cr.clear_shapes(occ.o, more, "occupancy"))) and len(touched) > 0
+    _assert_occ_equal(occ.m.occupancy_layer().as_dict(), occ.o.occupancy_layer())
     occ.close()
     p = Pair("tsdf", False)
     for i, (d, T) in enumerate(frames):

@@ -71,6 +71,11 @@ def test_detection_primitive_scene_with_added_box(gpu):
         c = pts[:, 0] / pts[:, 2] * cam.fu + cam.cu
         r = pts[:, 1] / pts[:, 2] * cam.fv + cam.cv
         assert np.all((c >= c0 - 1e-3) & (c <= c0 + 80 + 1e-3) & (r >= r0 - 1e-3) & (r <= r0 + 60 + 1e-3))
+    # the same view at twice the resolution on the same mapper: the detector's per-pixel buffers grow
+    cs2, cam2, _ = cameras(640, 480)
+    d = syn.render_depth(syn.plane_scene(4.0), cs2, np.eye(4), max_dist=8.0)
+    d[160:280, 120:280] = 2.0
+    assert len(_detect_and_compare(m, d, T, cam2, _cam_dict(cam2))) > 0
     m.close()
 
 

@@ -464,6 +464,12 @@ def test_esdf_explicit_block_lists_and_params(gpu):
         m.esdf_integrator().integrate_blocks(lst)
         o.integrate_esdf(lst, ep)
         assert_esdf_equal(m.esdf_layer().as_dict(), o.esdf_layer())
+    # a list several times longer than any before, on the same mapper: the upload buffer grows
+    far = np.stack([500 + np.arange(4 * len(lst)), np.full(4 * len(lst), 500), np.full(4 * len(lst), 500)], axis=1)
+    lst = np.vstack([m.tsdf_layer().get_all_block_indices(), far]).astype(np.int32)
+    m.esdf_integrator().integrate_blocks(lst)
+    o.integrate_esdf(lst, ep)
+    assert_esdf_equal(m.esdf_layer().as_dict(), o.esdf_layer())
     m.close()
 
 
