@@ -129,11 +129,6 @@ struct NvbMapper {
   int tsdf_count_ub = 0;   // host-side upper bound of *tsdf.count
   int esdf_extra_ub = 0;   // blocks submitted to the ESDF through explicit lists
 
-  // ViewpointCache of the projective integrator's ViewCalculator (C/include/nvblox/integrators/view_calculator.h:196,211-244):
-  // up to two (pose, sensor) -> block-list entries, newest first. A list is kept as the view bitset it was compacted from (a
-  // few KB on the device): a hit skips the raycast and replays the compaction + allocation, which yields the same list in the
-  // same order and re-allocates blocks that were deallocated in between, like allocateBlocksWhereRequired does in the reference.
-  BlockTensorMap tsdf_tmap;  // TMA descriptor of the TSDF slab (nvb_tsdf.cu)
   DeviceArray<int4> union_list;  // nvb_blocks_union's own output list
   DeviceArray<int> union_list_count;
 
@@ -161,6 +156,10 @@ struct NvbMapper {
   int do_depth_preprocessing = 0;
   int depth_preprocessing_num_dilations = 4;
   DeviceArray<float> pre_depth;
+  // ViewpointCache of the projective integrator's ViewCalculator (C/include/nvblox/integrators/view_calculator.h:196,211-244):
+  // up to two (pose, sensor) -> block-list entries, newest first. A list is kept as the view bitset it was compacted from (a
+  // few KB on the device): a hit skips the raycast and replays the compaction + allocation, which yields the same list in the
+  // same order and re-allocates blocks that were deallocated in between, like allocateBlocksWhereRequired does in the reference.
   int vc_n = 0;
   float vc_T[2][16];
   NvbCamera vc_cam[2];
@@ -945,13 +944,8 @@ int enqueueFrame(NvbMapper* m, const float* depth, const unsigned char* mask, in
       launchOccupancyIntegrate(m->frame_blocks.get(), m->frame_count, m->tsdf.blocks, depth_dev, mask_dev, mask_mode, rows,
                                cols, T_C_L, *cam, p, o, m->num_sms, m->bits.get(), grid.num_words, m->stream);
     } else {
-      // the slab's tensor descriptor follows reallocations (growLayer) by being re-encoded when base or capacity changed
-      if (tsdfUseTma() && (m->tsdf_tmap.base != m->tsdf.blocks || m->tsdf_tmap.capacity != m->tsdf.capacity)) {
-        if (encodeBlockTensorMap(&m->tsdf_tmap, m->tsdf.blocks, m->tsdf.capacity, kTsdfBlockBytes))
-          return fail(NVB_ERR_CUDA, "cuTensorMapEncodeTiled failed for the TSDF slab");
-      }
       launchTsdfIntegrate(m->frame_blocks.get(), m->frame_count, m->tsdf.blocks, depth_dev, mask_dev, mask_mode, rows, cols,
-                          T_C_L, *cam, p, m->num_sms, m->bits.get(), grid.num_words, tsdfUseTma() ? &m->tsdf_tmap : nullptr, m->stream);
+                          T_C_L, *cam, p, m->num_sms, m->bits.get(), grid.num_words, m->stream);
     }
     endStage(m);
     m->launches++;
@@ -1207,9 +1201,6 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   m->projective_layer_type = opts->projective_layer_type;
   m->keep_last_view = opts->keep_last_view ? 1 : 0;
   m->esdf_persistent = opts->esdf_persistent;
-  // A/B switch for measurements: 0 host loop, 1 four-phase wavefront, 2 gather-emulate-sweep wavefront
-  if (const char* e = getenv("NVB_ESDF_MODE")) m->esdf_persistent = atoi(e);
-  if (const char* e = getenv("NVB_WAVEX_RESERVED_SMS")) m->esdf_reserved_sms = std::max(0, std::min(64, atoi(e)));
   m->esdf_split_min_k = esdfWaveXSplitMinK();
   if (const char* e = getenv("NVB_GES_SWITCH")) m->ges_switch = atoi(e);
   {
@@ -1221,12 +1212,10 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   NVB_CUDA(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
   {
     // The ESDF chain is the frame's critical path; the next frame's raycast / compaction / TSDF update only has to finish
-    // before the next mark kernel. NVB_ESDF_STREAM_PRIORITY=0 switches the preference off (A/B).
+    // before the next mark kernel, so the ESDF stream gets the highest priority.
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    const char* pe = getenv("NVB_ESDF_STREAM_PRIORITY");
-    const int prio = (pe && atoi(pe) == 0) ? lo : hi;
-    NVB_CUDA(cudaStreamCreateWithPriority(&m->esdf_stream, cudaStreamNonBlocking, prio));
+    NVB_CUDA(cudaStreamCreateWithPriority(&m->esdf_stream, cudaStreamNonBlocking, hi));
   }
   NVB_CUDA(cudaEventCreateWithFlags(&m->esdf_ready, cudaEventDisableTiming));
   NVB_CUDA(cudaEventCreateWithFlags(&m->esdf_done, cudaEventDisableTiming));
@@ -2396,11 +2385,8 @@ int ransacFit(NvbMapper* m, const float4* pts, int n, int iterations, float thre
   NVB_CUDA(m->gp_costs.grow(m, it, std::max(it, 2 * m->gp_costs.size())));
   NVB_CUDA(m->gp_planes.grow(m, it, std::max(it, 2 * m->gp_planes.size())));
   NVB_CUDA(m->gp_result.grow(m, 5, 5));
-  // A/B switch for measurements: the reference's launch shape (256-thread CTAs, points read from global memory)
-  const char* e = getenv("NVB_RANSAC_REFERENCE_SHAPE");
-  const bool reference_shape = e && atoi(e) == 1;
   launchRansacFit(pts, n, iterations, threshold, m->gp_states.get(), m->gp_costs.get(), m->gp_planes.get(), m->gp_result.get(),
-                  reference_shape, m->stream);
+                  m->stream);
   m->launches += 2;
   float out[5];
   NVB_CUDA(cudaMemcpyAsync(out, m->gp_result.get(), sizeof(out), cudaMemcpyDeviceToHost, m->stream));

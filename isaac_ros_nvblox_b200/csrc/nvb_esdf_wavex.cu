@@ -61,9 +61,6 @@ namespace {
 #define NVB_WAVEX_PROF 0  // 1: per-phase times and per-stage cycle counters of CTA 0 / group 0 (nvb_mapper_debug_phase_max,
                           // tools/wavex_profile.py); the timers spill at 96 registers, so quote its shares, not its times
 #endif
-#ifndef NVB_WAVEX_SPEC_HALO
-#define NVB_WAVEX_SPEC_HALO 0  // 1: the face halo of every allocated neighbour travels with the own block and the stamps (slower, DESIGN §9)
-#endif
 #if NVB_WAVEX_PROF
 #define X_PROF_BEGIN() long long tq = clock64();
 #define X_PROF(i) \
@@ -403,15 +400,10 @@ __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer
 
 // ---- halo voxels, as cp.async copies straight into the two region planes -- the 16-byte cell and the flag word of a voxel
 // from its block's exchange-slab slot: no registers are held across the wait (the register version held up to 20 words per
-// lane and spilled at 96 registers). By default only the batches of the members in
-// a live pair are fetched, after the stamps. With NVB_WAVEX_SPEC_HALO the face halo of every ALLOCATED face neighbour is issued
-// before the member stamps are known, with the own block and the stamps (one round trip after the record instead of two);
-// on the H100 the extra, mostly cold face fetches cost more than the round trip they save (DESIGN §9). Speculation is safe:
-// the replay reads a halo voxel only if its block is a live source (live[p] is a subset of the members) or a member destination (liveMasks), and the sweeps and the stores
-// touch the inner 8x8x8 only, so the voxels copied from a non-member's stale exchange-slab entry land in shared memory and are
-// never read. (The cells travel .cg, through L2 only. The flag words and the own block's words (ownAsync) are 4-byte copies,
-// which have no .cg form, so they go .ca. The L1 lines those leave behind cannot go stale unnoticed: every grid barrier ends
-// with an acquire (or a __threadfence), which invalidates the SM's L1, and within the single-CTA tail the writer is this SM.)
+// lane and spilled at 96 registers). Only the batches of the members in a live pair are fetched, after the stamps. The cells
+// travel .cg, through L2 only. The flag words and the own block's words (ownAsync) are 4-byte copies, which have no .cg form,
+// so they go .ca. The L1 lines those leave behind cannot go stale unnoticed: every grid barrier ends with an acquire
+// (gridBarrierRA), which invalidates the SM's L1, and within the single-CTA tail the writer is this SM.
 __device__ __forceinline__ void cpAsync4(unsigned int* smem_dst, const unsigned int* gsrc) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned int)__cvta_generic_to_shared(smem_dst)), "l"(gsrc)
                : "memory");
@@ -677,10 +669,9 @@ __device__ __noinline__ void processCandidate(int ring, int K) {
   const int* row = &xs.rec[group][1];
   const unsigned char* blk = c.blocks + (size_t)slot * kEsdfBlockBytes;
   // membership of the 27 blocks in this ring (sources of the passes); the loads travel with the loads of the own block (when
-  // not split) and (NVB_WAVEX_SPEC_HALO) the face halo
+  // not split)
   int sv = ring - 1;
   if (lane64 < 27 && row[lane64] >= 0) sv = __ldcg(c.stamp[ci] + row[lane64]);
-  if (NVB_WAVEX_SPEC_HALO) haloAsync(tab, R, row, c.X[ci], lane64, 0x3Fu, 0x7FFFFFFu);
   if (split) {
     const unsigned int m = __ballot_sync(0xffffffffu, lane64 < 27 && sv == ring);
     if (lane64 == 0) xs.mask[group] = m, xs.changed[group] = 0;
@@ -690,19 +681,16 @@ __device__ __noinline__ void processCandidate(int ring, int K) {
     if (lane64 == 0) xs.mask[group] = m, xs.changed[group] = 0;
     ownToShared(R, own, lane64);
   }
-  if (NVB_WAVEX_SPEC_HALO) cpAsyncWaitAll();
   groupSync(group);
   const LiveMasks L = liveMasks(xs.mask[group], xs.live[group], lane64 == 0);
   X_PROF_BIN(1, 9, K)
-  // the halo of the members that take part in a live pair (with NVB_WAVEX_SPEC_HALO: only their edge and corner batches),
-  // and when split, B's boundary planes along the live passes' axes
-  const unsigned int rest = NVB_WAVEX_SPEC_HALO ? (L.needed & ~kFaceBlocks) : L.needed;
+  // the halo of the members that take part in a live pair, and when split, B's boundary planes along the live passes' axes
   if (split) {
     ownAsync(R, blk, lane64, L.axes, true);
     if (lane64 == 0) atomicAdd(&xs.n_split, 1);
   }
-  if (rest) haloAsync(tab, R, row, c.X[ci], lane64, haloBatches(rest), rest);  // group-uniform
-  if (rest || split) cpAsyncWaitAll();
+  if (L.needed) haloAsync(tab, R, row, c.X[ci], lane64, haloBatches(L.needed), L.needed);  // group-uniform
+  if (L.needed || split) cpAsyncWaitAll();
   groupSync(group);  // (also publishes xs.live[group], written by lane 0 in liveMasks and read by every lane in replayX)
   X_PROF_KBIN(2, 15, K)
   const bool ch = replayX(tab, R, L, lane64, group, c.max_sq);
@@ -767,9 +755,6 @@ __device__ __noinline__ void processSeed(int ring, int slot) {
   groupSync(group);
 }
 
-#ifndef NVB_WAVEX_BARRIER_RA
-#define NVB_WAVEX_BARRIER_RA 1  // 0: gridBarrier (two __threadfence = fence.sc around a relaxed atomic and a volatile poll)
-#endif
 // Grid barrier with a release arrival and acquire polling: the same ordering as gridBarrier's two __threadfences (the CTA's
 // writes, gathered by the __syncthreads, are released by thread 0's arrival; its acquire load of the final count makes every
 // CTA's writes visible, and invalidates the SM's L1), without the heavier sequentially-consistent fences.
@@ -801,10 +786,7 @@ __device__ __forceinline__ void counterBarrierScan(XShared& xs, unsigned int* ba
     __stcg(counts + cta, make_int2(min(xs.ncand, seg), xs.nchanged));  // (registrations past the segment were dropped)
     xs.ncand = 0, xs.nchanged = 0;
   }
-  if (NVB_WAVEX_BARRIER_RA)
-    gridBarrierRA(bar, generation, nctas);
-  else
-    gridBarrier(bar, generation, nctas);
+  gridBarrierRA(bar, generation, nctas);
   int2 v = make_int2(0, 0);
   if (tid < nctas) v = __ldcg(counts + tid);
   const int lane = tid & 31, warp = tid >> 5;
@@ -1019,7 +1001,7 @@ cudaError_t launchEsdfComputeX(const EsdfCtx& c, int num_sms, int reserved_sms, 
   (*launches)++;
   // `reserved_sms` SMs are left to the other resident kernels: the raycast / compaction / TSDF kernels of the next frame then
   // run there instead of stealing issue slots from ring-critical CTAs (80-frame C2 bench on one H100 SXM at a 400 W power
-  // limit, NVB_WAVEX_RESERVED_SMS = 0 / 2 / 4 / 8, two runs each: 2367, 2339 / 2404, 2407 / 2399, 2378 / 2379, 2336 frames/s),
+  // limit, nvb_mapper_set_esdf_reserved_sms = 0 / 2 / 4 / 8, two runs each: 2367, 2339 / 2404, 2407 / 2399, 2378 / 2379, 2336 frames/s),
   // and a multi-GPU rank's NCCL all-gather can start -- and wait for its peers -- while a wavefront is in flight (a
   // cooperative grid that fills every SM serialises the two).
   const int grid = esdfWaveXGrid(num_sms, reserved_sms);

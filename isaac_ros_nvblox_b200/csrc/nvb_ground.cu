@@ -255,24 +255,6 @@ __global__ void __launch_bounds__(kFitThreads) ransacFitKernel(const float4* pts
   }
 }
 
-// The reference's launch shape, for measurements only (NVB_RANSAC_REFERENCE_SHAPE=1): 256-thread CTAs, every thread reads
-// every point from global memory. Same arithmetic, same results.
-__global__ void __launch_bounds__(256) ransacFitGlobalKernel(const float4* pts, int n, int iterations, float thr,
-                                                             const curandState* states, float* costs, float4* planes) {
-  const int it = blockIdx.x * blockDim.x + threadIdx.x;
-  float4 pl;
-  if (it >= iterations) return;
-  if (!samplePlane(pts, n, it, iterations, states, &pl)) {
-    costs[it] = FLT_MAX;
-    return;
-  }
-  const float thr2 = thr * thr;
-  float cost = 0.0f;
-  for (int j = 0; j < n; j++) cost += msacTerm(pl, pts[j], thr, thr2);
-  costs[it] = cost;
-  planes[it] = pl;
-}
-
 // std::min_element over the costs (lowest cost, lowest index on ties: the costs are never NaN, every summand being
 // d^2 < t^2 or t^2) -> {nx, ny, nz, d, found}.
 __global__ void __launch_bounds__(kArgminThreads) ransacArgminKernel(const float* costs, const float4* planes, int iterations,
@@ -344,13 +326,10 @@ void launchRansacInit(void* states, int first, int n, cudaStream_t stream) {
 }
 
 void launchRansacFit(const float4* pts, int n, int iterations, float threshold, const void* states, float* costs,
-                     float4* planes, float* out5, bool reference_shape, cudaStream_t stream) {
+                     float4* planes, float* out5, cudaStream_t stream) {
   const curandState* st = static_cast<const curandState*>(states);
-  if (reference_shape)
-    ransacFitGlobalKernel<<<iterations / 256 + 1, 256, 0, stream>>>(pts, n, iterations, threshold, st, costs, planes);
-  else
-    ransacFitKernel<<<(iterations + kFitThreads - 1) / kFitThreads, kFitThreads, 0, stream>>>(pts, n, iterations, threshold, st,
-                                                                                                costs, planes);
+  ransacFitKernel<<<(iterations + kFitThreads - 1) / kFitThreads, kFitThreads, 0, stream>>>(pts, n, iterations, threshold, st,
+                                                                                              costs, planes);
   ransacArgminKernel<<<1, kArgminThreads, 0, stream>>>(costs, planes, iterations, out5);
 }
 

@@ -346,23 +346,10 @@ void launchUnpackList(const int4* in, const int* count, int* out, int cap, cudaS
 void launchCompactAllocate(const CompactArgs& args, cudaStream_t stream);
 
 // nvb_tsdf.cu
-// A CUtensorMap (128 bytes, 64-byte aligned) that describes a layer slab to the TMA unit, and what it was encoded for.
-struct alignas(64) TensorMapBytes {
-  unsigned long long opaque[16];
-};
-struct BlockTensorMap {
-  TensorMapBytes desc;
-  const void* base = nullptr;
-  int capacity = 0;
-};
-bool tsdfUseTma();
-// 0 on success; the slab must be viewed as [capacity * block_bytes / 1024][256] 32-bit words
-int encodeBlockTensorMap(BlockTensorMap* out, void* base, int capacity, int block_bytes);
-// tmap == nullptr: the register-prefetch kernel
 void launchTsdfIntegrate(const int4* frame_blocks, const int* frame_count, unsigned char* tsdf_blocks,
                          const float* depth, const unsigned char* mask, int mask_mode, int rows, int cols,
                          const Rigid& T_C_L, const NvbCamera& cam, const TsdfKernelParams& p, int num_sms,
-                         unsigned int* bits_to_clear, int num_words, const BlockTensorMap* tmap, cudaStream_t stream);
+                         unsigned int* bits_to_clear, int num_words, cudaStream_t stream);
 
 void launchOccupancyIntegrate(const int4* frame_blocks, const int* frame_count, unsigned char* occ_blocks,
                               const float* depth, const unsigned char* mask, int mask_mode, int rows, int cols,
@@ -688,7 +675,7 @@ size_t ransacStateBytes();  // one XORWOW state
 void launchRansacInit(void* states, int first, int n, cudaStream_t stream);
 // MSAC over n >= 1 points (float4, w unused) -> out5 = {nx, ny, nz, d, found (int)}
 void launchRansacFit(const float4* pts, int n, int iterations, float threshold, const void* states, float* costs,
-                     float4* planes, float* out5, bool reference_shape, cudaStream_t stream);
+                     float4* planes, float* out5, cudaStream_t stream);
 
 // nvb_dynamics.cu: DynamicsDetection::computeDynamics and MaskPreprocessor::removeSmallConnectedComponents
 struct DynamicsArgs {

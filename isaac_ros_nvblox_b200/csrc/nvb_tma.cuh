@@ -75,25 +75,5 @@ __device__ __forceinline__ void bulkWait() {
 // Generic-proxy writes to shared memory -> visible to the async proxy (before a bulk store reads them).
 __device__ __forceinline__ void fenceProxyAsyncShared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-
-// ---- 2-D tiled tensor copies (cp.async.bulk.tensor.2d, SASS UTMALDG / UTMASTG) through a CUtensorMap descriptor.
-// `tmap` is the address of a descriptor that lives in kernel-parameter (__grid_constant__) or global memory; c0 is the
-// coordinate along the contiguous dimension, c1 the row. The shared-memory tile must be 128-byte aligned.
-__device__ __forceinline__ void tensorLoad2d(void* smem_dst, const void* tmap, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-          smemAddr(smem_dst)),
-      "l"(tmap), "r"(c0), "r"(c1), "r"(smemAddr(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tensorStore2d(const void* tmap, int c0, int c1, const void* smem_src) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%1, %2}], [%3];" ::"l"(tmap), "r"(c0), "r"(c1),
-               "r"(smemAddr(smem_src))
-               : "memory");
-}
-__device__ __forceinline__ void prefetchTensorMap(const void* tmap) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
-}
-
 }  // namespace tma
 }  // namespace nvb

@@ -15,11 +15,6 @@
 // kernel arguments (the reference dereferences a device pointer to a functor it
 // re-uploads every frame). Unchanged words are not written back.
 #include "nvb_internal.cuh"
-#include "nvb_tma.cuh"
-
-#include <cuda.h>  // CUtensorMap + enums only; no driver symbol is linked
-
-#include <cstdlib>
 
 namespace nvb {
 
@@ -221,116 +216,6 @@ __global__ void __launch_bounds__(256) tsdfIntegrateKernel(const __grid_constant
     }
     if (inext >= n) break;
     i = inext, blk = nblk, word = nword;
-  }
-}
-
-// The same update with the VoxelBlocks staged through shared memory by the TMA unit. The TSDF slab is described to the
-// hardware as a 2-D fp32 tensor [4 * capacity rows][256 columns] (row pitch 1 KiB), so VoxelBlock `slot` is the 256 x 4 box
-// at row 4 * slot: one cp.async.bulk.tensor.2d (UTMALDG) brings it in, one (UTMASTG) writes it back.
-//
-// Warp-specialised: warp 8 is the copy warp (one lane issues every load and store of the CTA), warps 0-7 fuse. A CTA walks
-// its blocks (cta, cta + grid, ...) through a ring of kTmaStages 4 KiB tiles; per stage `full` (the tile has landed) and
-// `done` (the eight fusing warps are finished with it). The fusing warps never wait for each other: each owns 1/8 of every
-// tile, and has the projection + depth look-up of block k+1 in flight while it fuses block k (they do not depend on the
-// voxel data). Blocks nothing changed in are not stored.
-constexpr int kTmaStages = 6;
-constexpr int kTmaFuseWarps = 8;
-constexpr int kTmaThreads = 32 * (kTmaFuseWarps + 1);
-
-struct VoxelSample {
-  float d, z;
-  bool ok, active;
-};
-
-template <bool kDistort>
-__global__ void __launch_bounds__(kTmaThreads) tsdfIntegrateTmaKernel(const __grid_constant__ TsdfArgs a,
-                                                                      const __grid_constant__ TensorMapBytes tmap) {
-  __shared__ __align__(128) float4 tile[kTmaStages][256];
-  __shared__ __align__(8) uint64_t full[kTmaStages];
-  __shared__ __align__(8) uint64_t done[kTmaStages];
-  __shared__ int changed_in[kTmaStages];
-  const int n = *a.frame_count;
-  const int tid = threadIdx.x;
-  for (int w = blockIdx.x * blockDim.x + tid; w < a.num_words; w += gridDim.x * blockDim.x) a.bits_to_clear[w] = 0;
-  if ((int)blockIdx.x >= n) return;
-  const int nk = (n - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // blocks of this CTA
-  if (tid == 0) {
-    for (int s = 0; s < kTmaStages; s++) {
-      tma::mbarInit(&full[s], 1);
-      tma::mbarInit(&done[s], kTmaFuseWarps);
-      changed_in[s] = 0;
-    }
-    tma::fenceBarrierInit();
-  }
-  __syncthreads();
-  if (tid >= 32 * kTmaFuseWarps) {
-    // ---- copy warp
-    if (tid != 32 * kTmaFuseWarps) return;
-    tma::prefetchTensorMap(&tmap);
-    // stage k % kTmaStages <- block k of this CTA (an unallocated block completes its phase without bytes)
-    auto produce = [&](int k) {
-      const int slot = a.frame_blocks[blockIdx.x + k * gridDim.x].w;
-      uint64_t* bar = &full[k % kTmaStages];
-      if (slot >= 0) {
-        tma::mbarArriveExpectTx(bar, kTsdfBlockBytes);
-        tma::tensorLoad2d(tile[k % kTmaStages], &tmap, 0, 4 * slot, bar);
-      } else {
-        tma::mbarArrive(bar);
-      }
-    };
-    for (int k = 0; k < nk && k < kTmaStages; k++) produce(k);
-    for (int k = 0; k < nk; k++) {
-      const int s = k % kTmaStages;
-      tma::mbarWait(&done[s], (unsigned int)(k / kTmaStages) & 1u);
-      if (changed_in[s]) {
-        changed_in[s] = 0;
-        tma::tensorStore2d(&tmap, 0, 4 * a.frame_blocks[blockIdx.x + k * gridDim.x].w, tile[s]);
-      }
-      tma::bulkCommit();  // one (possibly empty) group per block keeps the group count in step with k
-      // refill the stage of block k-1 once its store has finished reading the tile
-      if (k >= 1 && k - 1 + kTmaStages < nk) {
-        tma::bulkWaitRead<1>();
-        produce(k - 1 + kTmaStages);
-      }
-    }
-    tma::bulkWait<0>();  // the tiles must outlive the stores that read them
-    return;
-  }
-  // ---- fusing warps. Voxel pair owned by this thread: linear voxel offset 2*tid = x*64 + y*8 + z
-  const int vx = tid >> 5, vy = (tid >> 2) & 7, vz = (tid & 3) * 2;
-  const int lane = tid & 31;
-  auto sample = [&](int k, VoxelSample& s0, VoxelSample& s1) {
-    s0.ok = s1.ok = false, s0.active = s1.active = false, s0.d = s1.d = 0.f, s0.z = s1.z = 0.f;
-    if (k >= nk) return;
-    const int4 blk = a.frame_blocks[blockIdx.x + k * gridDim.x];
-    if (blk.w < 0) return;
-    s0.ok = sampleVoxel<kDistort>(a, blk, vx, vy, vz, s0.d, s0.z, s0.active);
-    s1.ok = sampleVoxel<kDistort>(a, blk, vx, vy, vz + 1, s1.d, s1.z, s1.active);
-  };
-  VoxelSample c0, c1, n0, n1;
-  sample(0, c0, c1);
-  for (int k = 0; k < nk; k++) {
-    const int s = k % kTmaStages;
-    sample(k + 1, n0, n1);
-    tma::mbarWait(&full[s], (unsigned int)(k / kTmaStages) & 1u);
-    bool changed = false;
-    if (c0.ok || c1.ok) {
-      float4 word = tile[s][tid];
-      const bool ch0 = c0.ok && fuseVoxel(a, c0.d, c0.z, c0.active, word.x, word.y);
-      const bool ch1 = c1.ok && fuseVoxel(a, c1.d, c1.z, c1.active, word.z, word.w);
-      changed = ch0 || ch1;
-      if (changed) {
-        tile[s][tid] = word;
-        tma::fenceProxyAsyncShared();  // this thread's tile writes -> visible to the TMA store
-      }
-    }
-    const bool any = __any_sync(0xffffffffu, changed);
-    __syncwarp();
-    if (lane == 0) {
-      if (any) atomicOr(&changed_in[s], 1);
-      tma::mbarArrive(&done[s]);  // release: the warp's writes (ordered by __syncwarp) precede the arrival
-    }
-    c0 = n0, c1 = n1;
   }
 }
 
@@ -568,70 +453,28 @@ __global__ void __launch_bounds__(512) freespaceUpdateKernel(const __grid_consta
   }
 }
 
-// Resident CTAs per SM of the projective update kernels. 8 x 256 threads fill an SM's thread slots, which keeps the
-// cooperative ESDF wavefront of the previous frame (side stream, one 256-thread CTA per SM) from starting until
-// this kernel drains; NVB_TSDF_CTAS_PER_SM is the A/B switch for that trade-off.
-static int projectiveCtasPerSm() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("NVB_TSDF_CTAS_PER_SM");
-    v = e ? atoi(e) : 8;
-    if (v < 1 || v > 8) v = 8;
-  }
-  return v;
-}
+// Resident CTAs per SM of the projective update kernels: 8 x 256 threads fill an SM's thread slots (one full wave). That
+// keeps the cooperative ESDF wavefront of the previous frame (side stream, one 256-thread CTA per SM) from starting until
+// this kernel drains.
+constexpr int kProjectiveCtasPerSm = 8;
 
-// NVB_TSDF_TMA=1 selects the TMA-staged kernel (A/B switch; both kernels are parity-tested); NVB_TSDF_TMA_CTAS_PER_SM its
-// grid. The default stays the register-prefetch kernel: at 5 cm the update is bound by instruction issue, not by memory
-// (mostly the IEEE divisions and the range checks the bit-exact projection needs), so what pays is resident warps: on the
-// 80-frame C2 bench (one H100 SXM, 400 W power limit) the update takes 20.8 us per frame with registers, 25.1 us with the
-// TMA ring at 4 CTAs per SM.
-bool tsdfUseTma() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("NVB_TSDF_TMA");
-    v = (e && atoi(e) != 0) ? 1 : 0;
-  }
-  return v != 0;
-}
-static int tsdfTmaCtasPerSm() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("NVB_TSDF_TMA_CTAS_PER_SM");
-    v = e ? atoi(e) : 4;
-    if (v < 1 || v > 8) v = 4;
-  }
-  return v;
-}
-
-// Descriptor of a layer slab as a 2-D tensor of 32-bit words: [rows_per_block * capacity][256], box = one block.
-// cuTensorMapEncodeTiled is a driver entry point; it is resolved through the runtime so the library does not link libcuda.
-int encodeBlockTensorMap(BlockTensorMap* out, void* base, int capacity, int block_bytes) {
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = nullptr;
-  if (!encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || !fn ||
-        q != cudaDriverEntryPointSuccess)
-      return 1;
-    encode = reinterpret_cast<EncodeFn>(fn);
-  }
-  static_assert(sizeof(CUtensorMap) == sizeof(TensorMapBytes), "descriptor size");
-  const int rows_per_block = block_bytes / 1024;
-  if (rows_per_block * 1024 != block_bytes || capacity <= 0) return 2;
-  const cuuint64_t dims[2] = {256, (cuuint64_t)capacity * rows_per_block};
-  const cuuint64_t strides[1] = {1024};
-  const cuuint32_t box[2] = {256, (cuuint32_t)rows_per_block};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = encode(reinterpret_cast<CUtensorMap*>(&out->desc), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims, strides,
-                            box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return 3;
-  out->base = base, out->capacity = capacity;
-  return 0;
+static TsdfArgs projectiveArgs(const int4* frame_blocks, const int* frame_count, unsigned char* blocks, const float* depth,
+                               const unsigned char* mask, int mask_mode, int rows, int cols, const Rigid& T_C_L,
+                               const NvbCamera& cam, const TsdfKernelParams& p, unsigned int* bits_to_clear, int num_words) {
+  TsdfArgs a;
+  a.frame_blocks = frame_blocks;
+  a.frame_count = frame_count;
+  a.tsdf_blocks = blocks;
+  a.depth = depth;
+  a.mask = mask;
+  a.mask_mode = mask_mode;
+  a.rows = rows, a.cols = cols;
+  a.T_C_L = T_C_L;
+  a.cam = cam;
+  a.p = p;
+  a.bits_to_clear = bits_to_clear;
+  a.num_words = num_words;
+  return a;
 }
 
 void launchMarkFreeSphere(const MarkFreeArgs& a, int num_sms, cudaStream_t stream) {
@@ -641,29 +484,11 @@ void launchMarkFreeSphere(const MarkFreeArgs& a, int num_sms, cudaStream_t strea
 void launchTsdfIntegrate(const int4* frame_blocks, const int* frame_count, unsigned char* tsdf_blocks,
                          const float* depth, const unsigned char* mask, int mask_mode, int rows, int cols,
                          const Rigid& T_C_L, const NvbCamera& cam, const TsdfKernelParams& p, int num_sms,
-                         unsigned int* bits_to_clear, int num_words, const BlockTensorMap* tmap, cudaStream_t stream) {
-  TsdfArgs a;
-  a.frame_blocks = frame_blocks;
-  a.frame_count = frame_count;
-  a.tsdf_blocks = tsdf_blocks;
-  a.depth = depth;
-  a.mask = mask;
-  a.mask_mode = mask_mode;
-  a.rows = rows, a.cols = cols;
-  a.T_C_L = T_C_L;
-  a.cam = cam;
-  a.p = p;
-  a.bits_to_clear = bits_to_clear;
-  a.num_words = num_words;
+                         unsigned int* bits_to_clear, int num_words, cudaStream_t stream) {
+  const TsdfArgs a = projectiveArgs(frame_blocks, frame_count, tsdf_blocks, depth, mask, mask_mode, rows, cols, T_C_L, cam, p,
+                                    bits_to_clear, num_words);
   // the lens-distortion variant is a separate instantiation so the pinhole path keeps its register budget
-  if (tmap && tsdfUseTma()) {
-    const int grid = num_sms * tsdfTmaCtasPerSm();
-    if (cam.has_distortion) tsdfIntegrateTmaKernel<true><<<grid, kTmaThreads, 0, stream>>>(a, tmap->desc);
-    else tsdfIntegrateTmaKernel<false><<<grid, kTmaThreads, 0, stream>>>(a, tmap->desc);
-    return;
-  }
-  // 8 resident 256-thread CTAs per SM (2048 threads): one full wave.
-  const int grid = num_sms * projectiveCtasPerSm();
+  const int grid = num_sms * kProjectiveCtasPerSm;
   if (cam.has_distortion) tsdfIntegrateKernel<true><<<grid, 256, 0, stream>>>(a);
   else tsdfIntegrateKernel<false><<<grid, 256, 0, stream>>>(a);
 }
@@ -673,20 +498,9 @@ void launchOccupancyIntegrate(const int4* frame_blocks, const int* frame_count, 
                               const Rigid& T_C_L, const NvbCamera& cam, const TsdfKernelParams& p,
                               const OccKernelParams& op, int num_sms, unsigned int* bits_to_clear, int num_words,
                               cudaStream_t stream) {
-  TsdfArgs a;
-  a.frame_blocks = frame_blocks;
-  a.frame_count = frame_count;
-  a.tsdf_blocks = occ_blocks;
-  a.depth = depth;
-  a.mask = mask;
-  a.mask_mode = mask_mode;
-  a.rows = rows, a.cols = cols;
-  a.T_C_L = T_C_L;
-  a.cam = cam;
-  a.p = p;
-  a.bits_to_clear = bits_to_clear;
-  a.num_words = num_words;
-  const int grid = num_sms * projectiveCtasPerSm();
+  const TsdfArgs a = projectiveArgs(frame_blocks, frame_count, occ_blocks, depth, mask, mask_mode, rows, cols, T_C_L, cam, p,
+                                    bits_to_clear, num_words);
+  const int grid = num_sms * kProjectiveCtasPerSm;
   if (cam.has_distortion) occupancyIntegrateKernel<true><<<grid, 256, 0, stream>>>(a, op);
   else occupancyIntegrateKernel<false><<<grid, 256, 0, stream>>>(a, op);
 }

@@ -5,9 +5,8 @@
   300k  : the same at about 300 k candidates
 
 For each map: the host time of the synchronous compute_ground_plane call (median over repeats, read-backs included), the
-host time of the fit alone (ransac_fit_plane on the candidates, 1 000 iterations) in this library's launch shape and in the
-reference's (256-thread CTAs, every thread reading the points from global memory; NVB_RANSAC_REFERENCE_SHAPE=1), and the
-device time per kernel from torch.profiler. Prints one JSON object with the card's name and power limit.
+host time of the fit alone (ransac_fit_plane on the candidates, 1 000 iterations), and the device time per kernel from
+torch.profiler. Prints one JSON object with the card's name and power limit.
 
     python tools/ground_plane_profile.py [--repeats 20]
 """
@@ -91,12 +90,9 @@ def profile_map(nvb, m, repeats):
     out = {"tsdf_blocks": m.tsdf_layer().num_blocks(), "crossings": len(est.tsdf_zero_crossings()),
            "candidates": len(cand), "plane": plane,
            "compute_ground_plane_us": {"median": float(np.median(ts)), "min": float(np.min(ts))}}
-    for shape, env in (("fit_us", "0"), ("fit_reference_shape_us", "1")):
-        os.environ["NVB_RANSAC_REFERENCE_SHAPE"] = env
-        p0 = nvb.ransac_fit_plane(cand, 1000, mapper=m)
-        tf = [timed(lambda: nvb.ransac_fit_plane(cand, 1000, mapper=m))[0] for _ in range(repeats)]
-        out[shape] = {"median": float(np.median(tf)), "min": float(np.min(tf)), "same_plane": p0 == plane}
-    os.environ["NVB_RANSAC_REFERENCE_SHAPE"] = "0"
+    p0 = nvb.ransac_fit_plane(cand, 1000, mapper=m)
+    tf = [timed(lambda: nvb.ransac_fit_plane(cand, 1000, mapper=m))[0] for _ in range(repeats)]
+    out["fit_us"] = {"median": float(np.median(tf)), "min": float(np.min(tf)), "same_plane": p0 == plane}
     out["kernel_us"] = kernel_times(m, repeats)
     return out
 
