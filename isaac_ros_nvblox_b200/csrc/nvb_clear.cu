@@ -30,13 +30,13 @@ __global__ void selectOutsideRadiusKernel(DevLayer L, float cx, float cy, float 
   }
 }
 
-__global__ void trackerDropDeadKernel(const int4* dead, const int* dead_count, int* d0, int* d1, int* d2) {
+__global__ void trackerDropDeadKernel(const int4* dead, const int* dead_count, const TrackerLists t) {
   const int n = *dead_count;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int slot = dead[i].x;
-    if (d0) d0[slot] = 0;
-    if (d1) d1[slot] = 0;
-    if (d2) d2[slot] = 0;
+#pragma unroll
+    for (const TrackerList& l : t.list)
+      if (l.dirty) l.dirty[slot] = 0;
   }
 }
 
@@ -73,9 +73,7 @@ __global__ void shapeSelectKernel(const __grid_constant__ ShapeClearArgs a) {
     for (int s = 0; s < a.num_shapes && !touched; s++) touched = shapeTouchesBlock(a.shapes[s], idx, a.block_size);
     if (!touched) continue;
     a.sel[atomicAdd(a.sel_count, 1)] = make_int4(i, idx[0], idx[1], idx[2]);
-    if (a.dirty != nullptr && atomicExch(a.dirty + i, 1) == 0) a.todo_slots[atomicAdd(a.todo_count, 1)] = i;
-    if (a.dirty2 != nullptr && atomicExch(a.dirty2 + i, 1) == 0) a.todo2_slots[atomicAdd(a.todo2_count, 1)] = i;
-    if (a.dirty3 != nullptr && atomicExch(a.dirty3 + i, 1) == 0) a.todo3_slots[atomicAdd(a.todo3_count, 1)] = i;
+    trackerAdd(a.tracker, i);
   }
 }
 
@@ -123,11 +121,9 @@ void launchSelectOutsideRadius(const DevLayer& layer, const float center[3], flo
                                                                  dead, dead_count);
 }
 
-void launchTrackerDropDead(const int4* dead, const int* dead_count, int upper, int* dirty0, int* dirty1, int* dirty2,
-                           cudaStream_t stream) {
-  if (!dirty0 && !dirty1 && !dirty2) return;
+void launchTrackerDropDead(const int4* dead, const int* dead_count, int upper, const TrackerLists& t, cudaStream_t stream) {
   const int grid = upper < 1 ? 1 : (upper + 255) / 256 < kHelperCtas ? (upper + 255) / 256 : kHelperCtas;
-  trackerDropDeadKernel<<<grid, 256, 0, stream>>>(dead, dead_count, dirty0, dirty1, dirty2);
+  trackerDropDeadKernel<<<grid, 256, 0, stream>>>(dead, dead_count, t);
 }
 
 void launchShapeSelect(const ShapeClearArgs& a, cudaStream_t stream) {

@@ -304,6 +304,20 @@ struct OccKernelParams {
   float min_log_odds, max_log_odds;
 };
 
+// The block-update tracker on the device (BlocksToUpdateTracker, map/blocks_to_update_tracker.h). A consumer's pending
+// blocks: a dirty word per projective slot and the list of the slots whose word is set; a null `dirty`: not told.
+enum BlocksToUpdateType { kEsdfBlocks, kFreespaceBlocks, kColorMeshBlocks, kNumBlocksToUpdateTypes };
+struct TrackerList { int *dirty, *slots, *count; };
+struct TrackerLists { TrackerList list[kNumBlocksToUpdateTypes]; };  // by BlocksToUpdateType
+#ifdef __CUDACC__
+// addBlocksToUpdate (map/blocks_to_update_tracker.cpp:33-63): unique append of `slot` to every consumer that is told.
+__device__ __forceinline__ void trackerAdd(const TrackerLists& t, int slot) {
+#pragma unroll
+  for (const TrackerList& l : t.list)
+    if (l.dirty != nullptr && atomicExch(l.dirty + slot, 1) == 0) l.slots[atomicAdd(l.count, 1)] = slot;
+}
+#endif
+
 // ---------------------------------------------------------------------------
 // Kernel launchers (implemented in the .cu files; all enqueue on `stream`).
 // ---------------------------------------------------------------------------
@@ -326,15 +340,7 @@ struct CompactArgs {
   int allocate;                    // 1: find-or-insert into layer
   DevLayer layer;
   int* error;
-  int* dirty;                      // per-slot dirty flag for the ESDF tracker (may be null)
-  int* todo_slots;
-  int* todo_count;
-  int* dirty2;                     // second consumer of the tracker (freespace; may be null)
-  int* dirty3;                     // third consumer (mesh; may be null)
-  int* todo3_slots;
-  int* todo3_count;
-  int* todo2_slots;
-  int* todo2_count;
+  TrackerLists tracker;            // told about every block found or inserted (allocate only)
 };
 int compactNumTiles(const ViewGrid& grid);
 bool compactUsesTickets(const ViewGrid& grid);
@@ -466,12 +472,10 @@ __device__ __forceinline__ bool isVoxelFreespace(const DevLayer& layer, int slot
 // nvb_tsdf.cu: freespace (FreespaceIntegrator, integrators/internal/cuda/impl/freespace_integrator_impl.cuh)
 struct FreespaceArgs {
   DevLayer tsdf, fs;
-  // blocks to update: TSDF slots from the tracker, or explicit indices
-  const int* todo_slots;
-  const int* todo_count;
+  // blocks to update: TSDF slots from the tracker (its dirty words are cleared for the consumed slots), or explicit indices
+  TrackerList todo;
   const int* in_xyz;
   int n_explicit;
-  int* tracker_dirty;  // cleared for the consumed slots (tracker mode)
   int4* work;          // {tsdf slot, freespace slot, -, -}
   int* work_count;
   int* error;
@@ -500,9 +504,7 @@ struct MarkFreeArgs {
   int4* out;       // {x, y, z, slot} of the blocks inside the radius
   int* out_count;
   int* error;
-  int *dirty, *todo_slots, *todo_count;     // ESDF tracker (nullptr before its first query)
-  int *dirty2, *todo2_slots, *todo2_count;  // freespace tracker
-  int *dirty3, *todo3_slots, *todo3_count;  // mesh tracker
+  TrackerLists tracker;
 };
 void launchMarkFreeSphere(const MarkFreeArgs& a, int num_sms, cudaStream_t stream);
 
@@ -554,7 +556,6 @@ struct DecayArgs {
   // outputs
   int4* dead;  // {slot, x, y, z} of deallocated blocks
   int* dead_count;
-  int* tracker_dirty;
 };
 void launchDecay(const DecayArgs& a, int num_sms, cudaStream_t stream);
 void launchMarkSkipped(const DevLayer& layer, const int* xyz_dev, int n, int* skip_stamp, int skip_seq, cudaStream_t stream);
@@ -585,11 +586,9 @@ struct MeshCtx {
   int* arena_state;  // kArena* ints
   int* counts;       // per list entry: pre-weld vertex count
   int* offsets;      // per list entry: arena offset
-  const int* in_xyz;       // explicit list (device) or ...
-  const int* in_slots;     // ... TSDF slots from the tracker
-  const int* in_count_dev;
+  const int* in_xyz;       // explicit list (device, in_count_host entries) or ...
+  TrackerList todo;        // ... TSDF slots from the tracker
   int in_count_host;
-  int* tracker_dirty;
   float block_size, voxel_size, min_weight, cutoff_distance_m;
   int weld;
   int* error;
@@ -622,7 +621,7 @@ void launchSliceAabb(const DevLayer& esdf, int zb, int* out4, cudaStream_t strea
 void launchSliceImage(const DevLayer& esdf, float block_size, float min_x, float min_y, float slice_height, float unobserved_value,
                       int rows, int cols, float* image, signed char* grid, cudaStream_t stream);
 void launchRemoveBlocks(const DevLayer& layer, const int4* dead, const int* dead_count, int upper, cudaStream_t stream);
-void launchTodoAll(const DevLayer& tsdf, int* dirty, int* todo_slots, int* todo_count, cudaStream_t stream);
+void launchTodoAll(const DevLayer& tsdf, const TrackerList& t, cudaStream_t stream);
 // Drops the slots that are dead in `layer` from a list of its slots (*count entries), keeping the order of the others.
 void launchDropDeadSlots(const DevLayer& layer, int* list, int* count, cudaStream_t stream);
 
@@ -632,8 +631,7 @@ void launchSelectOutsideRadius(const DevLayer& layer, const float center[3], flo
                                int* dead_count, cudaStream_t stream);
 // BlocksToUpdateTracker::removeClearedBlocksFromTracking: zero the dirty words of the dead slots (null arrays skipped); the
 // todo lists then lose them through launchDropDeadSlots.
-void launchTrackerDropDead(const int4* dead, const int* dead_count, int upper, int* dirty0, int* dirty1, int* dirty2,
-                           cudaStream_t stream);
+void launchTrackerDropDead(const int4* dead, const int* dead_count, int upper, const TrackerLists& t, cudaStream_t stream);
 struct ShapeClearArgs {
   DevLayer layer;
   int voxel_kind;                    // 0 TsdfVoxel, 1 OccupancyVoxel, 2 ColorVoxel
@@ -642,9 +640,7 @@ struct ShapeClearArgs {
   float block_size;
   int4* sel;                         // {slot, x, y, z} of the blocks a shape touches
   int* sel_count;
-  int *dirty, *todo_slots, *todo_count;     // ESDF tracker (null: not told)
-  int *dirty2, *todo2_slots, *todo2_count;  // freespace tracker
-  int *dirty3, *todo3_slots, *todo3_count;  // mesh tracker
+  TrackerLists tracker;
 };
 void launchShapeSelect(const ShapeClearArgs& a, cudaStream_t stream);
 void launchShapeClear(const ShapeClearArgs& a, int num_sms, cudaStream_t stream);

@@ -130,9 +130,9 @@ __device__ __forceinline__ MeshHeader* meshHeader(const MeshCtx& c, int slot) {
 
 // Entry i of the call's list -> (index, TSDF slot). Lists are unique (a set in every caller).
 __device__ __forceinline__ bool listEntry(const MeshCtx& c, int i, int* bx, int* by, int* bz, int* tslot) {
-  if (c.in_slots) {
-    const int t = c.in_slots[i];
-    if (c.tracker_dirty) c.tracker_dirty[t] = 0;  // this block's pending update is being consumed
+  if (c.todo.slots) {
+    const int t = c.todo.slots[i];
+    c.todo.dirty[t] = 0;  // this block's pending update is being consumed
     *bx = c.tsdf.block_index[3 * t], *by = c.tsdf.block_index[3 * t + 1], *bz = c.tsdf.block_index[3 * t + 2];
     *tslot = *bx == kDeadSlotX ? -1 : t;
   } else {
@@ -146,7 +146,7 @@ __device__ __forceinline__ bool listEntry(const MeshCtx& c, int i, int* bx, int*
 __global__ void __launch_bounds__(kMeshThreads) meshCountKernel(MeshCtx c) {
   __shared__ CubeShared s;
   __shared__ int s_entry[4];
-  const int n = c.in_count_dev ? *c.in_count_dev : c.in_count_host;
+  const int n = c.todo.count ? *c.todo.count : c.in_count_host;
   const int tid = threadIdx.x;
   for (int i = blockIdx.x; i < n; i += gridDim.x) {
     __syncthreads();
@@ -195,7 +195,7 @@ __global__ void __launch_bounds__(1024) meshScanKernel(MeshCtx c) {
   __shared__ int warp_sum[32];
   __shared__ int carry;
   __shared__ long long base;
-  const int n = c.in_count_dev ? *c.in_count_dev : c.in_count_host;
+  const int n = c.todo.count ? *c.todo.count : c.in_count_host;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) carry = 0;
   __syncthreads();
@@ -249,7 +249,7 @@ __device__ __forceinline__ void edgeVertex(const float pos[8][3], const float sd
 __global__ void __launch_bounds__(kMeshThreads) meshEmitKernel(MeshCtx c) {
   __shared__ CubeShared s;
   __shared__ int s_entry[4];
-  const int n = c.in_count_dev ? *c.in_count_dev : c.in_count_host;
+  const int n = c.todo.count ? *c.todo.count : c.in_count_host;
   const int tid = threadIdx.x;
   if (blockIdx.x == 0 && tid == 0) c.arena_state[kArenaUsed] = c.arena_state[kArenaLastBase] + c.arena_state[kArenaLastTotal];
   for (int i = blockIdx.x; i < n; i += gridDim.x) {
@@ -258,8 +258,8 @@ __global__ void __launch_bounds__(kMeshThreads) meshEmitKernel(MeshCtx c) {
     __syncthreads();
     if (tid == 0) {
       int bx, by, bz, tslot;
-      if (c.in_slots) {
-        const int t = c.in_slots[i];
+      if (c.todo.slots) {
+        const int t = c.todo.slots[i];
         bx = c.tsdf.block_index[3 * t], by = c.tsdf.block_index[3 * t + 1], bz = c.tsdf.block_index[3 * t + 2], tslot = t;
       } else {
         bx = c.in_xyz[3 * i], by = c.in_xyz[3 * i + 1], bz = c.in_xyz[3 * i + 2];
@@ -339,7 +339,7 @@ __global__ void __launch_bounds__(kMeshThreads) meshWeldKernel(MeshCtx c) {
   float* stage_v = reinterpret_cast<float*>(key);
   __shared__ int warp_sum[kMeshThreads / 32];
   __shared__ int s_ms;
-  const int n = c.in_count_dev ? *c.in_count_dev : c.in_count_host;
+  const int n = c.todo.count ? *c.todo.count : c.in_count_host;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int i = blockIdx.x; i < n; i += gridDim.x) {
     const int nv = c.counts[i];
@@ -416,8 +416,8 @@ __global__ void __launch_bounds__(kMeshThreads) meshWeldKernel(MeshCtx c) {
     }
     if (tid == 0) {
       int bx, by, bz;
-      if (c.in_slots) {
-        const int t = c.in_slots[i];
+      if (c.todo.slots) {
+        const int t = c.todo.slots[i];
         bx = c.tsdf.block_index[3 * t], by = c.tsdf.block_index[3 * t + 1], bz = c.tsdf.block_index[3 * t + 2];
       } else {
         bx = c.in_xyz[3 * i], by = c.in_xyz[3 * i + 1], bz = c.in_xyz[3 * i + 2];
@@ -436,13 +436,13 @@ __global__ void __launch_bounds__(kMeshThreads) meshWeldKernel(MeshCtx c) {
 // ---- colour (updateAppearanceGPU, mesh_integrator_appearance.cu:281-380)
 __global__ void __launch_bounds__(kMeshThreads) meshColorKernel(MeshCtx c) {
   __shared__ int s_ms, s_cs;
-  const int n = c.in_count_dev ? *c.in_count_dev : c.in_count_host;
+  const int n = c.todo.count ? *c.todo.count : c.in_count_host;
   const int tid = threadIdx.x;
   for (int i = blockIdx.x; i < n; i += gridDim.x) {
     __syncthreads();
     int bx, by, bz;
-    if (c.in_slots) {
-      const int t = c.in_slots[i];
+    if (c.todo.slots) {
+      const int t = c.todo.slots[i];
       bx = c.tsdf.block_index[3 * t], by = c.tsdf.block_index[3 * t + 1], bz = c.tsdf.block_index[3 * t + 2];
     } else {
       bx = c.in_xyz[3 * i], by = c.in_xyz[3 * i + 1], bz = c.in_xyz[3 * i + 2];

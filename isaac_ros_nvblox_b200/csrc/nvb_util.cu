@@ -106,8 +106,8 @@ __global__ void rehashKernel(DevLayer L, int count) {
 }
 
 // BlocksToUpdateState::setUpdateAllBlocks (map/blocks_to_update_tracker.h): the todo
-// list becomes every allocated TSDF slot.
-// (*todo_count is zeroed by a memset in front of this kernel; deallocated slots are skipped.)
+// list becomes every allocated TSDF slot. The kernel only appends: the caller zeroes *todo_count first, which drops the
+// pending entries like setUpdateAllBlocks clears the pending set. Deallocated slots are skipped.
 __global__ void todoAllKernel(DevLayer tsdf, int* dirty, int* todo_slots, int* todo_count) {
   const int n = *tsdf.count < tsdf.capacity ? *tsdf.count : tsdf.capacity;
   const int lane = threadIdx.x & 31;
@@ -262,9 +262,8 @@ void launchFillU64(unsigned long long* p, unsigned long long v, size_t n, cudaSt
 void launchRehash(const DevLayer& layer, int count, cudaStream_t stream) {
   if (count > 0) rehashKernel<<<(count + 255) / 256, 256, 0, stream>>>(layer, count);
 }
-void launchTodoAll(const DevLayer& tsdf, int* dirty, int* todo_slots, int* todo_count, cudaStream_t stream) {
-  cudaMemsetAsync(todo_count, 0, sizeof(int), stream);
-  todoAllKernel<<<296, 256, 0, stream>>>(tsdf, dirty, todo_slots, todo_count);
+void launchTodoAll(const DevLayer& tsdf, const TrackerList& t, cudaStream_t stream) {
+  todoAllKernel<<<296, 256, 0, stream>>>(tsdf, t.dirty, t.slots, t.count);
 }
 
 }  // namespace nvb
