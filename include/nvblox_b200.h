@@ -535,6 +535,53 @@ NVB_API int32_t nvb_mapper_dynamics_device_buffers(NvbMapper* m, NvbDynamicsBuff
  * enqueued so far on producer's stream. No host synchronisation. */
 NVB_API int32_t nvb_mapper_wait_for(NvbMapper* waiter, NvbMapper* producer);
 
+/* ImageMasker parameters (C/include/nvblox/semantics/image_masker.h:110-119). */
+typedef struct {
+  float occlusion_threshold_m;              /* 0.25: a point more than this behind the nearest one seen from the mask camera is occluded */
+  float depth_masked_image_invalid_pixel;   /* -1: written to the masked (foreground) output where the pixel is not masked */
+  float depth_unmasked_image_invalid_pixel; /* -1: written to the unmasked (background) output where the pixel is masked */
+} NvbImageMaskerParams;
+NVB_API void nvb_default_image_masker_params(NvbImageMaskerParams* p);
+/* ImageMasker::splitImageOnGPU(depth, mask, T_CM_CD, depth_camera, mask_camera, ...) (C/src/semantics/image_masker.cu:
+ * 316-392) in three launches on the mapper's stream: a mask-sized min-depth image is filled with FLT_MAX; every depth pixel
+ * is unprojected, moved by T_CM_CD (column-major 4x4) into the mask camera and projected, and its z is min-reduced into
+ * the 5 x 5 patch around (int)(u + k - 2), (int)(v + k - 2); then a pixel goes to the foreground when it projects, the mask
+ * (bytes != 0) is set at (int)u, (int)v and min_depth + occlusion_threshold_m >= z there. Every other pixel, and every +-inf
+ * or NaN depth, goes to the background. Each output holds the depth where the other holds its invalid value. With
+ * with_overlay != 0 the RGB overlay is grey 12.75 * depth (clamped to 0..255; NaN 255) with red 255 on foreground pixels.
+ * Deviations from the reference: a projection exactly on u == width or v == height is a miss here (the reference reads
+ * past the mask's row); a negative depth has grey 0 (undefined in the reference). Sizes must match the cameras
+ * (width x height); depth, mask (mask_rows x mask_cols bytes) are in `memory`. Host inputs are staged in buffers the
+ * mapper keeps. The outputs stay in the mapper (nvb_mapper_split_output, nvb_mapper_split_device_buffers); the call does
+ * not synchronise (the reference does). */
+NVB_API int32_t nvb_mapper_split_depth_image(NvbMapper* m, const float* depth, int32_t depth_rows, int32_t depth_cols,
+                                             const uint8_t* mask, int32_t mask_rows, int32_t mask_cols, int32_t memory,
+                                             const float* T_CM_CD, const NvbCamera* depth_cam, const NvbCamera* mask_cam,
+                                             const NvbImageMaskerParams* params, int32_t with_overlay);
+/* Outputs of nvb_mapper_split_depth_image. */
+typedef enum { NVB_SPLIT_BACKGROUND = 0, NVB_SPLIT_FOREGROUND = 1, NVB_SPLIT_OVERLAY = 2 } NvbSplitOutput;
+/* One output of the last split: *rows, *cols of the frame (0 x 0 before the first split, and for the overlay when the last
+ * split made none); out (rows x cols floats, resp. x 3 bytes for the overlay, in `memory`) may be NULL. A host copy
+ * synchronises the mapper's stream; a device copy is enqueued on it. */
+NVB_API int32_t nvb_mapper_split_output(NvbMapper* m, int32_t which, void* out, int32_t memory, int32_t* rows, int32_t* cols);
+/* The split's device buffers, for a consumer on another stream (a second mapper, through nvb_mapper_wait_for). They stay
+ * valid, and their contents unchanged, until the next nvb_mapper_split_depth_image on this mapper or its destruction. */
+typedef struct {
+  const float* background;  /* the unmasked depth */
+  const float* foreground;  /* the masked depth */
+  const uint8_t* overlay;   /* RGB; NULL when the last split made none */
+  int32_t rows, cols;
+} NvbSplitBuffers;
+NVB_API int32_t nvb_mapper_split_device_buffers(NvbMapper* m, NvbSplitBuffers* out);
+/* ImageMasker::splitImageOnGPU(color, mask, ...) (C/src/semantics/image_masker.cu:44-78,305-314): the mask lies on top of
+ * the image; a pixel with mask != 0 is copied to masked_out, the others to unmasked_out, and the other output is black.
+ * overlay_out (may be NULL) is the input with red = 255 on masked pixels. rgb and the outputs are rows x cols x 3 bytes,
+ * mask rows x cols bytes, all in `memory`. Device buffers: enqueued on the mapper's stream; host buffers: returns when the
+ * outputs are written. */
+NVB_API int32_t nvb_mapper_split_color_image(NvbMapper* m, const uint8_t* rgb, const uint8_t* mask, int32_t memory,
+                                             int32_t rows, int32_t cols, uint8_t* unmasked_out, uint8_t* masked_out,
+                                             uint8_t* overlay_out);
+
 /* EsdfSlicer::sliceLayerToDistanceImage (C/include/nvblox/integrators/esdf_slicer.h:52-78, C/src/integrators/esdf_slicer.cu:
  * 25-67,112-215) and, if grid_host != NULL, EsdfSlicer::occupancyGridFromSliceImage (:78-110,254-300) of the ESDF layer
  * (3-D or 2-D) at slice_height_m: one pixel per voxel over the AABB of the ESDF blocks at that height, rows along y,

@@ -14,6 +14,7 @@ NVB_OK = 0
 NVB_MEM_HOST, NVB_MEM_DEVICE = 0, 1
 NVB_LAYER_TSDF, NVB_LAYER_ESDF, NVB_LAYER_OCCUPANCY, NVB_LAYER_FREESPACE, NVB_LAYER_COLOR, NVB_LAYER_MESH = 0, 1, 2, 3, 4, 5
 NVB_PROJECTIVE_TSDF, NVB_PROJECTIVE_OCCUPANCY, NVB_PROJECTIVE_TSDF_WITH_FREESPACE = 0, 1, 2
+NVB_SPLIT_BACKGROUND, NVB_SPLIT_FOREGROUND, NVB_SPLIT_OVERLAY = 0, 1, 2
 
 # Every symbol include/nvblox_b200.h declares (checked by tests/test_cabi_symbols.py).
 EXPORTED_SYMBOLS = [
@@ -49,6 +50,8 @@ EXPORTED_SYMBOLS = [
     "nvb_mapper_compute_ground_plane", "nvb_mapper_ground_plane", "nvb_mapper_ground_plane_points", "nvb_ransac_fit_plane",
     "nvb_mapper_compute_dynamics", "nvb_mapper_remove_small_components", "nvb_mapper_dynamic_mask", "nvb_mapper_dynamic_overlay",
     "nvb_mapper_dynamic_points", "nvb_mapper_dynamics_device_buffers", "nvb_mapper_wait_for",
+    "nvb_default_image_masker_params", "nvb_mapper_split_depth_image", "nvb_mapper_split_output",
+    "nvb_mapper_split_device_buffers", "nvb_mapper_split_color_image",
     "nvb_layer_query_voxels", "nvb_layer_interpolate", "nvb_query_esdf", "nvb_query_tsdf", "nvb_query_occupancy",
 ]
 
@@ -147,6 +150,16 @@ class NvbGroundPlaneParams(C.Structure):
 class NvbDynamicsBuffers(C.Structure):
     _fields_ = [("depth", C.c_void_p), ("mask", C.c_void_p), ("cleaned_mask", C.c_void_p), ("overlay", C.c_void_p),
                 ("points", C.c_void_p), ("num_points", C.c_void_p), ("rows", C.c_int32), ("cols", C.c_int32)]
+
+
+class NvbImageMaskerParams(C.Structure):
+    _fields_ = [("occlusion_threshold_m", C.c_float), ("depth_masked_image_invalid_pixel", C.c_float),
+                ("depth_unmasked_image_invalid_pixel", C.c_float)]
+
+
+class NvbSplitBuffers(C.Structure):
+    _fields_ = [("background", C.c_void_p), ("foreground", C.c_void_p), ("overlay", C.c_void_p), ("rows", C.c_int32),
+                ("cols", C.c_int32)]
 
 
 class NvbMapperOptions(C.Structure):
@@ -308,6 +321,13 @@ def load(path=None):
     L.nvb_mapper_dynamic_points.argtypes = [vp, vp, i32, i32, ip]
     L.nvb_mapper_dynamics_device_buffers.argtypes = [vp, C.POINTER(NvbDynamicsBuffers)]
     L.nvb_mapper_wait_for.argtypes = [vp, vp]
+    L.nvb_default_image_masker_params.argtypes = [C.POINTER(NvbImageMaskerParams)]
+    L.nvb_default_image_masker_params.restype = None
+    L.nvb_mapper_split_depth_image.argtypes = [vp, vp, i32, i32, vp, i32, i32, i32, fp, C.POINTER(NvbCamera),
+                                               C.POINTER(NvbCamera), C.POINTER(NvbImageMaskerParams), i32]
+    L.nvb_mapper_split_output.argtypes = [vp, i32, vp, i32, ip, ip]
+    L.nvb_mapper_split_device_buffers.argtypes = [vp, C.POINTER(NvbSplitBuffers)]
+    L.nvb_mapper_split_color_image.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp]
     i64 = C.c_int64
     L.nvb_layer_query_voxels.argtypes = [vp, i32, vp, i32, i64, vp, vp]
     L.nvb_layer_interpolate.argtypes = [vp, i32, vp, i32, i64, vp, vp]

@@ -254,6 +254,16 @@ struct NvbMapper {
   DeviceArray<int> cc_labels;
   DeviceArray<int> cc_sizes;
   DeviceArray<unsigned char> cc_stage;  // host masks staged for the filter (input, then output)
+  // image masker (nvb_masker.cu): the last split's outputs, sized by pixels; staged host inputs and the min-depth scratch
+  DeviceArray<float> msk_depth_stage;
+  DeviceArray<unsigned char> msk_mask_stage;
+  DeviceArray<float> msk_min_depth;      // mask-sized
+  DeviceArray<float> msk_background;
+  DeviceArray<float> msk_foreground;
+  DeviceArray<unsigned char> msk_overlay;
+  DeviceArray<unsigned char> msk_color;  // host colour splits: input, mask and the three outputs
+  int msk_rows = 0, msk_cols = 0;
+  bool msk_has_overlay = false;
   cudaEvent_t dyn_event = nullptr;    // nvb_mapper_wait_for: recorded on this mapper's stream
   cudaEvent_t query_event = nullptr;  // point queries (nvb_query_*): the hand-over between this mapper and the query's stream
   // last integrated view (Mapper::last_posed_depth_image_, mapper.h:830-833), kept when keep_last_view is set
@@ -2671,6 +2681,113 @@ int32_t nvb_mapper_wait_for(NvbMapper* waiter, NvbMapper* producer) {
   NVB_CUDA(cudaEventRecord(producer->dyn_event, producer->stream));
   NVB_CUDA(cudaSetDevice(waiter->device));
   NVB_CUDA(cudaStreamWaitEvent(waiter->stream, producer->dyn_event, 0));
+  return NVB_OK;
+}
+
+void nvb_default_image_masker_params(NvbImageMaskerParams* p) {
+  if (!p) return;
+  p->occlusion_threshold_m = 0.25f;
+  p->depth_masked_image_invalid_pixel = -1.0f;
+  p->depth_unmasked_image_invalid_pixel = -1.0f;
+}
+
+int32_t nvb_mapper_split_depth_image(NvbMapper* m, const float* depth, int32_t depth_rows, int32_t depth_cols,
+                                     const uint8_t* mask, int32_t mask_rows, int32_t mask_cols, int32_t memory,
+                                     const float* T_CM_CD, const NvbCamera* depth_cam, const NvbCamera* mask_cam,
+                                     const NvbImageMaskerParams* params, int32_t with_overlay) {
+  if (!m || !depth || !mask || !T_CM_CD || !depth_cam || !mask_cam || !params) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (depth_rows <= 0 || depth_cols <= 0 || mask_rows <= 0 || mask_cols <= 0)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "images must have positive size");
+  if (depth_rows != depth_cam->height || depth_cols != depth_cam->width)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "depth image size does not match the depth camera");
+  if (mask_rows != mask_cam->height || mask_cols != mask_cam->width)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "mask size does not match the mask camera");
+  if ((long long)depth_rows * depth_cols > kMaxDynamicsPixels || (long long)mask_rows * mask_cols > kMaxDynamicsPixels)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "image too large");
+  NVB_CUDA(cudaSetDevice(m->device));
+  const size_t n = (size_t)depth_rows * depth_cols, mn = (size_t)mask_rows * mask_cols;
+  // Growing synchronises the mapper's streams first, so no pending split still uses the old buffers.
+  NVB_CUDA(m->msk_background.grow(m, n, n));
+  NVB_CUDA(m->msk_foreground.grow(m, n, n));
+  if (with_overlay) NVB_CUDA(m->msk_overlay.grow(m, 3 * n, 3 * n));
+  NVB_CUDA(m->msk_min_depth.grow(m, mn, mn));
+  MaskerArgs a{};
+  a.depth = depth, a.mask = mask;
+  if (memory == NVB_MEM_HOST) {
+    NVB_CUDA(m->msk_depth_stage.grow(m, n, n));
+    NVB_CUDA(m->msk_mask_stage.grow(m, mn, mn));
+    NVB_CUDA(cudaMemcpyAsync(m->msk_depth_stage.get(), depth, n * sizeof(float), cudaMemcpyHostToDevice, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(m->msk_mask_stage.get(), mask, mn, cudaMemcpyHostToDevice, m->stream));
+    a.depth = m->msk_depth_stage.get(), a.mask = m->msk_mask_stage.get();
+  }
+  a.rows = depth_rows, a.cols = depth_cols, a.mrows = mask_rows, a.mcols = mask_cols;
+  a.T_CM_CD = rigidFromColMajor(T_CM_CD);
+  a.depth_cam = *depth_cam, a.mask_cam = *mask_cam;
+  a.occlusion_threshold_m = params->occlusion_threshold_m;
+  a.masked_invalid = params->depth_masked_image_invalid_pixel;
+  a.unmasked_invalid = params->depth_unmasked_image_invalid_pixel;
+  a.min_depth = m->msk_min_depth.get();
+  a.unmasked = m->msk_background.get(), a.masked = m->msk_foreground.get();
+  a.overlay = with_overlay ? m->msk_overlay.get() : nullptr;
+  launchSplitDepth(a, m->num_sms, m->stream);
+  NVB_CUDA(cudaGetLastError());
+  m->launches += 3;
+  m->msk_rows = depth_rows, m->msk_cols = depth_cols, m->msk_has_overlay = with_overlay != 0;
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_split_output(NvbMapper* m, int32_t which, void* out, int32_t memory, int32_t* rows, int32_t* cols) {
+  if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  const size_t n = (size_t)m->msk_rows * m->msk_cols;
+  const void* src;
+  size_t bytes;
+  if (which == NVB_SPLIT_BACKGROUND) src = m->msk_background.get(), bytes = n * sizeof(float);
+  else if (which == NVB_SPLIT_FOREGROUND) src = m->msk_foreground.get(), bytes = n * sizeof(float);
+  else if (which == NVB_SPLIT_OVERLAY) src = m->msk_overlay.get(), bytes = m->msk_has_overlay ? 3 * n : 0;
+  else return fail(NVB_ERR_INVALID_ARGUMENT, "bad split output");
+  *rows = bytes ? m->msk_rows : 0, *cols = bytes ? m->msk_cols : 0;
+  NVB_CUDA(cudaSetDevice(m->device));
+  return copyDynamicsOut(m, out, src, bytes, memory);
+}
+
+int32_t nvb_mapper_split_device_buffers(NvbMapper* m, NvbSplitBuffers* out) {
+  if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  out->background = m->msk_background.get(), out->foreground = m->msk_foreground.get();
+  out->overlay = m->msk_has_overlay ? m->msk_overlay.get() : nullptr;
+  out->rows = m->msk_rows, out->cols = m->msk_cols;
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_split_color_image(NvbMapper* m, const uint8_t* rgb, const uint8_t* mask, int32_t memory, int32_t rows,
+                                     int32_t cols, uint8_t* unmasked_out, uint8_t* masked_out, uint8_t* overlay_out) {
+  if (!m || !rgb || !mask || !unmasked_out || !masked_out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (rows <= 0 || cols <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "image must have positive size");
+  if ((long long)rows * cols > kMaxDynamicsPixels) return fail(NVB_ERR_INVALID_ARGUMENT, "image too large");
+  NVB_CUDA(cudaSetDevice(m->device));
+  const size_t n = (size_t)rows * cols;
+  ColorSplitArgs a{};
+  a.pixels = (long long)n;
+  a.rgb = rgb, a.mask = mask, a.unmasked = unmasked_out, a.masked = masked_out, a.overlay = overlay_out;
+  unsigned char* s = nullptr;
+  if (memory == NVB_MEM_HOST) {  // [rgb | mask | unmasked | masked | overlay]
+    NVB_CUDA(m->msk_color.grow(m, 13 * n, 13 * n));
+    s = m->msk_color.get();
+    NVB_CUDA(cudaMemcpyAsync(s, rgb, 3 * n, cudaMemcpyHostToDevice, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(s + 3 * n, mask, n, cudaMemcpyHostToDevice, m->stream));
+    a.rgb = s, a.mask = s + 3 * n, a.unmasked = s + 4 * n, a.masked = s + 7 * n, a.overlay = overlay_out ? s + 10 * n : nullptr;
+  }
+  launchSplitColor(a, m->stream);
+  NVB_CUDA(cudaGetLastError());
+  m->launches++;
+  if (memory == NVB_MEM_HOST) {
+    NVB_CUDA(cudaMemcpyAsync(unmasked_out, a.unmasked, 3 * n, cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaMemcpyAsync(masked_out, a.masked, 3 * n, cudaMemcpyDeviceToHost, m->stream));
+    if (overlay_out) NVB_CUDA(cudaMemcpyAsync(overlay_out, a.overlay, 3 * n, cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+  }
   return NVB_OK;
 }
 

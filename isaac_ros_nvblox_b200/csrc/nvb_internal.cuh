@@ -700,6 +700,32 @@ struct CcArgs {
 };
 void launchRemoveSmallComponents(const CcArgs& a, int num_sms, cudaStream_t stream);
 
+// nvb_masker.cu: ImageMasker::splitImageOnGPU (depth, with occlusion, and colour)
+struct MaskerArgs {
+  const float* depth;         // rows x cols, device
+  int rows, cols;             // the depth camera's size
+  const unsigned char* mask;  // mrows x mcols, device
+  int mrows, mcols;           // the mask camera's size
+  Rigid T_CM_CD;
+  NvbCamera depth_cam, mask_cam;
+  float occlusion_threshold_m, masked_invalid, unmasked_invalid;
+  float* min_depth;           // mrows x mcols scratch
+  float* unmasked;            // rows x cols: the background
+  float* masked;              // rows x cols: the foreground
+  unsigned char* overlay;     // rows x cols x 3 (RGB), or nullptr
+};
+// fill + min depth + split: three launches
+void launchSplitDepth(const MaskerArgs& a, int num_sms, cudaStream_t stream);
+struct ColorSplitArgs {
+  const unsigned char* rgb;   // pixels x 3
+  const unsigned char* mask;  // pixels
+  long long pixels;
+  unsigned char* unmasked;    // pixels x 3
+  unsigned char* masked;      // pixels x 3
+  unsigned char* overlay;     // pixels x 3, or nullptr
+};
+void launchSplitColor(const ColorSplitArgs& a, cudaStream_t stream);
+
 // nvb_query.cu: point queries (VoxelBlockLayer::getVoxels, interpolation::interpolateOnCPU, nvblox_torch's sdf_query.cu)
 struct QueryLayer {
   DevLayer layer;

@@ -841,6 +841,90 @@ class DynamicsDetection:
         return {k: getattr(b, k) for k, _ in b._fields_}
 
 
+class ImageMasker:
+    """ImageMasker (semantics/image_masker.h) on one mapper's device and stream: split_depth sends each depth pixel that
+    lands, unoccluded, on a set pixel of a mask seen from another camera to the foreground, the rest to the background.
+    The depth split's outputs live in the mapper until its next split; the colour split writes the caller's buffers."""
+
+    def __init__(self, mapper):
+        self._m = mapper
+        self._p = _lib.NvbImageMaskerParams()
+        mapper._L.nvb_default_image_masker_params(C.byref(self._p))
+
+    def params(self, occlusion_threshold_m=None, depth_masked_image_invalid_pixel=None,
+               depth_unmasked_image_invalid_pixel=None):
+        """Sets the given parameters; returns all three as a dict."""
+        for k, v in (("occlusion_threshold_m", occlusion_threshold_m),
+                     ("depth_masked_image_invalid_pixel", depth_masked_image_invalid_pixel),
+                     ("depth_unmasked_image_invalid_pixel", depth_unmasked_image_invalid_pixel)):
+            if v is not None:
+                setattr(self._p, k, float(v))
+        return {k: getattr(self._p, k) for k, _ in self._p._fields_}
+
+    def _split(self, depth, depth_rows, depth_cols, mask, mask_rows, mask_cols, memory, T_CM_CD, depth_camera, mask_camera,
+               overlay):
+        check(self._m._L.nvb_mapper_split_depth_image(self._m._h, depth, int(depth_rows), int(depth_cols), mask,
+                                                      int(mask_rows), int(mask_cols), memory, _fp(colmajor(T_CM_CD)),
+                                                      C.byref(depth_camera.c), C.byref(mask_camera.c), C.byref(self._p),
+                                                      1 if overlay else 0))
+
+    def split_depth(self, depth, mask, T_CM_CD, depth_camera, mask_camera, overlay=False):
+        """splitImageOnGPU(depth, mask, T_CM_CD, depth_camera, mask_camera, ...): host arrays in, host arrays out ->
+        (background, foreground) float32, plus the (rows, cols, 3) uint8 overlay when `overlay`."""
+        d = np.ascontiguousarray(depth, dtype=np.float32)
+        mk = np.ascontiguousarray(mask, dtype=np.uint8)
+        if d.ndim != 2 or mk.ndim != 2:
+            raise ValueError("depth and mask must be (rows, cols) images")
+        self._split(d.ctypes.data, d.shape[0], d.shape[1], mk.ctypes.data, mk.shape[0], mk.shape[1], _lib.NVB_MEM_HOST,
+                    T_CM_CD, depth_camera, mask_camera, overlay)
+        out = (self.output(_lib.NVB_SPLIT_BACKGROUND), self.output(_lib.NVB_SPLIT_FOREGROUND))
+        return out + (self.output(_lib.NVB_SPLIT_OVERLAY),) if overlay else out
+
+    def split_depth_device(self, depth_ptr, depth_rows, depth_cols, mask_ptr, mask_rows, mask_cols, T_CM_CD, depth_camera,
+                           mask_camera, overlay=False):
+        """The same on raw device pointers, enqueued on mapper.cuda_stream() without synchronising -> device_buffers()."""
+        self._split(depth_ptr, depth_rows, depth_cols, mask_ptr, mask_rows, mask_cols, _lib.NVB_MEM_DEVICE, T_CM_CD,
+                    depth_camera, mask_camera, overlay)
+        return self.device_buffers()
+
+    def output(self, which):
+        """One output of the last split (NVB_SPLIT_BACKGROUND / _FOREGROUND / _OVERLAY) as a host array."""
+        rows, cols = C.c_int32(0), C.c_int32(0)
+        fn = self._m._L.nvb_mapper_split_output
+        check(fn(self._m._h, int(which), None, _lib.NVB_MEM_HOST, C.byref(rows), C.byref(cols)))
+        if which == _lib.NVB_SPLIT_OVERLAY:
+            out = np.zeros((rows.value, cols.value, 3), np.uint8)
+        else:
+            out = np.zeros((rows.value, cols.value), np.float32)
+        if out.size:
+            check(fn(self._m._h, int(which), out.ctypes.data, _lib.NVB_MEM_HOST, C.byref(rows), C.byref(cols)))
+        return out
+
+    def device_buffers(self):
+        """The last split's device buffers (raw pointers; overlay None when it made none), valid until the next split."""
+        b = _lib.NvbSplitBuffers()
+        check(self._m._L.nvb_mapper_split_device_buffers(self._m._h, C.byref(b)))
+        return {k: getattr(b, k) for k, _ in b._fields_}
+
+    def split_color(self, rgb, mask, overlay=False):
+        """splitImageOnGPU(color, mask, ...): (rows, cols, 3) uint8 and a (rows, cols) mask on top of it -> (unmasked,
+        masked), plus the overlay when `overlay`."""
+        c = np.ascontiguousarray(rgb, dtype=np.uint8)
+        mk = np.ascontiguousarray(mask, dtype=np.uint8)
+        if c.ndim != 3 or c.shape[2] != 3 or mk.shape != c.shape[:2]:
+            raise ValueError("rgb must be (rows, cols, 3) and mask (rows, cols)")
+        outs = [np.empty_like(c) for _ in range(3 if overlay else 2)]
+        check(self._m._L.nvb_mapper_split_color_image(self._m._h, c.ctypes.data, mk.ctypes.data, _lib.NVB_MEM_HOST,
+                                                      c.shape[0], c.shape[1], outs[0].ctypes.data, outs[1].ctypes.data,
+                                                      outs[2].ctypes.data if overlay else None))
+        return tuple(outs)
+
+    def split_color_device(self, rgb_ptr, mask_ptr, rows, cols, unmasked_ptr, masked_ptr, overlay_ptr=None):
+        """The same on raw device pointers, enqueued on mapper.cuda_stream() without synchronising."""
+        check(self._m._L.nvb_mapper_split_color_image(self._m._h, rgb_ptr, mask_ptr, _lib.NVB_MEM_DEVICE, int(rows),
+                                                      int(cols), unmasked_ptr, masked_ptr, overlay_ptr))
+
+
 _filter_mappers = {}
 
 
