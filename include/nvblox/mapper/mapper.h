@@ -18,6 +18,8 @@
 #include "nvblox/integrators/weighting_function.h"
 #include "nvblox/geometry/plane.h"
 #include "nvblox/integrators/shape_clearer.h"
+#include "nvblox/io/mesh_io.h"
+#include "nvblox/io/pointcloud_io.h"
 #include "nvblox/map/layer.h"
 #include "nvblox/mesh/mesh_integrator.h"
 #include "nvblox/sensors/camera.h"
@@ -337,6 +339,13 @@ class Mapper {
                                                                                                   : -1;
     b200_detail::check(nvb_mapper_create(&o, &m_), "Mapper", nvb_last_error());
   }
+  // Mapper(map_filepath, block_memory_pool_params, cuda_stream) -- mapper/mapper.h:128-134: a TSDF mapper holding the map of
+  // the file (loadMap; a file that cannot be loaded leaves the mapper empty, as in the reference).
+  Mapper(const std::string& map_filepath, BlockMemoryPoolParams block_memory_pool_params = BlockMemoryPoolParams(),
+         std::shared_ptr<CudaStream> cuda_stream = std::make_shared<CudaStreamOwning>())
+      : Mapper(0.05f, block_memory_pool_params, ProjectiveLayerType::kTsdf, std::move(cuda_stream)) {
+    loadMap(map_filepath, block_memory_pool_params);
+  }
   ~Mapper() { nvb_mapper_destroy(m_); }
   Mapper(const Mapper&) = delete;
   Mapper& operator=(const Mapper&) = delete;
@@ -466,6 +475,23 @@ class Mapper {
                        nvb_last_error());
   }
   void clear() { b200_detail::check(nvb_mapper_clear(m_), "clear", nvb_last_error()); }
+  // Mapper::saveLayerCake / loadMap (mapper.h:662-671, mapper.cpp:636-687): the map in the reference's .nvblx file. loadMap
+  // takes the voxel size from the file and returns false (the map unchanged) on a file it cannot load; nvb_last_error()
+  // says why. Tables this mapper cannot hold are skipped (nvb_mapper_load_map).
+  bool saveLayerCake(const std::string& filename) const { return nvb_mapper_save_map(m_, filename.c_str()) == NVB_OK; }
+  bool saveLayerCake(const char* filename) const { return saveLayerCake(std::string(filename)); }
+  bool loadMap(const std::string& filename, const BlockMemoryPoolParams = BlockMemoryPoolParams()) {
+    return nvb_mapper_load_map(m_, filename.c_str(), nullptr) == NVB_OK;
+  }
+  bool loadMap(const char* filename, BlockMemoryPoolParams block_memory_pool_params = BlockMemoryPoolParams()) {
+    return loadMap(std::string(filename), block_memory_pool_params);
+  }
+  // Mapper::save*AsPly (mapper.h:676-697)
+  bool saveColorMeshAsPly(const std::string& filename) const { return io::outputColorMeshLayerToPly(color_mesh_layer(), filename); }
+  bool saveEsdfAsPly(const std::string& filename) const { return io::outputVoxelLayerToPly(esdf_layer(), filename); }
+  bool saveTsdfAsPly(const std::string& filename) const { return io::outputVoxelLayerToPly(tsdf_layer(), filename); }
+  bool saveFreespaceAsPly(const std::string& filename) const { return io::outputVoxelLayerToPly(freespace_layer(), filename); }
+  bool saveOccupancyAsPly(const std::string& filename) const { return io::outputVoxelLayerToPly(occupancy_layer(), filename); }
   // Mapper::updateFreespace(update_time_ms, T_L_C, camera, depth_frame, update_full_layer) (mapper.h:196-214)
   void updateFreespace(Time update_time_ms, const Transform& T_L_C, const Camera& camera,
                        const DepthImageConstView& depth_frame, UpdateFullLayer full = UpdateFullLayer::kNo) {

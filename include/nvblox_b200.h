@@ -53,7 +53,8 @@ typedef enum {
   NVB_ERR_CUDA = -2,
   NVB_ERR_CAPACITY = -3,      /* a slab / hash could not be grown */
   NVB_ERR_INDEX_RANGE = -4,   /* a block index does not fit the 21-bit hash key */
-  NVB_ERR_NO_DEVICE = -5
+  NVB_ERR_NO_DEVICE = -5,
+  NVB_ERR_IO = -6             /* a map file could not be opened, read or written, or libsqlite3.so.0 is missing */
 } NvbStatus;
 
 /* Where a caller buffer lives. */
@@ -722,6 +723,39 @@ NVB_API int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t*
 NVB_API int32_t nvb_layer_block_device_ptr(NvbMapper* m, int32_t layer, const int32_t xyz[3],
                                            void** out_ptr);
 NVB_API int32_t nvb_layer_block_bytes(int32_t layer);
+
+/* Map files: Mapper::saveLayerCake / Mapper::loadMap (src/mapper/mapper.cpp:636-687) in the reference's .nvblx format, an
+ * SQLite database with the tables <layer>_metadata (rows 'type' and 'block_size') and <layer>_data (one row of index_x,
+ * index_y, index_z and the block's voxels[8][8][8], byte for byte, per block) for tsdf_layer, esdf_layer, occupancy_layer,
+ * freespace_layer, color_layer and feature_layer. SQLite is loaded from libsqlite3.so.0 on first use; without it both calls
+ * fail with NVB_ERR_IO, which also stands for a file that cannot be opened, read or written (the reference logs and
+ * returns false).
+ *
+ * Save joins the mapper's streams and truncates `path`. All six tables are written, one transaction per layer; a layer
+ * this mapper does not hold (the other projective layer, freespace without NVB_PROJECTIVE_TSDF_WITH_FREESPACE, colour
+ * before its first use, features always) is an empty table with the block size. Rows go in (x, y, z) block-index order,
+ * so two saves of equal maps hold the same rows whatever the allocation history (the reference's order is its hash's). */
+NVB_API int32_t nvb_mapper_save_map(NvbMapper* m, const char* path);
+/* Load replaces the map with the file's: the projective layer this mapper holds (tsdf_layer or occupancy_layer), the
+ * ESDF, colour (TSDF mappers) and freespace (NVB_PROJECTIVE_TSDF_WITH_FREESPACE). Other tables, feature_layer always,
+ * are skipped, and the call still succeeds: loaded_blocks (optional, by NvbLayer id 0-4, then [5] the feature layer)
+ * reports the blocks loaded per layer, 0 for a skipped table. The voxel size becomes the file's block_size / 8; when it
+ * changes, the cached viewpoint of the projective integrator is dropped. Every consumer's next update covers every block
+ * (a fresh BlocksToUpdateTracker); a TSDF mapper ends with a full colour-mesh update. The freespace integrator's last
+ * update time, the last integrated view and the cleared-block set are kept. The file is validated before the map is
+ * touched, and a failed load leaves the map as it was:
+ *  - NVB_ERR_IO: no file, not a map file, no tsdf_layer table, a layer without block_size, block sizes that differ, a
+ *    blob of other than nvb_layer_block_bytes(layer) bytes, or an index twice;
+ *  - NVB_ERR_INDEX_RANGE: an index outside +-2^20;
+ *  - NVB_ERR_CAPACITY: a layer beyond 2^28 blocks. */
+NVB_API int32_t nvb_mapper_load_map(NvbMapper* m, const char* path, int32_t loaded_blocks[6]);
+/* io::outputVoxelLayerToPly's points (io/pointcloud_io.cpp:23-73) of NVB_LAYER_TSDF (weight > 1e-4, intensity distance),
+ * NVB_LAYER_OCCUPANCY (p = probabilityFromLogOdds(log_odds) > 0.5, intensity p), NVB_LAYER_FREESPACE (every voxel,
+ * intensity is_high_confidence_freespace) or NVB_LAYER_ESDF (observed, intensity voxel_size * sqrt(squared_distance_vox),
+ * negative inside): 4 floats {x, y, z, intensity} per point at the voxel centre, into xyzi (host or device memory). The
+ * order is canonical: blocks in (x, y, z) block-index order, then voxels in x, y, z order (the reference follows its
+ * hash). *n = the number of points; with cap < *n nothing is written. */
+NVB_API int32_t nvb_layer_export_points(NvbMapper* m, int32_t layer, int32_t memory, float* xyzi, int64_t cap, int64_t* n);
 
 /* ---- Point queries: the map read at arbitrary points on the GPU. A query reads the map and never writes it.
  * Points are n x 3 floats (x, y, z); spheres n x 4 floats (x, y, z, radius). A point's voxel is the one

@@ -11,6 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libnvblox_b200.so")
 
 NVB_OK = 0
+NVB_ERR_INDEX_RANGE, NVB_ERR_IO = -4, -6
 NVB_MEM_HOST, NVB_MEM_DEVICE = 0, 1
 NVB_LAYER_TSDF, NVB_LAYER_ESDF, NVB_LAYER_OCCUPANCY, NVB_LAYER_FREESPACE, NVB_LAYER_COLOR, NVB_LAYER_MESH = 0, 1, 2, 3, 4, 5
 NVB_PROJECTIVE_TSDF, NVB_PROJECTIVE_OCCUPANCY, NVB_PROJECTIVE_TSDF_WITH_FREESPACE = 0, 1, 2
@@ -53,6 +54,7 @@ EXPORTED_SYMBOLS = [
     "nvb_default_image_masker_params", "nvb_mapper_split_depth_image", "nvb_mapper_split_output",
     "nvb_mapper_split_device_buffers", "nvb_mapper_split_color_image",
     "nvb_layer_query_voxels", "nvb_layer_interpolate", "nvb_query_esdf", "nvb_query_tsdf", "nvb_query_occupancy",
+    "nvb_mapper_save_map", "nvb_mapper_load_map", "nvb_layer_export_points",
 ]
 
 
@@ -271,6 +273,9 @@ def load(path=None):
     L.nvb_layer_set_blocks.argtypes = [vp, i32, ip, i32, vp]
     L.nvb_layer_block_device_ptr.argtypes = [vp, i32, ip, C.POINTER(vp)]
     L.nvb_layer_block_bytes.argtypes = [i32]
+    L.nvb_mapper_save_map.argtypes = [vp, C.c_char_p]
+    L.nvb_mapper_load_map.argtypes = [vp, C.c_char_p, ip]
+    L.nvb_layer_export_points.argtypes = [vp, i32, i32, vp, C.c_int64, C.POINTER(C.c_int64)]
     L.nvb_mapper_last_esdf_stats.argtypes = [vp, C.POINTER(C.c_int64)]
     L.nvb_mapper_set_cache_last_viewpoint.argtypes = [vp, C.c_int32]
     L.nvb_mapper_get_cache_last_viewpoint.argtypes = [vp]

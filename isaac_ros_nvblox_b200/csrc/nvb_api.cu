@@ -1359,9 +1359,10 @@ void nvb_mapper_destroy(NvbMapper* m) {
   delete m;  // the device buffers free themselves
 }
 
-int32_t nvb_mapper_clear(NvbMapper* m) {
-  if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
-  NVB_CUDA(cudaSetDevice(m->device));
+// Empties the layers and the state derived from their blocks: the slabs and hashes, the tracker (every consumer's next
+// update covers every block), the ESDF scratch, the neighbour tables, the mesh arena and the fill-level bounds.
+// nvb_mapper_clear and nvb_mapper_load_map both start from here.
+static int resetLayers(NvbMapper* m) {
   NVB_CUDA(syncAll(m));
   std::vector<DevLayer*> layers = {&m->tsdf, &m->esdf};
   if (m->freespace.blocks) layers.push_back(&m->freespace);
@@ -1395,13 +1396,21 @@ int32_t nvb_mapper_clear(NvbMapper* m) {
     launchFillU64(m->mesh.hash.keys, kEmptyKey, (size_t)m->mesh.hash.mask + 1, m->stream);
     NVB_CUDA(cudaMemsetAsync(m->mesh_state.get(), 0, kArenaInts * sizeof(int), m->stream));
   }
-  m->esdf_mode = 0;
-  m->fs_last_update_ms = 0;
-  m->has_last_view = false;
   m->tsdf_count_ub = 0, m->tsdf_count_confirmed = 0, m->esdf_extra_ub = 0;
   m->cells_cum = 0, m->confirmed_cum = 0;
   for (int k = 0; k < kCountRing; k++) m->count_pending[k] = false;
   NVB_CUDA(syncAll(m));
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_clear(NvbMapper* m) {
+  if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
+  NVB_CUDA(cudaSetDevice(m->device));
+  const int rc = resetLayers(m);
+  if (rc) return rc;
+  m->esdf_mode = 0;
+  m->fs_last_update_ms = 0;
+  m->has_last_view = false;
   return NVB_OK;
 }
 
@@ -3188,6 +3197,162 @@ int32_t nvb_layer_block_device_ptr(NvbMapper* m, int32_t layer, const int32_t xy
     if (k == kEmptyKey) return NVB_OK;
     p = (p + 1) & L->hash.mask;
   }
+  return NVB_OK;
+}
+
+// The layer a map file's table k (NvbLayer id, kMapFileLayers) is saved from, or null when the mapper does not hold it.
+// Unlike layerOf, a colour layer is not created for this.
+static DevLayer* savedLayerOf(NvbMapper* m, int k) {
+  if (k == NVB_LAYER_TSDF) return m->projective_layer_type != NVB_PROJECTIVE_OCCUPANCY ? &m->tsdf : nullptr;
+  if (k == NVB_LAYER_OCCUPANCY) return m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY ? &m->tsdf : nullptr;
+  if (k == NVB_LAYER_ESDF) return &m->esdf;
+  if (k == NVB_LAYER_FREESPACE) return m->freespace.blocks ? &m->freespace : nullptr;
+  if (k == NVB_LAYER_COLOR) return m->color.blocks ? &m->color : nullptr;
+  return nullptr;  // the feature layer
+}
+
+int32_t nvb_mapper_save_map(NvbMapper* m, const char* path) {
+  if (!m || !path) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  NVB_CUDA(cudaSetDevice(m->device));
+  NVB_CUDA(syncAll(m));
+  std::vector<int> xyz[kMapFileLayers], order[kMapFileLayers];
+  std::vector<unsigned char> voxels[kMapFileLayers];
+  MapFileLayerOut out[kMapFileLayers] = {};
+  for (int k = 0; k < kMapFileLayers; k++) {
+    const DevLayer* L = savedLayerOf(m, k);
+    if (!L) continue;
+    // the slab below the high-water mark in one copy each, dead slots skipped, rows in (x, y, z) order
+    int hw = 0;
+    NVB_CUDA(cudaMemcpy(&hw, L->count, sizeof(int), cudaMemcpyDeviceToHost));
+    hw = std::min(hw, L->capacity);
+    xyz[k].resize(3 * (size_t)hw);
+    voxels[k].resize((size_t)hw * L->block_bytes);
+    NVB_CUDA(cudaMemcpy(xyz[k].data(), L->block_index, xyz[k].size() * sizeof(int), cudaMemcpyDeviceToHost));
+    NVB_CUDA(cudaMemcpy(voxels[k].data(), L->blocks, voxels[k].size(), cudaMemcpyDeviceToHost));
+    const int* b = xyz[k].data();
+    for (int sl = 0; sl < hw; sl++)
+      if (b[3 * sl] != kDeadSlotX) order[k].push_back(sl);
+    std::sort(order[k].begin(), order[k].end(), [b](int i, int j) {
+      return std::lexicographical_compare(b + 3 * i, b + 3 * i + 3, b + 3 * j, b + 3 * j + 3);
+    });
+    out[k] = {b, voxels[k].data(), order[k].data(), (int)order[k].size(), L->block_bytes};
+  }
+  std::string err;
+  const int rc = writeMapFile(path, out, m->block_size, &err);
+  return rc ? fail(rc, "saving " + std::string(path) + ": " + err) : NVB_OK;
+}
+
+// Slots [0, n) of the emptied layer L get the file's blocks in order: one copy of the voxels, one of the indices, the fill
+// level and the hash.
+static int uploadLoadedLayer(NvbMapper* m, DevLayer* L, const MapFileLayerIn& in) {
+  if (in.n == 0) return NVB_OK;
+  NVB_CUDA(cudaMemcpyAsync(L->blocks, in.voxels.get(), (size_t)in.n * L->block_bytes, cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(L->block_index, in.xyz.data(), in.xyz.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(L->count, &in.n, sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  launchRehash(*L, in.n, m->stream);
+  m->launches++;
+  return NVB_OK;
+}
+
+int32_t nvb_mapper_load_map(NvbMapper* m, const char* path, int32_t loaded_blocks[6]) {
+  if (!m || !path) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  NVB_CUDA(cudaSetDevice(m->device));
+  const bool occupancy = m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY;
+  const int proj = occupancy ? NVB_LAYER_OCCUPANCY : NVB_LAYER_TSDF;
+  bool want[kMapFileLayers] = {};
+  want[proj] = want[NVB_LAYER_ESDF] = true;
+  want[NVB_LAYER_COLOR] = !occupancy;
+  want[NVB_LAYER_FREESPACE] = m->projective_layer_type == NVB_PROJECTIVE_TSDF_WITH_FREESPACE;
+  MapFileLayerIn in[kMapFileLayers];
+  std::string err;
+  int rc = readMapFile(path, want, in, &err);
+  if (rc) return fail(rc, "loading " + std::string(path) + ": " + err);
+  // the slabs' growth, checked before the map changes (colour and freespace follow the projective slab)
+  const int n_proj = in[proj].n, n_esdf = in[NVB_LAYER_ESDF].n;
+  const long long need_t = std::max({n_proj, in[NVB_LAYER_COLOR].n, in[NVB_LAYER_FREESPACE].n});
+  long long cap_t = m->tsdf.capacity, cap_e = m->esdf.capacity;
+  while (cap_t < need_t) cap_t *= 2;
+  while (cap_e < n_esdf) cap_e *= 2;
+  if (cap_t > (1ll << 28) || cap_e > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "the map would exceed 2^28 blocks");
+
+  // Mapper::loadMap: the file's voxel size, a new cake and a fresh tracker (mapper.cpp:661-671)
+  if ((rc = resetLayers(m))) return rc;
+  const float voxel_size = in[NVB_LAYER_TSDF].block_size / (float)kVps;
+  if (voxel_size != m->voxel_size) {
+    m->voxel_size = voxel_size;
+    m->block_size = voxel_size * (float)kVps;
+    m->vc_n = 0;  // the cached views are sets of blocks of the old size
+  }
+  if ((rc = ensureTsdfCapacity(m, need_t))) return rc;
+  if ((rc = ensureEsdfCapacity(m, n_esdf))) return rc;
+  if (m->freespace.blocks && m->freespace.capacity < m->tsdf.capacity && (rc = growLayer(m, &m->freespace, m->tsdf.capacity)))
+    return rc;
+  if (in[NVB_LAYER_COLOR].n > 0 && (rc = ensureColorLayer(m))) return rc;
+  for (int k = 0; k < kMapFileLayers; k++) {
+    DevLayer* L = want[k] ? savedLayerOf(m, k) : nullptr;
+    if (L && (rc = uploadLoadedLayer(m, L, in[k]))) return rc;
+  }
+  // the clear pass's parent boxes of the loaded ESDF blocks: pruning stays exact
+  launchEsdfParentBoxes(m->esdf, n_esdf, m->psum.get(), m->stream);
+  m->launches++;
+  // the fill-level bounds from the real counts (tightenEsdfBound)
+  m->tsdf_count_ub = m->tsdf_count_confirmed = n_proj;
+  m->confirmed_cum = m->cells_cum;
+  m->esdf_extra_ub = std::max(0, n_esdf - n_proj);
+  NVB_CUDA(syncAll(m));
+  if ((rc = checkDeviceError(m))) return rc;
+  // a new colour mesh layer and a full mesh update (mapper.cpp:673-678)
+  if (!occupancy && (rc = nvb_mapper_update_mesh(m, 1))) return rc;
+  if (loaded_blocks)
+    for (int k = 0; k < kMapFileLayers; k++) loaded_blocks[k] = want[k] ? in[k].n : 0;
+  return NVB_OK;
+}
+
+int32_t nvb_layer_export_points(NvbMapper* m, int32_t layer, int32_t memory, float* xyzi, int64_t cap, int64_t* n) {
+  if (!m || !n) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (layer != NVB_LAYER_TSDF && layer != NVB_LAYER_OCCUPANCY && layer != NVB_LAYER_FREESPACE && layer != NVB_LAYER_ESDF)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "points are exported from a TSDF, occupancy, freespace or ESDF layer");
+  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "unknown memory kind");
+  DevLayer* L = layerOf(m, layer);
+  if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper does not hold that layer");
+  NVB_CUDA(cudaSetDevice(m->device));
+  NVB_CUDA(syncAll(m));
+  int hw = 0;
+  NVB_CUDA(cudaMemcpy(&hw, L->count, sizeof(int), cudaMemcpyDeviceToHost));
+  hw = std::min(hw, L->capacity);
+  *n = 0;
+  if (hw == 0) return NVB_OK;
+  if ((long long)hw * kVpb > 0x7fffffffll) return fail(NVB_ERR_CAPACITY, "more than 2^31 voxels to export");
+  DeviceArray<unsigned long long> keys;
+  DeviceArray<int> slots, totals;
+  DeviceArray<int2> counts;
+  DeviceArray<unsigned char> temp;
+  const size_t temp_bytes = groundSortTempBytes(hw);
+  NVB_CUDA(keys.grow(m, 2 * (size_t)hw, 2 * (size_t)hw));
+  NVB_CUDA(slots.grow(m, 2 * (size_t)hw, 2 * (size_t)hw));
+  NVB_CUDA(counts.grow(m, hw, hw));
+  NVB_CUDA(totals.grow(m, 2, 2));
+  NVB_CUDA(temp.grow(m, std::max<size_t>(temp_bytes, 1), std::max<size_t>(temp_bytes, 1)));
+  NVB_CUDA(launchGroundSortBlocks(*L, hw, keys.get(), slots.get(), temp.get(), temp_bytes, m->stream));
+  ExportPointsArgs a{};
+  a.layer = *L, a.layer_id = layer, a.slots = slots.get() + hw, a.num_blocks = hw;
+  a.counts = counts.get(), a.totals = totals.get();
+  a.block_size = m->block_size, a.voxel_size = m->voxel_size;
+  launchExportCount(a, m->stream);
+  m->launches += 3;
+  int total = 0;
+  NVB_CUDA(cudaMemcpyAsync(&total, a.totals, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  *n = total;
+  if (!xyzi || cap < total || total == 0) return NVB_OK;
+  DeviceArray<float4> staged;
+  if (memory == NVB_MEM_HOST) NVB_CUDA(staged.grow(m, total, total));
+  a.out = memory == NVB_MEM_HOST ? staged.get() : reinterpret_cast<float4*>(xyzi);
+  launchExportEmit(a, m->stream);
+  m->launches++;
+  if (memory == NVB_MEM_HOST)
+    NVB_CUDA(cudaMemcpyAsync(xyzi, staged.get(), (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
   return NVB_OK;
 }
 

@@ -385,16 +385,7 @@ __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer
   if (psum_slot) {
     lo0 = __reduce_min_sync(0xffffffffu, lo0), lo1 = __reduce_min_sync(0xffffffffu, lo1), lo2 = __reduce_min_sync(0xffffffffu, lo2);
     hi0 = __reduce_max_sync(0xffffffffu, hi0), hi1 = __reduce_max_sync(0xffffffffu, hi1), hi2 = __reduce_max_sync(0xffffffffu, hi2);
-    if ((lane64 & 31) == 0) {
-      unsigned int v = 0u;
-      if (lo0 <= hi0) {
-        const bool fits = lo0 >= -16 && lo1 >= -16 && lo2 >= -16 && hi0 <= 15 && hi1 <= 15 && hi2 <= 15;
-        v = fits ? ((1u << 31) | (unsigned)(lo0 + 16) | ((unsigned)(hi0 + 16) << 5) | ((unsigned)(lo1 + 16) << 10) |
-                    ((unsigned)(hi1 + 16) << 15) | ((unsigned)(lo2 + 16) << 20) | ((unsigned)(hi2 + 16) << 25))
-                 : 0xffffffffu;
-      }
-      psum_slot[lane64 >> 5] = v;
-    }
+    if ((lane64 & 31) == 0) psum_slot[lane64 >> 5] = parentBoxWord(lo0, hi0, lo1, hi1, lo2, hi2);
   }
 }
 

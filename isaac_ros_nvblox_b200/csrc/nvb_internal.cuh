@@ -7,6 +7,9 @@
 // nvblox_core/cmake/nvblox_targets.cmake:120-171 -- see DESIGN.md "Numerics").
 #pragma once
 #include <cstdint>
+#include <memory>
+#include <string>
+#include <vector>
 
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -460,6 +463,17 @@ int esdfWaveXSplitMinK();  // kSplitMinK, or NVB_WAVEX_SPLIT_MIN_K (read at mapp
 cudaError_t runEsdfComputeHostLoop(const EsdfCtx& c, int num_sms, cudaStream_t stream, int* launches);
 int esdfPersistentMaxCtas(int num_sms);
 
+// The clear pass's parent-box word of half an ESDF block (EsdfCtx::psum) from the bounds of the block offsets its voxels'
+// parents point into: 0 without parents, the six bounds + 16 in 5 bits each under bit 31, or 0xffffffff when a bound
+// leaves [-16, 15].
+__host__ __device__ __forceinline__ unsigned int parentBoxWord(int lo0, int hi0, int lo1, int hi1, int lo2, int hi2) {
+  if (lo0 > hi0) return 0u;
+  const bool fits = lo0 >= -16 && lo1 >= -16 && lo2 >= -16 && hi0 <= 15 && hi1 <= 15 && hi2 <= 15;
+  return fits ? ((1u << 31) | (unsigned)(lo0 + 16) | ((unsigned)(hi0 + 16) << 5) | ((unsigned)(lo1 + 16) << 10) |
+                 ((unsigned)(hi1 + 16) << 15) | ((unsigned)(lo2 + 16) << 20) | ((unsigned)(hi2 + 16) << 25))
+              : 0xffffffffu;
+}
+
 constexpr int kFreespaceVoxelBytes = 24;
 constexpr int kFreespaceBlockBytes = 512 * kFreespaceVoxelBytes;  // 12 288
 #ifdef __CUDACC__
@@ -751,5 +765,47 @@ void launchQueryTsdf(const QueryLayers& q, bool multi, const float* xyz, long lo
                      cudaStream_t stream);
 void launchQueryOccupancy(const QueryLayers& q, bool multi, float initial_log_odds, const float* xyz, long long n, float* out,
                           int num_sms, cudaStream_t stream);
+
+// nvb_map_io.cu: map files (the reference's .nvblx SQLite layer cake) and the voxel-layer point export
+constexpr int kMapFileLayers = 6;  // tables by NvbLayer id: tsdf, esdf, occupancy, freespace, color, then feature_layer
+const char* mapFileTableName(int k);
+// One layer to write: the blocks of slab slots order[0, n), xyz (3 ints) and voxels (block_bytes) indexed by slot.
+struct MapFileLayerOut {
+  const int* xyz;
+  const unsigned char* voxels;
+  const int* order;
+  int n;
+  int block_bytes;
+};
+struct PinnedFree {
+  void operator()(unsigned char* p) const { cudaFreeHost(p); }
+};
+// One layer read: present = the file has its tables; n blocks in (x, y, z) order, their voxels in pinned memory.
+struct MapFileLayerIn {
+  bool present = false;
+  float block_size = 0.0f;
+  int n = 0;
+  std::vector<int> xyz;
+  std::unique_ptr<unsigned char, PinnedFree> voxels;
+};
+// Truncates `path` and writes the six layers' tables, one transaction per layer. NVB_OK or NVB_ERR_IO (*err says why).
+int writeMapFile(const char* path, const MapFileLayerOut layers[kMapFileLayers], float block_size, std::string* err);
+// Reads and validates `path`: every present layer has a positive block_size and they agree, tsdf_layer is present, and the
+// tables with want[k] hold unique in-range indices with blobs of nvb_layer_block_bytes(k). Only those are read.
+int readMapFile(const char* path, const bool want[kMapFileLayers], MapFileLayerIn in[kMapFileLayers], std::string* err);
+// psum words of ESDF slots [0, n) from their voxels
+void launchEsdfParentBoxes(const DevLayer& esdf, int n, unsigned int* psum, cudaStream_t stream);
+struct ExportPointsArgs {
+  DevLayer layer;
+  int layer_id;       // NVB_LAYER_TSDF, _OCCUPANCY, _FREESPACE or _ESDF
+  const int* slots;   // num_blocks slots in (x, y, z) block-index order, free slots (-1) last
+  int num_blocks;
+  int2* counts;       // per listed block: kept voxels, then their exclusive prefix sums
+  int* totals;        // 2 ints: all kept voxels, 0
+  float4* out;        // {x, y, z, intensity} per kept voxel
+  float block_size, voxel_size;
+};
+void launchExportCount(const ExportPointsArgs& a, cudaStream_t stream);  // counts + scan + totals
+void launchExportEmit(const ExportPointsArgs& a, cudaStream_t stream);
 
 }  // namespace nvb

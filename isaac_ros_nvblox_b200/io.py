@@ -71,6 +71,20 @@ def output_color_mesh_layer_to_ply(mesh_layer, filename):
     return output_mesh_to_ply(get_mesh(mesh_layer), filename)
 
 
+def output_points_to_ply(points, intensities, filename):
+    """io::outputPointsToPly (pointcloud_io.cpp) through PlyWriter: `x y z intensity` per point under `property float
+    intensity`, no faces. False (and no file) without points, like the reference."""
+    p = np.asarray(points, np.float32).reshape(-1, 3)
+    t = np.asarray(intensities, np.float32).reshape(-1)
+    if len(p) == 0 or len(t) != len(p):
+        return False
+    with open(filename, "w") as f:
+        f.write("ply\nformat ascii 1.0\nelement vertex %d\nproperty float x\nproperty float y\nproperty float z\n"
+                "property float intensity\nend_header\n" % len(p))
+        f.write("".join("%s %s %s %s\n" % (_fmt(a), _fmt(b), _fmt(c), _fmt(i)) for (a, b, c), i in zip(p, t)))
+    return True
+
+
 def read_ply(filename):
     """Minimal reader of the files written above (for the tests): -> (header property names, (v, k) float array, (f, 3) int array)."""
     with open(filename) as f:
@@ -78,7 +92,8 @@ def read_ply(filename):
     assert lines[0] == "ply" and lines[1] == "format ascii 1.0"
     end = lines.index("end_header")
     nv = int([l for l in lines[:end] if l.startswith("element vertex")][0].split()[-1])
-    nf = int([l for l in lines[:end] if l.startswith("element face")][0].split()[-1])
+    faces = [l for l in lines[:end] if l.startswith("element face")]
+    nf = int(faces[0].split()[-1]) if faces else 0
     props = [l.split()[-1] for l in lines[:end] if l.startswith("property") and "list" not in l]
     body = lines[end + 1:]
     verts = np.array([[float(x) for x in l.split()] for l in body[:nv]], np.float64).reshape(nv, len(props))

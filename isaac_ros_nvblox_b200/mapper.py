@@ -14,10 +14,12 @@ Everything forwards to the C-ABI in libnvblox_b200.so through ctypes; numpy arra
 are host buffers, integers are raw device pointers.
 """
 import ctypes as C
+import os
 
 import numpy as np
 
 from . import _lib
+from . import io as _io
 from ._lib import (NvbBoundingShape, NvbCamera, NvbDecayExclusion, NvbEsdfParams, NvbEsdfSliceParams, NvbFreespaceParams, NvbGroundPlaneParams, NvbMapperOptions, NvbOccupancyDecayParams,
                    NvbOccupancyParams, NvbTsdfDecayParams, NvbTsdfParams, check)
 
@@ -180,6 +182,16 @@ class _Layer:
             return {}
         v, _ = self.get_blocks(idx)
         return {tuple(int(c) for c in k): v[i] for i, k in enumerate(idx)}
+
+    def export_points(self):
+        """io::outputVoxelLayerToPly's points (io/pointcloud_io.cpp:23-73) of a TSDF, occupancy, freespace or ESDF layer:
+        (n, 4) float32 {x, y, z, intensity} at the kept voxels' centres, blocks in (x, y, z) order, then voxels in x, y, z
+        order."""
+        n = C.c_int64(0)
+        check(self._m._L.nvb_layer_export_points(self._m._h, self._id, _lib.NVB_MEM_HOST, None, 0, C.byref(n)))
+        out = np.zeros((max(n.value, 1), 4), dtype=np.float32)
+        check(self._m._L.nvb_layer_export_points(self._m._h, self._id, _lib.NVB_MEM_HOST, out.ctypes.data, n.value, C.byref(n)))
+        return out[:n.value]
 
     def get_voxels(self, points):
         """VoxelBlockLayer::getVoxels / getVoxelsGPU (map/layer.h:265-295): the voxel holding each point, as stored, and
@@ -1249,6 +1261,39 @@ class Mapper:
 
     def clear(self):
         check(self._L.nvb_mapper_clear(self._h))
+
+    # --- map files (Mapper::saveLayerCake / loadMap, src/mapper/mapper.cpp:636-687) and voxel PLY export ------------
+    MAP_FILE_LAYERS = ("tsdf", "esdf", "occupancy", "freespace", "color", "feature")
+
+    def save_layer_cake(self, path):
+        """Writes the map to `path` (truncated) in the reference's .nvblx format: all six layers' tables, rows in (x, y, z)
+        block-index order."""
+        check(self._L.nvb_mapper_save_map(self._h, os.fsencode(path)))
+        return True
+
+    def load_map(self, path):
+        """Replaces the map with the one in `path`; the voxel size follows the file. Returns the blocks loaded per layer,
+        {"tsdf", "esdf", "occupancy", "freespace", "color", "feature"}: 0 for a table this mapper cannot hold (skipped)."""
+        out = (C.c_int32 * 6)()
+        check(self._L.nvb_mapper_load_map(self._h, os.fsencode(path), out))
+        return dict(zip(self.MAP_FILE_LAYERS, list(out)))
+
+    def _save_layer_as_ply(self, layer, filename):
+        pts = layer.export_points()
+        return _io.output_points_to_ply(pts[:, :3], pts[:, 3], filename)
+
+    def save_tsdf_as_ply(self, filename):
+        """Mapper::saveTsdfAsPly: io::outputVoxelLayerToPly(tsdf_layer()). False (no file) without points."""
+        return self._save_layer_as_ply(self._tsdf, filename)
+
+    def save_esdf_as_ply(self, filename):
+        return self._save_layer_as_ply(self._esdf, filename)
+
+    def save_occupancy_as_ply(self, filename):
+        return self._save_layer_as_ply(self._occupancy, filename)
+
+    def save_freespace_as_ply(self, filename):
+        return self._save_layer_as_ply(self._freespace, filename)
 
     # --- the hot path ----------------------------------------------------
     @staticmethod
