@@ -2455,6 +2455,17 @@ static int weld_cmp(const void* a, const void* b) {
   return x->idx < y->idx ? -1 : (x->idx > y->idx ? 1 : 0); /* the radix sort is stable */
 }
 
+/* Index3D(v * kValueScale) in weldVerticesCubKernel (mesh_integrator.cu:755-757) converts on the device: cvt.rzi.s32.f32,
+ * which truncates, saturates out-of-range values to INT32_MIN / INT32_MAX and maps NaN to 0 (PTX ISA, cvt). A plain C cast
+ * is undefined there, and x86's cvttss2si gives INT32_MIN for both overflows -- wrong for vertices past +2147483.647 m. */
+static int32_t weld_key_coord(float v) {
+  const float s = v * 1000.0f;
+  if (s != s) return 0;
+  if (s >= 2147483648.0f) return INT32_MAX;
+  if (s < -2147483648.0f) return INT32_MIN;
+  return (int32_t)s;
+}
+
 /* weldVerticesCubKernel<128, 20> (mesh_integrator.cu:691-803). */
 static void mesh_weld(MeshBlock* b) {
   const int n = b->nv;
@@ -2463,7 +2474,7 @@ static void mesh_weld(MeshBlock* b) {
   for (int i = 0; i < n; i++) {
     /* Index3DHash(Index3D(x * 1000, y * 1000, z * 1000)) (core/hash.h:32-40): float products truncated to int, then
      * x + y * 17191 + z * 17191^2 in size_t arithmetic */
-    const int32_t x = (int32_t)(b->v[3 * i] * 1000.0f), y = (int32_t)(b->v[3 * i + 1] * 1000.0f), z = (int32_t)(b->v[3 * i + 2] * 1000.0f);
+    const int32_t x = weld_key_coord(b->v[3 * i]), y = weld_key_coord(b->v[3 * i + 1]), z = weld_key_coord(b->v[3 * i + 2]);
     const uint64_t sl = 17191ull;
     k[i].key = (uint64_t)(int64_t)x + (uint64_t)(int64_t)y * sl + (uint64_t)(int64_t)z * (sl * sl);
     k[i].idx = b->tri[i];

@@ -203,7 +203,7 @@ def test_continuation_after_load_matches_the_oracle(gpu, tmp_path, persistent):
 
 def _bad_file(tmp_path, name, edit):
     p = str(tmp_path / name)
-    shutil.copy(FIXTURE, p)
+    shutil.copyfile(FIXTURE, p)  # contents only: from a read-only checkout, shutil.copy would make the copy read-only too
     db = sqlite3.connect(p)
     edit(db)
     db.commit()
