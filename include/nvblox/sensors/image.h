@@ -53,6 +53,30 @@ using DepthImageConstView = ImageView<float>;
 using MonoImageConstView = ImageView<uint8_t>;
 using ColorImageConstView = ImageView<Color>;
 
+// Writable view (the reference's ImageView<float> / ImageView<Color>, sensors/image.h:326-444) of a buffer the caller owns:
+// rows x cols pixels on the device unless told otherwise; a view of an owning Image is host memory.
+template <typename T>
+class MutableImageView {
+ public:
+  MutableImageView() = default;
+  MutableImageView(int rows, int cols, T* data = nullptr, MemoryType mt = MemoryType::kDevice)
+      : data_(data), rows_(rows), cols_(cols), mt_(mt) {}
+  MutableImageView(Image<T>& img) : data_(img.dataPtr()), rows_(img.rows()), cols_(img.cols()), mt_(MemoryType::kHost) {}
+  T* dataPtr() const { return data_; }
+  const T* dataConstPtr() const { return data_; }
+  int rows() const { return rows_; }
+  int cols() const { return cols_; }
+  int width() const { return cols_; }
+  int height() const { return rows_; }
+  bool on_device() const { return mt_ == MemoryType::kDevice; }
+ private:
+  T* data_ = nullptr;
+  int rows_ = 0, cols_ = 0;
+  MemoryType mt_ = MemoryType::kDevice;
+};
+using DepthImageView = MutableImageView<float>;
+using ColorImageView = MutableImageView<Color>;
+
 class MaskedDepthImageConstView : public DepthImageConstView {
  public:
   MaskedDepthImageConstView(const DepthImageConstView& image, std::optional<MonoImageConstView> mask = std::nullopt,

@@ -330,6 +330,32 @@ NVB_API int32_t nvb_sphere_tracer_render_depth(NvbMapper* m, const float* T_L_C,
                                                float truncation_distance_m, int32_t ray_subsampling_factor,
                                                float* out_depth_host);
 
+/* A standalone SphereTracer's parameters (C/include/nvblox/rays/sphere_tracer.h:204-218); each must be positive
+ * (the setters' CHECK_GTs, C/src/rays/sphere_tracer.cu:319-333). */
+typedef struct {
+  int32_t maximum_steps;              /* 100 */
+  float maximum_ray_length_m;         /* 15.0 */
+  float surface_distance_epsilon_vox; /* 0.1 */
+} NvbSphereTracerParams;
+NVB_API void nvb_default_sphere_tracer_params(NvbSphereTracerParams* p);
+/* SphereTracer::renderImageOnGPU(camera, T_L_C, tsdf_layer, truncation_distance_m, &depth, memory, ray_subsampling_factor)
+ * (C/src/rays/sphere_tracer.cu:134-173, 389-485) of the mapper's TSDF layer: out_depth receives (height / f) * (width / f)
+ * floats, row-major, the depth t * d_C.z of each converged ray and -1 elsewhere. Ray (r, c) goes through the image-plane
+ * point f * (c, r) + f / 2. f must divide the image size; an occupancy mapper has no TSDF layer to trace.
+ * memory = NVB_MEM_DEVICE: the render is enqueued on `stream` (a cudaStream_t; NULL is the default stream) after the work
+ * already there and on the mapper, the stream's next work and the mapper's follow it, and nothing synchronises.
+ * memory = NVB_MEM_HOST: the outputs are staged on the device and written when the call returns. */
+NVB_API int32_t nvb_render_depth(NvbMapper* m, const NvbSphereTracerParams* p, const float* T_L_C, const NvbCamera* cam,
+                                 float truncation_distance_m, int32_t ray_subsampling_factor, int32_t memory, float* out_depth,
+                                 void* stream);
+/* SphereTracer::renderRgbdImageOnGPU (C/src/rays/sphere_tracer.cu:239-300, 487-644): the depth of nvb_render_depth, and in
+ * out_rgb 3 bytes (r, g, b) per ray: the colour of the colour voxel that holds the hit point T_L_C.t + t * d_L, whatever its
+ * weight (an allocated block that was never coloured gives grey 127). A miss, a hit without a colour block, and every hit of
+ * a mapper that never integrated colour, give black. Memory and ordering as nvb_render_depth. */
+NVB_API int32_t nvb_render_rgbd(NvbMapper* m, const NvbSphereTracerParams* p, const float* T_L_C, const NvbCamera* cam,
+                                float truncation_distance_m, int32_t ray_subsampling_factor, int32_t memory, float* out_depth,
+                                uint8_t* out_rgb, void* stream);
+
 /* Mapper::integrateDepth(MaskedDepthImageConstView, T_L_C, Camera)
  * (mapper.h:167-172, mapper_impl.h:28-81) =
  * ProjectiveTsdfIntegrator::integrateFrame (projective_tsdf_integrator.h:48-52)

@@ -55,6 +55,7 @@ EXPORTED_SYMBOLS = [
     "nvb_mapper_split_device_buffers", "nvb_mapper_split_color_image",
     "nvb_layer_query_voxels", "nvb_layer_interpolate", "nvb_query_esdf", "nvb_query_tsdf", "nvb_query_occupancy",
     "nvb_mapper_save_map", "nvb_mapper_load_map", "nvb_layer_export_points",
+    "nvb_default_sphere_tracer_params", "nvb_render_depth", "nvb_render_rgbd",
 ]
 
 
@@ -106,6 +107,11 @@ class NvbColorParams(C.Structure):
                 ("sphere_tracing_ray_subsampling_factor", C.c_int32), ("sphere_tracer_maximum_steps", C.c_int32),
                 ("sphere_tracer_maximum_ray_length_m", C.c_float), ("sphere_tracer_surface_distance_epsilon_vox", C.c_float),
                 ("workspace_bounds_type", C.c_int32), ("workspace_min", C.c_float * 3), ("workspace_max", C.c_float * 3)]
+
+
+class NvbSphereTracerParams(C.Structure):
+    _fields_ = [("maximum_steps", C.c_int32), ("maximum_ray_length_m", C.c_float),
+                ("surface_distance_epsilon_vox", C.c_float)]
 
 
 class NvbFreespaceParams(C.Structure):
@@ -339,6 +345,10 @@ def load(path=None):
     L.nvb_query_esdf.argtypes = [C.POINTER(vp), i32, vp, i64, i32, vp, vp]
     L.nvb_query_tsdf.argtypes = [C.POINTER(vp), i32, vp, i64, vp, vp]
     L.nvb_query_occupancy.argtypes = [C.POINTER(vp), i32, vp, i64, vp, vp]
+    L.nvb_default_sphere_tracer_params.argtypes = [C.POINTER(NvbSphereTracerParams)]
+    L.nvb_default_sphere_tracer_params.restype = None
+    L.nvb_render_depth.argtypes = [vp, C.POINTER(NvbSphereTracerParams), fp, C.POINTER(NvbCamera), f32, i32, i32, vp, vp]
+    L.nvb_render_rgbd.argtypes = [vp, C.POINTER(NvbSphereTracerParams), fp, C.POINTER(NvbCamera), f32, i32, i32, vp, vp, vp]
     L.nvb_mapper_kernel_launches.restype = C.c_int64
     for name in EXPORTED_SYMBOLS:
         f = getattr(L, name)

@@ -3873,3 +3873,80 @@ int32_t nvb_query_occupancy(NvbMapper* const* mappers, int32_t num_mappers, cons
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------
+// SphereTracer renders (nvb_color.cu)
+// ---------------------------------------------------------------------------
+namespace {
+
+// Depth (out_rgb == nullptr) or RGBD. Device outputs are ordered like the point queries (runOrdered on `stream`); host
+// outputs are rendered into temporaries on `stream` and copied back before the call returns.
+int renderImpl(NvbMapper* m, const NvbSphereTracerParams* p, const float* T_L_C, const NvbCamera* cam, float trunc_m, int f,
+               int32_t memory, float* out_depth, uint8_t* out_rgb, void* stream) {
+  if (m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "the sphere tracer needs a TSDF layer");
+  if (p->maximum_steps <= 0 || !(p->maximum_ray_length_m > 0.0f) || !(p->surface_distance_epsilon_vox > 0.0f))
+    return fail(NVB_ERR_INVALID_ARGUMENT, "sphere tracer parameter out of range");  // CHECK_GT, sphere_tracer.cu:319-333
+  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (cam->width <= 0 || cam->height <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "the camera must have a positive size");
+  if (f <= 0 || cam->width % f != 0 || cam->height % f != 0)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "the ray subsampling factor must divide the image size");  // CHECK_EQ, :432-433
+  NVB_CUDA(cudaSetDevice(m->device));
+  RenderArgs a{};
+  a.tsdf = m->tsdf;
+  a.color = m->color;
+  a.T_L_C = rigidFromColMajor(T_L_C);
+  a.cam = *cam;
+  a.block_size = m->block_size;
+  a.voxel_size_inv = voxelSizeInv(m->block_size);
+  a.trunc_m = trunc_m;
+  a.max_steps = p->maximum_steps;
+  a.max_ray_len = p->maximum_ray_length_m;
+  a.eps_m = p->surface_distance_epsilon_vox * m->voxel_size;
+  a.subsample = f;
+  a.drows = cam->height / f, a.dcols = cam->width / f;  // getSubsampledImageSize (:335-339)
+  const size_t n = (size_t)a.drows * a.dcols;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  DeviceArray<float> depth_dev;
+  DeviceArray<unsigned char> rgb_dev;
+  if (memory == NVB_MEM_DEVICE) {
+    a.depth = out_depth, a.rgb = out_rgb;
+  } else {
+    NVB_CUDA(depth_dev.grow(m, n, n));
+    if (out_rgb) NVB_CUDA(rgb_dev.grow(m, 3 * n, 3 * n));
+    a.depth = depth_dev.get(), a.rgb = out_rgb ? rgb_dev.get() : nullptr;
+  }
+  const int rc = runOrdered(&m, 1, st, [&](cudaStream_t s) { launchRender(a, s); });
+  if (rc || memory == NVB_MEM_DEVICE) return rc;
+  NVB_CUDA(cudaMemcpyAsync(out_depth, a.depth, n * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (out_rgb) NVB_CUDA(cudaMemcpyAsync(out_rgb, a.rgb, 3 * n, cudaMemcpyDeviceToHost, st));
+  NVB_CUDA(cudaStreamSynchronize(st));
+  return NVB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+void nvb_default_sphere_tracer_params(NvbSphereTracerParams* p) {
+  if (!p) return;
+  p->maximum_steps = 100;  // rays/sphere_tracer.h:216-218
+  p->maximum_ray_length_m = 15.0f;
+  p->surface_distance_epsilon_vox = 0.1f;
+}
+
+int32_t nvb_render_depth(NvbMapper* m, const NvbSphereTracerParams* p, const float* T_L_C, const NvbCamera* cam,
+                         float truncation_distance_m, int32_t ray_subsampling_factor, int32_t memory, float* out_depth,
+                         void* stream) {
+  if (!m || !p || !T_L_C || !cam || !out_depth) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  return renderImpl(m, p, T_L_C, cam, truncation_distance_m, ray_subsampling_factor, memory, out_depth, nullptr, stream);
+}
+
+int32_t nvb_render_rgbd(NvbMapper* m, const NvbSphereTracerParams* p, const float* T_L_C, const NvbCamera* cam,
+                        float truncation_distance_m, int32_t ray_subsampling_factor, int32_t memory, float* out_depth,
+                        uint8_t* out_rgb, void* stream) {
+  if (!m || !p || !T_L_C || !cam || !out_depth || !out_rgb) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  return renderImpl(m, p, T_L_C, cam, truncation_distance_m, ray_subsampling_factor, memory, out_depth, out_rgb, stream);
+}
+
+}  // extern "C"

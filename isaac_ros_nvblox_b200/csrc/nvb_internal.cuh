@@ -547,6 +547,17 @@ struct ColorArgs {
 void launchColorSelect(const ColorArgs& a, int num_sms, cudaStream_t stream);
 void launchSphereTrace(const ColorArgs& a, cudaStream_t stream);
 void launchColorIntegrate(const ColorArgs& a, int num_sms, cudaStream_t stream);
+// SphereTracer::renderImageOnGPU / renderRgbdImageOnGPU (nvb_color.cu): one image of drows x dcols rays.
+struct RenderArgs {
+  DevLayer tsdf, color;  // color.blocks == nullptr: the mapper has no colour layer (every hit is black)
+  Rigid T_L_C;
+  NvbCamera cam;
+  float block_size, voxel_size_inv, trunc_m, max_ray_len, eps_m;
+  int max_steps, subsample, drows, dcols;
+  float* depth;          // drows x dcols
+  unsigned char* rgb;    // drows x dcols x 3 (RGB), or nullptr: depth only
+};
+void launchRender(const RenderArgs& a, cudaStream_t stream);
 
 struct DecayArgs {
   DevLayer layer;  // the projective layer (TsdfVoxel or OccupancyVoxel blocks)
