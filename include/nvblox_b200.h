@@ -356,6 +356,49 @@ NVB_API int32_t nvb_render_rgbd(NvbMapper* m, const NvbSphereTracerParams* p, co
                                 float truncation_distance_m, int32_t ray_subsampling_factor, int32_t memory, float* out_depth,
                                 uint8_t* out_rgb, void* stream);
 
+/* primitives::Scene (C/include/nvblox/primitives/primitives.h, scene.h, src/primitives/primitives.cpp, scene.cpp,
+ * primitives/internal/impl/scene_impl.h): planes, cubes, spheres and cylinders, and the exact distance fields and depth images
+ * they give. Primitive::Type order. */
+typedef enum { NVB_PRIM_PLANE = 0, NVB_PRIM_CUBE = 1, NVB_PRIM_SPHERE = 2, NVB_PRIM_CYLINDER = 3 } NvbPrimitiveType;
+/* One primitive: params are the plane's unit normal (norm 1 +- 1e-3), the cube's x, y, z size, the sphere's radius, or the
+ * cylinder's radius and height (axis along z); the unused entries are ignored. */
+typedef struct {
+  int32_t type;
+  float center[3];
+  float params[4];
+} NvbPrimitive;
+/* A scene: the primitives (host memory, any number) and the box a generated layer covers (Scene::aabb(), by default
+ * (-5, -5, -1) to (5, 5, 9)). */
+typedef struct {
+  const NvbPrimitive* primitives;
+  int32_t num_primitives;
+  float aabb_min[3];
+  float aabb_max[3];
+} NvbScene;
+/* Scene::generateDepthImageFromScene(camera, T_S_C, max_dist, &depth, invalid_depth): out_depth receives height * width
+ * floats, row-major; pixel (r, c) casts the ray T_S_C.linear() * vectorFromPixelIndices((c, r)).normalized() from T_S_C's
+ * origin, and gets the z of the nearest hit within max_dist in the camera frame, or invalid_depth.
+ * memory = NVB_MEM_DEVICE: enqueued on `stream` (a cudaStream_t on the current device; NULL is the default stream), nothing
+ * synchronises. memory = NVB_MEM_HOST: the image is written when the call returns. */
+NVB_API int32_t nvb_scene_render_depth(const NvbScene* scene, const NvbCamera* cam, const float* T_S_C, float max_dist,
+                                       float invalid_depth, int32_t memory, float* out_depth, void* stream);
+/* Scene::getSignedDistanceToPoint(p, max_dist) of n points (xyz, 3 floats each) into out (n floats); both in `memory`,
+ * ordered like nvb_scene_render_depth. */
+NVB_API int32_t nvb_scene_signed_distance(const NvbScene* scene, const float* xyz, int32_t memory, int64_t n, float max_dist,
+                                          float* out, void* stream);
+/* Scene::generateLayerFromScene<VoxelType>(max_dist, layer) on the mapper's layer_id: NVB_LAYER_TSDF or NVB_LAYER_OCCUPANCY
+ * (whichever is the mapper's projective layer) or NVB_LAYER_FREESPACE (a mapper with one). Every block the AABB touches is
+ * allocated; then every voxel of the layer whose centre lies in the (closed) AABB is written: TSDF max(sdf, -max_dist) with
+ * weight 1, occupancy the log odds of probability 1 where sdf <= sqrt(3) * voxel_size / 2 and of 0 elsewhere, freespace only
+ * is_high_confidence_freespace, true where sdf is above that. The block-update tracker is not told. An AABB of more than
+ * 2^28 blocks is NVB_ERR_CAPACITY and changes nothing. Synchronous. */
+NVB_API int32_t nvb_scene_generate_layer(NvbMapper* m, int32_t layer_id, const NvbScene* scene, float max_dist);
+/* nvblox_torch's Scene::toMapper for one mapper (nvblox_torch/cpp/src/py_scene.cu): the projective layer (TSDF, or
+ * occupancy on an occupancy mapper) is replaced by the scene's layer with max_dist = 4 voxels, like VoxelBlockLayer::copyFrom;
+ * every block of it is marked for the ESDF, freespace and mesh consumers, and the ESDF is updated. The colour, mesh and
+ * freespace layers are left as they are. Synchronous. */
+NVB_API int32_t nvb_scene_to_mapper(NvbMapper* m, const NvbScene* scene);
+
 /* Mapper::integrateDepth(MaskedDepthImageConstView, T_L_C, Camera)
  * (mapper.h:167-172, mapper_impl.h:28-81) =
  * ProjectiveTsdfIntegrator::integrateFrame (projective_tsdf_integrator.h:48-52)

@@ -56,6 +56,7 @@ EXPORTED_SYMBOLS = [
     "nvb_layer_query_voxels", "nvb_layer_interpolate", "nvb_query_esdf", "nvb_query_tsdf", "nvb_query_occupancy",
     "nvb_mapper_save_map", "nvb_mapper_load_map", "nvb_layer_export_points",
     "nvb_default_sphere_tracer_params", "nvb_render_depth", "nvb_render_rgbd",
+    "nvb_scene_render_depth", "nvb_scene_signed_distance", "nvb_scene_generate_layer", "nvb_scene_to_mapper",
 ]
 
 
@@ -112,6 +113,18 @@ class NvbColorParams(C.Structure):
 class NvbSphereTracerParams(C.Structure):
     _fields_ = [("maximum_steps", C.c_int32), ("maximum_ray_length_m", C.c_float),
                 ("surface_distance_epsilon_vox", C.c_float)]
+
+
+NVB_PRIM_PLANE, NVB_PRIM_CUBE, NVB_PRIM_SPHERE, NVB_PRIM_CYLINDER = 0, 1, 2, 3
+
+
+class NvbPrimitive(C.Structure):
+    _fields_ = [("type", C.c_int32), ("center", C.c_float * 3), ("params", C.c_float * 4)]
+
+
+class NvbScene(C.Structure):
+    _fields_ = [("primitives", C.POINTER(NvbPrimitive)), ("num_primitives", C.c_int32), ("aabb_min", C.c_float * 3),
+                ("aabb_max", C.c_float * 3)]
 
 
 class NvbFreespaceParams(C.Structure):
@@ -349,6 +362,10 @@ def load(path=None):
     L.nvb_default_sphere_tracer_params.restype = None
     L.nvb_render_depth.argtypes = [vp, C.POINTER(NvbSphereTracerParams), fp, C.POINTER(NvbCamera), f32, i32, i32, vp, vp]
     L.nvb_render_rgbd.argtypes = [vp, C.POINTER(NvbSphereTracerParams), fp, C.POINTER(NvbCamera), f32, i32, i32, vp, vp, vp]
+    L.nvb_scene_render_depth.argtypes = [C.POINTER(NvbScene), C.POINTER(NvbCamera), fp, f32, f32, i32, vp, vp]
+    L.nvb_scene_signed_distance.argtypes = [C.POINTER(NvbScene), vp, i32, i64, f32, vp, vp]
+    L.nvb_scene_generate_layer.argtypes = [vp, i32, C.POINTER(NvbScene), f32]
+    L.nvb_scene_to_mapper.argtypes = [vp, C.POINTER(NvbScene)]
     L.nvb_mapper_kernel_launches.restype = C.c_int64
     for name in EXPORTED_SYMBOLS:
         f = getattr(L, name)

@@ -137,6 +137,9 @@ struct NvbMapper {
   DeviceArray<int4> fs_work;
   int tsdf_count_ub = 0;   // host-side upper bound of *tsdf.count
   int esdf_extra_ub = 0;   // blocks submitted to the ESDF through explicit lists
+  // Blocks the colour, mesh and freespace layers may hold beyond the projective layer's fill level: those of a projective
+  // layer that nvb_scene_to_mapper replaced. These layers are sized to the projective slab's capacity, so it keeps room for them.
+  int derived_extra_ub = 0;
 
   DeviceArray<int4> union_list;  // nvb_blocks_union's own output list
   DeviceArray<int> union_list_count;
@@ -703,6 +706,7 @@ void pollCounts(NvbMapper* m) {
 
 int ensureTsdfCapacity(NvbMapper* m, long long new_cells) {
   pollCounts(m);
+  new_cells += m->derived_extra_ub;
   if ((long long)m->tsdf_count_ub + new_cells <= m->tsdf.capacity) return NVB_OK;
   // refine the bound with a synchronous read
   NVB_CUDA(syncAll(m));
@@ -1396,7 +1400,7 @@ static int resetLayers(NvbMapper* m) {
     launchFillU64(m->mesh.hash.keys, kEmptyKey, (size_t)m->mesh.hash.mask + 1, m->stream);
     NVB_CUDA(cudaMemsetAsync(m->mesh_state.get(), 0, kArenaInts * sizeof(int), m->stream));
   }
-  m->tsdf_count_ub = 0, m->tsdf_count_confirmed = 0, m->esdf_extra_ub = 0;
+  m->tsdf_count_ub = 0, m->tsdf_count_confirmed = 0, m->esdf_extra_ub = 0, m->derived_extra_ub = 0;
   m->cells_cum = 0, m->confirmed_cum = 0;
   for (int k = 0; k < kCountRing; k++) m->count_pending[k] = false;
   NVB_CUDA(syncAll(m));
@@ -3947,6 +3951,263 @@ int32_t nvb_render_rgbd(NvbMapper* m, const NvbSphereTracerParams* p, const floa
                         uint8_t* out_rgb, void* stream) {
   if (!m || !p || !T_L_C || !cam || !out_depth || !out_rgb) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   return renderImpl(m, p, T_L_C, cam, truncation_distance_m, ray_subsampling_factor, memory, out_depth, out_rgb, stream);
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------
+// primitives::Scene (nvb_scene.cu)
+// ---------------------------------------------------------------------------
+namespace {
+
+// The scene's own checks: the Plane constructor's CHECK_NEAR(normal.norm(), 1.0, 1e-3) (primitives.h), evaluated in double
+// like glog's, and Primitive::toString's LOG(FATAL) on an unknown type.
+int validateScene(const NvbScene* s) {
+  if (!s) return fail(NVB_ERR_INVALID_ARGUMENT, "null scene");
+  if (s->num_primitives < 0 || (s->num_primitives > 0 && !s->primitives)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad primitive list");
+  for (int i = 0; i < s->num_primitives; i++) {
+    const NvbPrimitive& q = s->primitives[i];
+    if (q.type < NVB_PRIM_PLANE || q.type > NVB_PRIM_CYLINDER) return fail(NVB_ERR_INVALID_ARGUMENT, "unknown primitive type");
+    if (q.type == NVB_PRIM_PLANE) {
+      const double norm = std::sqrt(sum3(q.params[0] * q.params[0], q.params[1] * q.params[1], q.params[2] * q.params[2]));
+      if (!(norm <= 1.0 + 1e-3 && norm >= 1.0 - 1e-3)) return fail(NVB_ERR_INVALID_ARGUMENT, "a plane's normal is not unit length");
+    }
+  }
+  return NVB_OK;
+}
+
+// The scene with its primitives copied into stream-ordered device memory, released (stream-ordered) by the destructor: the
+// copy and the free are enqueued on the stream after the caller's work, and the host does not wait for either.
+struct DeviceScene {
+  NvbScene s{};
+  cudaStream_t st = nullptr;
+  ~DeviceScene() {
+    if (s.primitives) cudaFreeAsync(const_cast<NvbPrimitive*>(s.primitives), st);
+  }
+  cudaError_t upload(const NvbScene& host, cudaStream_t stream) {
+    s = host, s.primitives = nullptr, st = stream;
+    if (host.num_primitives == 0) return cudaSuccess;
+    const size_t bytes = (size_t)host.num_primitives * sizeof(NvbPrimitive);
+    NvbPrimitive* d = nullptr;
+    cudaError_t e = cudaMallocAsync(&d, bytes, stream);
+    if (e != cudaSuccess) return e;
+    s.primitives = d;
+    return cudaMemcpyAsync(d, host.primitives, bytes, cudaMemcpyHostToDevice, stream);
+  }
+};
+
+int deviceSms() {
+  int dev = 0, sms = kHelperCtas;
+  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms;
+}
+
+// getBlockIndicesTouchedByBoundingBox (geometry/internal/impl/bounding_boxes_impl.h:28-53): the block-index box of the scene's
+// AABB and its number of blocks, which must be at most 2^28, with indices inside the hash key's +-2^20.
+int sceneBlockBox(const NvbMapper* m, const NvbScene* scene, int3* lo_out, int3* size_out, long long* cells) {
+  const int3 lo = blockIndexFromPosition(m->block_size, Vec3{scene->aabb_min[0], scene->aabb_min[1], scene->aabb_min[2]});
+  const int3 hi = blockIndexFromPosition(m->block_size, Vec3{scene->aabb_max[0], scene->aabb_max[1], scene->aabb_max[2]});
+  const int3 size = make_int3(std::max(0, hi.x - lo.x + 1), std::max(0, hi.y - lo.y + 1), std::max(0, hi.z - lo.z + 1));
+  *cells = (long long)size.x * size.y * size.z;
+  if (*cells > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "the scene's AABB covers more than 2^28 blocks");
+  if (*cells > 0 && (!indexInRange(lo.x, lo.y, lo.z) || !indexInRange(hi.x, hi.y, hi.z)))
+    return fail(NVB_ERR_INDEX_RANGE, "the scene's AABB reaches a block index outside +-2^20");
+  if (lo_out) *lo_out = lo, *size_out = size;
+  return NVB_OK;
+}
+
+// Scene::generateLayerFromScene on L (the mapper's layer layer_id): allocation, then the fill, on m->stream.
+int generateLayerImpl(NvbMapper* m, DevLayer* L, int layer_id, const NvbScene* scene, float max_dist) {
+  SceneLayerArgs a{};
+  int rc;
+  if ((rc = sceneBlockBox(m, scene, &a.box_lo, &a.box_size, &a.cells))) return rc;
+  if (L == &m->tsdf) {
+    if ((rc = ensureTsdfCapacity(m, a.cells))) return rc;
+    m->cells_cum += a.cells;
+    m->tsdf_count_ub = (int)std::min<long long>((long long)m->tsdf_count_ub + a.cells, 0x7fffffff);
+  } else {  // the freespace slab: at least the TSDF slab's capacity, doubled until the AABB's blocks fit
+    NVB_CUDA(syncAll(m));
+    int count = 0;
+    NVB_CUDA(cudaMemcpy(&count, L->count, sizeof(int), cudaMemcpyDeviceToHost));
+    long long cap = std::max(L->capacity, m->tsdf.capacity);
+    while (cap < (long long)std::min(count, L->capacity) + a.cells) cap *= 2;
+    if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "the freespace layer would exceed 2^28 blocks");
+    if (cap > L->capacity && (rc = growLayer(m, L, (int)cap))) return rc;
+  }
+  NVB_CUDA(cudaSetDevice(m->device));
+  NVB_CUDA(joinEsdf(m));  // an update_esdf_async may still be reading the layer
+  DeviceScene ds;
+  NVB_CUDA(ds.upload(*scene, m->stream));
+  a.scene = ds.s;
+  a.layer = *L;
+  a.layer_id = layer_id;
+  a.block_size = m->block_size;
+  a.max_dist = max_dist;
+  // getVoxelGroundTruthValue: sqrt(3.0) * voxel_size rounded to float, halved in double (exact)
+  a.occupied_threshold_m = (float)(std::sqrt(3.0) * (double)m->voxel_size) / 2.0f;
+  a.occupied_log_odds = logOddsFromProbability(1.0f);
+  a.free_log_odds = logOddsFromProbability(0.0f);
+  a.error = m->error_dev;
+  launchSceneAllocate(a, m->num_sms, m->stream);
+  launchSceneFill(a, m->num_sms, m->stream);
+  m->launches += 2;
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  return checkDeviceError(m);
+}
+
+// Fill level (slots handed out) of a layer, 0 for a layer the mapper does not have. The streams must be idle.
+int slabFill(const DevLayer& L, int* out) {
+  *out = 0;
+  if (!L.blocks) return NVB_OK;
+  NVB_CUDA(cudaMemcpy(out, L.count, sizeof(int), cudaMemcpyDeviceToHost));
+  *out = std::min(*out, L.capacity);
+  return NVB_OK;
+}
+
+// The projective layer as VoxelBlockLayer::copyFrom leaves it before the copy: no blocks, with room for `cells` new ones. Its
+// slots are zeroed and handed out again from 0, so every consumer's dirty words are cleared too. The ESDF, colour, mesh and
+// freespace layers keep their blocks, so the capacity bounds count them as extra: the ESDF's through esdf_extra_ub, the others'
+// (which follow the projective slab) through derived_extra_ub. Both slabs are grown first, keeping their contents, so that a
+// failed growth leaves the map as it was.
+int emptyProjectiveLayer(NvbMapper* m, long long cells) {
+  NVB_CUDA(syncAll(m));
+  int esdf_n = 0, fs_n = 0, color_n = 0, mesh_n = 0, rc;
+  if ((rc = slabFill(m->esdf, &esdf_n)) || (rc = slabFill(m->freespace, &fs_n)) || (rc = slabFill(m->color, &color_n)) ||
+      (rc = slabFill(m->mesh, &mesh_n)))
+    return rc;
+  const long long derived = std::max({fs_n, color_n, mesh_n});
+  long long cap = m->tsdf.capacity;
+  while (cap < cells + derived) cap *= 2;
+  if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "TSDF layer would exceed 2^28 blocks");
+  if (cap > m->tsdf.capacity && ((rc = growLayer(m, &m->tsdf, (int)cap)) || (rc = growTracker(m, (int)cap)))) return rc;
+  if ((rc = ensureEsdfCapacity(m, cells + esdf_n))) return rc;
+  DevLayer* L = &m->tsdf;
+  int count = 0;
+  if ((rc = slabFill(*L, &count))) return rc;
+  NVB_CUDA(cudaMemsetAsync(L->blocks, 0, (size_t)count * L->block_bytes, m->stream));
+  NVB_CUDA(cudaMemsetAsync(L->count, 0, sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(L->free_count, 0, sizeof(int), m->stream));
+  launchFillU64(L->hash.keys, kEmptyKey, (size_t)L->hash.mask + 1, m->stream);
+  m->launches++;
+  for (TrackedBlocks& t : m->tracker) {
+    if (!t.dirty.get()) continue;
+    NVB_CUDA(cudaMemsetAsync(t.dirty.get(), 0, t.dirty.size() * sizeof(int), m->stream));
+    NVB_CUDA(cudaMemsetAsync(t.count, 0, sizeof(int), m->stream));
+  }
+  m->tsdf_count_ub = m->tsdf_count_confirmed = 0;
+  m->confirmed_cum = m->cells_cum;
+  for (int k = 0; k < kCountRing; k++) m->count_pending[k] = false;
+  m->esdf_extra_ub = esdf_n;
+  m->derived_extra_ub = (int)derived;
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  return NVB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t nvb_scene_render_depth(const NvbScene* scene, const NvbCamera* cam, const float* T_S_C, float max_dist,
+                               float invalid_depth, int32_t memory, float* out_depth, void* stream) {
+  int rc;
+  if ((rc = validateScene(scene))) return rc;
+  if (!cam || !T_S_C || !out_depth) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (cam->width <= 0 || cam->height <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "the camera must have a positive size");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  SceneDepthArgs a{};
+  a.cam = *cam;
+  a.T_S_C = rigidFromColMajor(T_S_C);
+  a.T_C_S = invertRigid(a.T_S_C);
+  a.max_dist = max_dist, a.invalid_depth = invalid_depth;
+  a.rows = cam->height, a.cols = cam->width;
+  const size_t n = (size_t)a.rows * a.cols;
+  float* staged = nullptr;
+  if (memory == NVB_MEM_HOST) NVB_CUDA(cudaMallocAsync(&staged, n * sizeof(float), st));
+  a.depth = memory == NVB_MEM_HOST ? staged : out_depth;
+  cudaError_t e;
+  {
+    DeviceScene ds;
+    e = ds.upload(*scene, st);
+    a.scene = ds.s;
+    if (e == cudaSuccess) {
+      launchSceneDepth(a, st);
+      e = cudaGetLastError();
+    }
+  }
+  if (e == cudaSuccess && staged) e = cudaMemcpyAsync(out_depth, staged, n * sizeof(float), cudaMemcpyDeviceToHost, st);
+  if (staged) cudaFreeAsync(staged, st);
+  if (e == cudaSuccess && staged) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(NVB_ERR_CUDA, std::string("nvb_scene_render_depth: ") + cudaGetErrorString(e));
+  return NVB_OK;
+}
+
+int32_t nvb_scene_signed_distance(const NvbScene* scene, const float* xyz, int32_t memory, int64_t n, float max_dist,
+                                  float* out, void* stream) {
+  int rc;
+  if ((rc = validateScene(scene))) return rc;
+  if (n < 0 || (n > 0 && (!xyz || !out))) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (n == 0) return NVB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const float* in_dev = xyz;
+  float* out_dev = out;
+  float* staged = nullptr;  // host memory: 3 n input floats, then n outputs
+  cudaError_t e = cudaSuccess;
+  if (memory == NVB_MEM_HOST) {
+    NVB_CUDA(cudaMallocAsync(&staged, (size_t)n * 4 * sizeof(float), st));
+    in_dev = staged, out_dev = staged + 3 * n;
+    e = cudaMemcpyAsync(staged, xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, st);
+  }
+  {
+    DeviceScene ds;
+    if (e == cudaSuccess) e = ds.upload(*scene, st);
+    if (e == cudaSuccess) {
+      launchSceneDistance(ds.s, in_dev, n, max_dist, out_dev, deviceSms(), st);
+      e = cudaGetLastError();
+    }
+  }
+  if (e == cudaSuccess && staged) e = cudaMemcpyAsync(out, out_dev, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st);
+  if (staged) cudaFreeAsync(staged, st);
+  if (e == cudaSuccess && staged) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(NVB_ERR_CUDA, std::string("nvb_scene_signed_distance: ") + cudaGetErrorString(e));
+  return NVB_OK;
+}
+
+int32_t nvb_scene_generate_layer(NvbMapper* m, int32_t layer_id, const NvbScene* scene, float max_dist) {
+  if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
+  int rc;
+  if ((rc = validateScene(scene))) return rc;
+  // scene_impl.h defines setVoxel for TsdfVoxel, OccupancyVoxel and FreespaceVoxel only
+  if (layer_id != NVB_LAYER_TSDF && layer_id != NVB_LAYER_OCCUPANCY && layer_id != NVB_LAYER_FREESPACE)
+    return fail(NVB_ERR_INVALID_ARGUMENT, "scenes generate TSDF, occupancy or freespace layers only");
+  DevLayer* L = layerOf(m, layer_id);
+  if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper has no such layer");
+  NVB_CUDA(cudaSetDevice(m->device));
+  return generateLayerImpl(m, L, layer_id, scene, max_dist);
+}
+
+int32_t nvb_scene_to_mapper(NvbMapper* m, const NvbScene* scene) {
+  if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
+  int rc;
+  if ((rc = validateScene(scene))) return rc;
+  NVB_CUDA(cudaSetDevice(m->device));
+  const int layer_id = m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY ? NVB_LAYER_OCCUPANCY : NVB_LAYER_TSDF;
+  // generateLayerImpl's checks, and every slab growth, before the layer is emptied
+  long long cells = 0;
+  if ((rc = sceneBlockBox(m, scene, nullptr, nullptr, &cells))) return rc;
+  // py_scene.cu: copyFrom of the scene's layer with max_distance = 4 voxels
+  if ((rc = emptyProjectiveLayer(m, cells))) return rc;
+  if ((rc = generateLayerImpl(m, &m->tsdf, layer_id, scene, 4.0f * m->voxel_size))) return rc;
+  // markBlocksForUpdate(all blocks): every started consumer's list becomes every block (launchTodoAll); the others start with
+  // every block on their first update anyway
+  for (int k = 0; k < kNumBlocksToUpdateTypes; k++) {
+    TrackedBlocks& t = m->tracker[k];
+    if (!t.initialized) continue;
+    launchTodoAll(m->tsdf, t.list(), m->stream);
+    m->launches++;
+  }
+  return nvb_mapper_update_esdf(m, 0);
 }
 
 }  // extern "C"

@@ -171,6 +171,27 @@ __host__ __device__ inline void removeDistortion(const NvbCamera& c, float& ux, 
   uy = (float)y;
 }
 
+#ifdef __CUDACC__
+// The ray of pixel (r, c) of the f-subsampled image goes through the image-plane point f * (c, r) + f / 2
+// (SphereTracer's sphereTracingKernel, src/rays/sphere_tracer.cu:134-173). dz is the camera-frame direction's z, u the
+// layer-frame direction. With f = 1 this is Camera::vectorFromPixelIndices(u).normalized() rotated by T's linear part, the
+// ray of Scene::generateDepthImageFromScene (nvb_scene.cu).
+template <bool kDistort>
+__device__ __forceinline__ void pixelRay(const NvbCamera& cam, const Rigid& T, int f, int r, int c, float& dz, Vec3& u) {
+  const float half = 0.5f * (float)f;
+  const float px = (float)(c * f) + half * 1.0f, py = (float)(r * f) + half * 1.0f;
+  // Camera::vectorFromImagePlaneCoordinates (camera_impl.h:89-104), then Eigen normalized()
+  float nx = (px - cam.cu) / cam.fu, ny = (py - cam.cv) / cam.fv;
+  if (kDistort) removeDistortion(cam, nx, ny);
+  const float norm = sqrtf(sum3(nx * nx, ny * ny, 1.0f * 1.0f));
+  const float dx = nx / norm, dy = ny / norm;
+  dz = 1.0f / norm;
+  u.x = sum3(T.r[0][0] * dx, T.r[0][1] * dy, T.r[0][2] * dz);
+  u.y = sum3(T.r[1][0] * dx, T.r[1][1] * dy, T.r[1][2] * dz);
+  u.z = sum3(T.r[2][0] * dx, T.r[2][1] * dy, T.r[2][2] * dz);
+}
+#endif  // __CUDACC__
+
 // ---------------------------------------------------------------------------
 // Device-resident block hash: packed Index3D -> slot in the layer's slab.
 // Open addressing, linear probing, 64-bit keys (3 x 21 bit, biased).
@@ -558,6 +579,33 @@ struct RenderArgs {
   unsigned char* rgb;    // drows x dcols x 3 (RGB), or nullptr: depth only
 };
 void launchRender(const RenderArgs& a, cudaStream_t stream);
+
+// primitives::Scene (nvb_scene.cu). The scene's primitives are in device memory here.
+struct SceneDepthArgs {  // Scene::generateDepthImageFromScene
+  NvbScene scene;
+  NvbCamera cam;
+  Rigid T_S_C, T_C_S;
+  float max_dist, invalid_depth;
+  int rows, cols;
+  float* depth;  // rows x cols
+};
+void launchSceneDepth(const SceneDepthArgs& a, cudaStream_t stream);
+// Scene::getSignedDistanceToPoint of n points (xyz) into out
+void launchSceneDistance(const NvbScene& scene, const float* xyz, long long n, float max_dist, float* out, int num_sms,
+                         cudaStream_t stream);
+struct SceneLayerArgs {  // Scene::generateLayerFromScene
+  NvbScene scene;
+  DevLayer layer;
+  int layer_id;                  // NVB_LAYER_TSDF, _OCCUPANCY or _FREESPACE
+  int3 box_lo, box_size;         // getBlockIndicesTouchedByBoundingBox: the block-index box of the AABB ...
+  long long cells;               // ... and its number of blocks
+  float block_size, max_dist;
+  float occupied_threshold_m;    // sqrt(3) * voxel_size / 2: an object is inside the voxel at or below it
+  float occupied_log_odds, free_log_odds;  // logOddsFromProbability(1), (0), computed on the host
+  int* error;
+};
+void launchSceneAllocate(const SceneLayerArgs& a, int num_sms, cudaStream_t stream);
+void launchSceneFill(const SceneLayerArgs& a, int num_sms, cudaStream_t stream);
 
 struct DecayArgs {
   DevLayer layer;  // the projective layer (TsdfVoxel or OccupancyVoxel blocks)
