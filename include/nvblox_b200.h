@@ -621,8 +621,8 @@ NVB_API void nvb_default_image_masker_params(NvbImageMaskerParams* p);
  * with_overlay != 0 the RGB overlay is grey 12.75 * depth (clamped to 0..255; NaN 255) with red 255 on foreground pixels.
  * Deviations from the reference: a projection exactly on u == width or v == height is a miss here (the reference reads
  * past the mask's row); a negative depth has grey 0 (undefined in the reference). Sizes must match the cameras
- * (width x height); depth, mask (mask_rows x mask_cols bytes) are in `memory`. Host inputs are staged in buffers the
- * mapper keeps. The outputs stay in the mapper (nvb_mapper_split_output, nvb_mapper_split_device_buffers); the call does
+ * (width x height); depth, mask (mask_rows x mask_cols bytes) are in `memory`. Host inputs are copied to the device on the
+ * mapper's stream before the call returns. The outputs stay in the mapper (nvb_mapper_split_output, nvb_mapper_split_device_buffers); the call does
  * not synchronise (the reference does). */
 NVB_API int32_t nvb_mapper_split_depth_image(NvbMapper* m, const float* depth, int32_t depth_rows, int32_t depth_cols,
                                              const uint8_t* mask, int32_t mask_rows, int32_t mask_cols, int32_t memory,

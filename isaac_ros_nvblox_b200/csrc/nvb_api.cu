@@ -83,6 +83,73 @@ class DeviceArray {
   size_t n_ = 0;
 };
 
+// A caller's buffers are host or device memory (NvbMemory); any other kind is rejected before anything is enqueued.
+int checkMemoryKind(int32_t memory) {
+  if (memory == NVB_MEM_HOST || memory == NVB_MEM_DEVICE) return NVB_OK;
+  return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+}
+
+// The device side of one call's caller buffers, all of one memory kind, for work on `st`. Device buffers are used in place.
+// Host buffers are staged in stream-ordered allocations on `st` from `pool` (the device's default pool when null): an input
+// is copied down when it is staged, the outputs are copied back by finish(), and the destructor frees the staging on `st`
+// behind everything enqueued so far, so an early return neither leaks it nor frees memory a kernel still reads, and the host
+// never waits for the release. A null or empty host buffer stays null on the device.
+class CallerBuffers {
+ public:
+  CallerBuffers(int32_t memory, cudaStream_t st, cudaMemPool_t pool) : host_(memory == NVB_MEM_HOST), st_(st), pool_(pool) {}
+  CallerBuffers(const CallerBuffers&) = delete;
+  CallerBuffers& operator=(const CallerBuffers&) = delete;
+  ~CallerBuffers() {
+    for (const Staged& s : staged_) cudaFreeAsync(s.dev, st_);
+  }
+
+  template <typename T>
+  cudaError_t in(const T* p, size_t bytes, const T** dev) {
+    void* d = nullptr;
+    const cudaError_t e = stage(const_cast<T*>(p), bytes, false, true, &d);
+    *dev = host_ ? static_cast<const T*>(d) : p;
+    return e;
+  }
+  // `upload` also copies the caller's contents down, so that what the kernels do not write comes back unchanged.
+  template <typename T>
+  cudaError_t out(T* p, size_t bytes, T** dev, bool upload = false) {
+    void* d = nullptr;
+    const cudaError_t e = stage(p, bytes, true, upload, &d);
+    *dev = host_ ? static_cast<T*>(d) : p;
+    return e;
+  }
+  // Host memory: the outputs are copied back and `st` is synchronised. Device memory: nothing to do.
+  cudaError_t finish() {
+    if (!host_) return cudaSuccess;
+    for (const Staged& s : staged_) {
+      if (!s.copy_back) continue;
+      const cudaError_t e = cudaMemcpyAsync(s.host, s.dev, s.bytes, cudaMemcpyDeviceToHost, st_);
+      if (e != cudaSuccess) return e;
+    }
+    return cudaStreamSynchronize(st_);
+  }
+
+ private:
+  struct Staged {
+    void* dev;
+    void* host;
+    size_t bytes;
+    bool copy_back;
+  };
+  cudaError_t stage(void* p, size_t bytes, bool copy_back, bool copy_down, void** dev) {
+    if (!host_ || !p || bytes == 0) return cudaSuccess;
+    cudaError_t e = pool_ ? cudaMallocFromPoolAsync(dev, bytes, pool_, st_) : cudaMallocAsync(dev, bytes, st_);
+    if (e != cudaSuccess) return e;
+    staged_.push_back({*dev, p, bytes, copy_back});
+    return copy_down ? cudaMemcpyAsync(*dev, p, bytes, cudaMemcpyHostToDevice, st_) : cudaSuccess;
+  }
+
+  bool host_;
+  cudaStream_t st_;
+  cudaMemPool_t pool_;
+  std::vector<Staged> staged_;
+};
+
 // One consumer of the block-update tracker: its dirty words and list, as large as the projective slab, and the list's
 // count in esdf_ints. Producers tell a consumer only once it is initialized, which its first all-blocks update does (the
 // lazy initialisation of BlocksToUpdateTracker, map/blocks_to_update_tracker.h).
@@ -126,8 +193,6 @@ struct NvbMapper {
   NvbColorParams cp{};
   DeviceArray<int4> color_work;  // blocks of the last colour frame {x, y, z, colour slot}
   DeviceArray<float> color_synth;  // sphere-traced synthetic depth
-  DeviceArray<unsigned char> color_stage;  // host colour image / mask staged on the device
-  DeviceArray<unsigned char> color_mask_stage;
   NvbFreespaceParams fp;
   NvbEsdfSliceParams sp;
   int esdf_mode = 0;                // EsdfMode: 0 unset, 1 3-D, 2 2-D slice (mapper.h:61, src/mapper/mapper.cpp:408-470)
@@ -232,7 +297,6 @@ struct NvbMapper {
   DeviceArray<int> gp_slots;                // 2 x gp_counts.size(): the slots, then the slots in (x, y, z) block-index order
   DeviceArray<int2> gp_counts;
   DeviceArray<unsigned char> gp_sort_temp;  // the radix sort's scratch
-  DeviceArray<float> gp_fit_stage;          // nvb_ransac_fit_plane: host points staged on the device (3 floats each)
   DeviceArray<int> gp_totals;
   DeviceArray<float3> gp_crossings;
   DeviceArray<float4> gp_candidates;
@@ -256,18 +320,17 @@ struct NvbMapper {
   int dyn_rows = 0, dyn_cols = 0;
   DeviceArray<int> cc_labels;
   DeviceArray<int> cc_sizes;
-  DeviceArray<unsigned char> cc_stage;  // host masks staged for the filter (input, then output)
-  // image masker (nvb_masker.cu): the last split's outputs, sized by pixels; staged host inputs and the min-depth scratch
-  DeviceArray<float> msk_depth_stage;
-  DeviceArray<unsigned char> msk_mask_stage;
+  // image masker (nvb_masker.cu): the last split's outputs, sized by pixels, and the min-depth scratch
   DeviceArray<float> msk_min_depth;      // mask-sized
   DeviceArray<float> msk_background;
   DeviceArray<float> msk_foreground;
   DeviceArray<unsigned char> msk_overlay;
-  DeviceArray<unsigned char> msk_color;  // host colour splits: input, mask and the three outputs
   int msk_rows = 0, msk_cols = 0;
   bool msk_has_overlay = false;
   cudaEvent_t dyn_event = nullptr;    // nvb_mapper_wait_for: recorded on this mapper's stream
+  // CallerBuffers' staging of host buffers. Unlike the device's default pool, it keeps freed memory across synchronisations,
+  // so a call does not map its staging anew each time.
+  cudaMemPool_t stage_pool = nullptr;
   cudaEvent_t query_event = nullptr;  // point queries (nvb_query_*): the hand-over between this mapper and the query's stream
   // last integrated view (Mapper::last_posed_depth_image_, mapper.h:830-833), kept when keep_last_view is set
   int keep_last_view = 0;
@@ -794,11 +857,12 @@ int checkDeviceError(NvbMapper* m) {
   return NVB_OK;
 }
 
-int validateFrameArgs(const NvbMapper* m, const float* depth, int rows, int cols, const float* T, const NvbCamera* cam) {
+int validateFrameArgs(const NvbMapper* m, const float* depth, int32_t memory, int rows, int cols, const float* T,
+                      const NvbCamera* cam) {
   if (!m || !depth || !T || !cam) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (rows <= 0 || cols <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "image must have positive size");
   if (!(cam->fu != 0.0f) || !(cam->fv != 0.0f)) return fail(NVB_ERR_INVALID_ARGUMENT, "camera focal length is zero");
-  return NVB_OK;
+  return checkMemoryKind(memory);
 }
 
 // arePosesClose (C/src/geometry/transforms.cpp:20-36) in binary32, Eigen::AngleAxisf(R).angle() through the quaternion.
@@ -1274,6 +1338,15 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   NVB_CUDA(cudaEventCreateWithFlags(&m->esdf_ready, cudaEventDisableTiming));
   NVB_CUDA(cudaEventCreateWithFlags(&m->esdf_done, cudaEventDisableTiming));
   NVB_CUDA(cudaEventCreateWithFlags(&m->mark_done, cudaEventDisableTiming));
+  {
+    cudaMemPoolProps props{};
+    props.allocType = cudaMemAllocationTypePinned;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = m->device;
+    NVB_CUDA(cudaMemPoolCreate(&m->stage_pool, &props));
+    uint64_t keep = ~0ull;  // never release
+    NVB_CUDA(cudaMemPoolSetAttribute(m->stage_pool, cudaMemPoolAttrReleaseThreshold, &keep));
+  }
   const int tcap = opts->tsdf_capacity_blocks > 0 ? opts->tsdf_capacity_blocks : kDefaultCapacity;
   const int ecap = std::max(opts->esdf_capacity_blocks > 0 ? opts->esdf_capacity_blocks : kDefaultCapacity, tcap);
   int rc;
@@ -1356,6 +1429,7 @@ void nvb_mapper_destroy(NvbMapper* m) {
   }
   if (m->dyn_event) cudaEventDestroy(m->dyn_event);
   if (m->query_event) cudaEventDestroy(m->query_event);
+  if (m->stage_pool) cudaMemPoolDestroy(m->stage_pool);  // a render's staging freed on a caller's stream is released once that free completes
   if (m->mesh.blocks) freeLayer(&m->mesh);
   cudaFreeHost(m->h_ints), cudaFreeHost(m->h_count_ring), cudaFreeHost(m->h_list);
   for (int k = 0; k < kCountRing; k++) cudaEventDestroy(m->count_events[k]);
@@ -1592,7 +1666,7 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
   if (out_count) *out_count = 0;
   if (depth) {
-    int rc = validateFrameArgs(m, depth, rows, cols, T_L_C, cam);
+    int rc = validateFrameArgs(m, depth, depth_memory, rows, cols, T_L_C, cam);
     if (rc) return rc;
   }
   if (exclusion && exclusion->num_excluded_blocks > 0 && !exclusion->excluded_blocks_xyz_host)
@@ -1627,15 +1701,13 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
     a.deallocate = m->tdp.deallocate_decayed_blocks ? 1 : 0;
   }
   // block exclusion
-  std::vector<int> excl;
-  DeviceArray<int> excl_dev;
+  CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
   if (exclusion && exclusion->num_excluded_blocks > 0) {
     const int ne = exclusion->num_excluded_blocks;
-    NVB_CUDA(excl_dev.grow(m, (size_t)ne * 3, (size_t)ne * 3));
-    NVB_CUDA(cudaMemcpyAsync(excl_dev.get(), exclusion->excluded_blocks_xyz_host, (size_t)ne * 3 * sizeof(int), cudaMemcpyHostToDevice,
-                             m->stream));
+    const int* excl_dev;
+    NVB_CUDA(host.in(exclusion->excluded_blocks_xyz_host, (size_t)ne * 3 * sizeof(int), &excl_dev));
     m->skip_seq++;
-    launchMarkSkipped(P, excl_dev.get(), ne, m->skip_stamp.get(), m->skip_seq, m->stream);
+    launchMarkSkipped(P, excl_dev, ne, m->skip_stamp.get(), m->skip_seq, m->stream);
     a.skip_stamp = m->skip_stamp.get();
     a.skip_seq = m->skip_seq;
   }
@@ -1645,15 +1717,10 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
     a.r2 = exclusion->exclusion_radius_m * exclusion->exclusion_radius_m;
   }
   // view exclusion
-  DeviceArray<float> depth_tmp;
+  CallerBuffers bufs(depth_memory, m->stream, m->stage_pool);
   if (depth) {
-    const float* depth_dev = depth;
-    if (depth_memory == NVB_MEM_HOST) {
-      NVB_CUDA(depth_tmp.grow(m, (size_t)rows * cols, (size_t)rows * cols));
-      NVB_CUDA(cudaMemcpyAsync(depth_tmp.get(), depth, (size_t)rows * cols * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-      depth_dev = depth_tmp.get();
-    }
-    a.depth = depth_dev, a.rows = rows, a.cols = cols;
+    NVB_CUDA(bufs.in(depth, (size_t)rows * cols * sizeof(float), &a.depth));
+    a.rows = rows, a.cols = cols;
     a.T_C_L = invertRigid(rigidFromColMajor(T_L_C));
     a.cam = *cam;
   }
@@ -1734,15 +1801,10 @@ int freespaceUpdateImpl(NvbMapper* m, const int* in_xyz_dev, int n_explicit, lon
   a.p.half_voxel_size = m->block_size * (0.5f / kVps);
   a.p.max_integration_distance_m = max_view_distance_m > 0.0f ? max_view_distance_m : FLT_MAX;
   a.p.truncation_distance_m = truncation_distance_m > 0.0f ? truncation_distance_m : FLT_MAX;
-  DeviceArray<float> depth_tmp;
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
   if (depth) {
-    const float* depth_dev = depth;
-    if (memory == NVB_MEM_HOST) {
-      NVB_CUDA(depth_tmp.grow(m, (size_t)rows * cols, (size_t)rows * cols));
-      NVB_CUDA(cudaMemcpyAsync(depth_tmp.get(), depth, (size_t)rows * cols * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-      depth_dev = depth_tmp.get();
-    }
-    a.depth = depth_dev, a.rows = rows, a.cols = cols;
+    NVB_CUDA(bufs.in(depth, (size_t)rows * cols * sizeof(float), &a.depth));
+    a.rows = rows, a.cols = cols;
     a.T_C_L = invertRigid(rigidFromColMajor(T_L_C));
     a.cam = *cam;
   }
@@ -1761,7 +1823,7 @@ int32_t nvb_mapper_update_freespace(NvbMapper* m, int64_t update_time_ms, const 
   if (m->projective_layer_type != NVB_PROJECTIVE_TSDF_WITH_FREESPACE)
     return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper has no freespace layer");  // CHECK(hasFreespaceLayer(...)), mapper_impl.h:180-181
   if (depth) {
-    int rc = validateFrameArgs(m, depth, rows, cols, T_L_C, cam);
+    int rc = validateFrameArgs(m, depth, depth_memory, rows, cols, T_L_C, cam);
     if (rc) return rc;
   }
   NVB_CUDA(cudaSetDevice(m->device));
@@ -1781,7 +1843,7 @@ int32_t nvb_freespace_update_blocks(NvbMapper* m, const int32_t* blocks_xyz_host
   if (num_blocks < 0 || (num_blocks > 0 && !blocks_xyz_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad block list");
   if (num_blocks == 0) return NVB_OK;  // early return (:337-339)
   if (depth) {
-    int rc = validateFrameArgs(m, depth, rows, cols, T_L_C, cam);
+    int rc = validateFrameArgs(m, depth, depth_memory, rows, cols, T_L_C, cam);
     if (rc) return rc;
   }
   NVB_CUDA(cudaSetDevice(m->device));
@@ -1797,11 +1859,10 @@ int32_t nvb_freespace_update_blocks(NvbMapper* m, const int32_t* blocks_xyz_host
   std::sort(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x != b.x ? a.x < b.x : (a.y != b.y ? a.y < b.y : a.z < b.z); });
   v.erase(std::unique(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x == b.x && a.y == b.y && a.z == b.z; }), v.end());
   num_blocks = (int)v.size();
-  DeviceArray<int> xyz_dev;
-  NVB_CUDA(xyz_dev.grow(m, (size_t)num_blocks * 3, (size_t)num_blocks * 3));
-  NVB_CUDA(cudaMemcpyAsync(xyz_dev.get(), v.data(), (size_t)num_blocks * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
-  return freespaceUpdateImpl(m, xyz_dev.get(), num_blocks, update_time_ms, depth, depth_memory, rows, cols, T_L_C, cam,
+  CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
+  const int* xyz_dev;
+  NVB_CUDA(host.in(&v[0].x, (size_t)num_blocks * 3 * sizeof(int), &xyz_dev));
+  return freespaceUpdateImpl(m, xyz_dev, num_blocks, update_time_ms, depth, depth_memory, rows, cols, T_L_C, cam,
                              max_view_distance_m, truncation_distance_m);
 }
 
@@ -1930,7 +1991,7 @@ int32_t nvb_view_raycast(NvbMapper* m, const float* depth, int32_t depth_memory,
                          const float* T_L_C, const NvbCamera* cam, float block_size,
                          float max_integration_distance_behind_surface_m, float max_integration_distance_m,
                          int32_t* out_xyz_host, int32_t cap, int32_t* out_count) {
-  int rc = validateFrameArgs(m, depth, rows, cols, T_L_C, cam);
+  int rc = validateFrameArgs(m, depth, depth_memory, rows, cols, T_L_C, cam);
   if (rc) return rc;
   if (!(block_size > 0.0f)) return fail(NVB_ERR_INVALID_ARGUMENT, "block_size must be > 0");
   NVB_CUDA(cudaSetDevice(m->device));
@@ -1943,7 +2004,7 @@ int32_t nvb_view_raycast(NvbMapper* m, const float* depth, int32_t depth_memory,
 int32_t nvb_mapper_integrate_depth_async(NvbMapper* m, const float* depth, const uint8_t* mask, int32_t mask_mode,
                                          int32_t memory, int32_t rows, int32_t cols, const float* T_L_C,
                                          const NvbCamera* cam) {
-  int rc = validateFrameArgs(m, depth, rows, cols, T_L_C, cam);
+  int rc = validateFrameArgs(m, depth, memory, rows, cols, T_L_C, cam);
   if (rc) return rc;
   NVB_CUDA(cudaSetDevice(m->device));
   // max_integration_distance_behind_surface_m = truncation_distance_vox * voxel_size
@@ -2103,11 +2164,6 @@ int fillTracerArgs(NvbMapper* m, ColorArgs* a, const float* T_L_C_cm, const NvbC
   return NVB_OK;
 }
 
-int stageBytes(NvbMapper* m, DeviceArray<unsigned char>* buf, const unsigned char* host, size_t bytes) {
-  NVB_CUDA(buf->grow(m, bytes, bytes));
-  NVB_CUDA(cudaMemcpyAsync(buf->get(), host, bytes, cudaMemcpyHostToDevice, m->stream));
-  return NVB_OK;
-}
 }  // namespace
 
 int32_t nvb_sphere_tracer_render_depth(NvbMapper* m, const float* T_L_C, const NvbCamera* cam, float truncation_distance_m,
@@ -2132,11 +2188,12 @@ int32_t nvb_mapper_integrate_color(NvbMapper* m, const uint8_t* color, const uin
   if (!m || !color || !T_L_C || !cam) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (rows <= 0 || cols <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "image must have positive size");
   if (!(cam->fu != 0.0f) || !(cam->fv != 0.0f)) return fail(NVB_ERR_INVALID_ARGUMENT, "camera focal length is zero");
+  int rc;
+  if ((rc = checkMemoryKind(memory))) return rc;
   if (out_count) *out_count = 0;
   // "Color is only integrated for Tsdf layers (not for occupancy)" (mapper_impl.h:118-119)
   if (m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
-  int rc;
   if ((rc = ensureColorLayer(m))) return rc;
   const float trunc_m = m->cp.truncation_distance_vox * m->voxel_size;
   ColorArgs a{};
@@ -2195,24 +2252,16 @@ int32_t nvb_mapper_integrate_color(NvbMapper* m, const uint8_t* color, const uin
   a.depth_subsample = rows / a.drows;  // projective_integrator_impl.cuh:320
   if (a.depth_subsample <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "the colour image is smaller than the synthetic depth image");
   a.mask_mode = mask_mode;
-  if (memory == NVB_MEM_HOST) {
-    if ((rc = stageBytes(m, &m->color_stage, color, (size_t)rows * cols * 3))) return rc;
-    a.color_image = m->color_stage.get();
-    a.mask = nullptr;
-    if (mask) {
-      if ((rc = stageBytes(m, &m->color_mask_stage, mask, (size_t)rows * cols))) return rc;
-      a.mask = m->color_mask_stage.get();
-    }
-  } else {
-    a.color_image = color, a.mask = mask;
-  }
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  NVB_CUDA(bufs.in(color, (size_t)rows * cols * 3, &a.color_image));
+  NVB_CUDA(bufs.in(mask, (size_t)rows * cols, &a.mask));
   NVB_CUDA(cudaMemsetAsync(a.work_count, 0, sizeof(int), m->stream));
   launchColorSelect(a, m->num_sms, m->stream);
   launchSphereTrace(a, m->stream);
   launchColorIntegrate(a, m->num_sms, m->stream);
   m->launches += 3;
   // Device-resident frames with no output requested stay asynchronous (read the list later with
-  // nvb_mapper_last_color_blocks); host buffers must be released and outputs filled, so those calls synchronise.
+  // nvb_mapper_last_color_blocks); host-memory frames and requested outputs return with the frame integrated.
   if (memory == NVB_MEM_DEVICE && !updated_xyz_host && !out_count) return NVB_OK;
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   int rc2 = nvb_mapper_last_color_blocks(m, updated_xyz_host, cap, out_count);
@@ -2523,24 +2572,20 @@ int32_t nvb_ransac_fit_plane(NvbMapper* m, const float* points, int32_t memory, 
                              float ransac_distance_threshold_m, float plane[4], int32_t* found) {
   if (!m || !plane || !found) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (n < 0 || (n > 0 && !points)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad point list");
-  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  int rc;
+  if ((rc = checkMemoryKind(memory))) return rc;
   if (num_ransac_iterations < 1) return fail(NVB_ERR_INVALID_ARGUMENT, "num_ransac_iterations must be >= 1");
   *found = 0;
   if (n < 3) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   const size_t points_n = n;
   NVB_CUDA(m->gp_fit_points.grow(m, points_n, std::max(points_n, 2 * m->gp_fit_points.size())));
-  const float* src = points;
-  if (memory == NVB_MEM_HOST) {
-    // staged on the device for the packing kernel, in a buffer kept by the mapper
-    NVB_CUDA(m->gp_fit_stage.grow(m, 3 * points_n, std::max(3 * points_n, 2 * m->gp_fit_stage.size())));
-    NVB_CUDA(cudaMemcpyAsync(m->gp_fit_stage.get(), points, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    src = m->gp_fit_stage.get();
-  }
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  const float* src;
+  NVB_CUDA(bufs.in(points, points_n * 3 * sizeof(float), &src));
   launchPackPoints(src, n, m->gp_fit_points.get(), m->stream);
   m->launches++;
   int f = 0;
-  int rc;
   if ((rc = ransacFit(m, m->gp_fit_points.get(), n, num_ransac_iterations, ransac_distance_threshold_m, plane, &f))) return rc;
   *found = f;
   return checkDeviceError(m);
@@ -2566,13 +2611,15 @@ int ensureDynamicsBuffers(NvbMapper* m, int pixels) {
   return NVB_OK;
 }
 
-int validMemory(int32_t memory) { return memory == NVB_MEM_HOST || memory == NVB_MEM_DEVICE; }
-
-// Copies `bytes` of a detector output to the caller's buffer; a host copy waits for it.
-int copyDynamicsOut(NvbMapper* m, void* out, const void* src, size_t bytes, int32_t memory) {
+// Copies `bytes` of one of the mapper's published outputs to the caller's `out` (in `memory`) on the mapper's stream; a
+// host copy waits for it.
+int copyToCaller(NvbMapper* m, void* out, const void* src, size_t bytes, int32_t memory) {
   if (!out || bytes == 0 || !src) return NVB_OK;
-  NVB_CUDA(cudaMemcpyAsync(out, src, bytes, memory == NVB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, m->stream));
-  if (memory == NVB_MEM_HOST) NVB_CUDA(cudaStreamSynchronize(m->stream));
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  void* dev;
+  NVB_CUDA(bufs.out(out, bytes, &dev));
+  NVB_CUDA(cudaMemcpyAsync(dev, src, bytes, cudaMemcpyDeviceToDevice, m->stream));
+  NVB_CUDA(bufs.finish());
   return NVB_OK;
 }
 }  // namespace
@@ -2581,11 +2628,10 @@ extern "C" {
 
 int32_t nvb_mapper_compute_dynamics(NvbMapper* m, const float* depth, int32_t memory, int32_t rows, int32_t cols,
                                     const float* T_L_C, const NvbCamera* cam) {
-  int rc = validateFrameArgs(m, depth, rows, cols, T_L_C, cam);
+  int rc = validateFrameArgs(m, depth, memory, rows, cols, T_L_C, cam);
   if (rc) return rc;
   if (m->projective_layer_type != NVB_PROJECTIVE_TSDF_WITH_FREESPACE)
     return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper has no freespace layer");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
   if ((long long)rows * cols > kMaxDynamicsPixels) return fail(NVB_ERR_INVALID_ARGUMENT, "depth image too large");
   NVB_CUDA(cudaSetDevice(m->device));
   const int pixels = rows * cols;
@@ -2611,7 +2657,7 @@ int32_t nvb_mapper_remove_small_components(NvbMapper* m, const uint8_t* mask_in,
                                            int32_t rows, int32_t cols, int32_t threshold) {
   if (!m || !mask_in || !mask_out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (rows <= 0 || cols <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "mask must have positive size");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   if ((long long)rows * cols > kMaxDynamicsPixels) return fail(NVB_ERR_INVALID_ARGUMENT, "mask too large");
   const int pixels = rows * cols;
   if (threshold <= 0) {  // "Simply copy the output if threshold is zero."
@@ -2632,41 +2678,34 @@ int32_t nvb_mapper_remove_small_components(NvbMapper* m, const uint8_t* mask_in,
   NVB_CUDA(m->cc_labels.grow(m, down, std::max(down, 2 * m->cc_labels.size())));
   NVB_CUDA(m->cc_sizes.grow(m, down, std::max(down, 2 * m->cc_sizes.size())));
   a.labels = m->cc_labels.get(), a.sizes = m->cc_sizes.get();
-  if (memory == NVB_MEM_HOST) {
-    NVB_CUDA(m->cc_stage.grow(m, pixels, pixels));
-    NVB_CUDA(cudaMemcpyAsync(m->cc_stage.get(), mask_in, (size_t)pixels, cudaMemcpyHostToDevice, m->stream));
-    a.in = m->cc_stage.get(), a.out = m->cc_stage.get();
-  } else {
-    a.in = mask_in, a.out = mask_out;
-  }
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  NVB_CUDA(bufs.in(mask_in, (size_t)pixels, &a.in));
+  NVB_CUDA(bufs.out(mask_out, (size_t)pixels, &a.out));
   launchRemoveSmallComponents(a, m->num_sms, m->stream);
   m->launches += a.drows > 0 && a.dcols > 0 ? 4 : 1;
-  if (memory == NVB_MEM_HOST) {
-    NVB_CUDA(cudaMemcpyAsync(mask_out, m->cc_stage.get(), (size_t)pixels, cudaMemcpyDeviceToHost, m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-  }
+  NVB_CUDA(bufs.finish());
   return NVB_OK;
 }
 
 int32_t nvb_mapper_dynamic_mask(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols) {
   if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   *rows = m->dyn_rows, *cols = m->dyn_cols;
   NVB_CUDA(cudaSetDevice(m->device));
-  return copyDynamicsOut(m, out, m->dyn_mask.get(), (size_t)m->dyn_rows * m->dyn_cols, memory);
+  return copyToCaller(m, out, m->dyn_mask.get(), (size_t)m->dyn_rows * m->dyn_cols, memory);
 }
 
 int32_t nvb_mapper_dynamic_overlay(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols) {
   if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   *rows = m->dyn_rows, *cols = m->dyn_cols;
   NVB_CUDA(cudaSetDevice(m->device));
-  return copyDynamicsOut(m, out, m->dyn_overlay.get(), (size_t)m->dyn_rows * m->dyn_cols * 3, memory);
+  return copyToCaller(m, out, m->dyn_overlay.get(), (size_t)m->dyn_rows * m->dyn_cols * 3, memory);
 }
 
 int32_t nvb_mapper_dynamic_points(NvbMapper* m, float* xyz, int32_t memory, int32_t cap, int32_t* out_count) {
   if (!m || !out_count) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   *out_count = 0;
   if (!m->dyn_totals.get()) return NVB_OK;  // never computed
   NVB_CUDA(cudaSetDevice(m->device));
@@ -2675,7 +2714,7 @@ int32_t nvb_mapper_dynamic_points(NvbMapper* m, float* xyz, int32_t memory, int3
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   *out_count = n;
   const int k = std::min(n, std::max(cap, 0));
-  return copyDynamicsOut(m, xyz, m->dyn_points.get(), (size_t)k * 3 * sizeof(float), memory);
+  return copyToCaller(m, xyz, m->dyn_points.get(), (size_t)k * 3 * sizeof(float), memory);
 }
 
 int32_t nvb_mapper_dynamics_device_buffers(NvbMapper* m, NvbDynamicsBuffers* out) {
@@ -2709,7 +2748,7 @@ int32_t nvb_mapper_split_depth_image(NvbMapper* m, const float* depth, int32_t d
                                      const float* T_CM_CD, const NvbCamera* depth_cam, const NvbCamera* mask_cam,
                                      const NvbImageMaskerParams* params, int32_t with_overlay) {
   if (!m || !depth || !mask || !T_CM_CD || !depth_cam || !mask_cam || !params) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   if (depth_rows <= 0 || depth_cols <= 0 || mask_rows <= 0 || mask_cols <= 0)
     return fail(NVB_ERR_INVALID_ARGUMENT, "images must have positive size");
   if (depth_rows != depth_cam->height || depth_cols != depth_cam->width)
@@ -2726,14 +2765,9 @@ int32_t nvb_mapper_split_depth_image(NvbMapper* m, const float* depth, int32_t d
   if (with_overlay) NVB_CUDA(m->msk_overlay.grow(m, 3 * n, 3 * n));
   NVB_CUDA(m->msk_min_depth.grow(m, mn, mn));
   MaskerArgs a{};
-  a.depth = depth, a.mask = mask;
-  if (memory == NVB_MEM_HOST) {
-    NVB_CUDA(m->msk_depth_stage.grow(m, n, n));
-    NVB_CUDA(m->msk_mask_stage.grow(m, mn, mn));
-    NVB_CUDA(cudaMemcpyAsync(m->msk_depth_stage.get(), depth, n * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-    NVB_CUDA(cudaMemcpyAsync(m->msk_mask_stage.get(), mask, mn, cudaMemcpyHostToDevice, m->stream));
-    a.depth = m->msk_depth_stage.get(), a.mask = m->msk_mask_stage.get();
-  }
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);  // released behind the split: the call does not synchronise
+  NVB_CUDA(bufs.in(depth, n * sizeof(float), &a.depth));
+  NVB_CUDA(bufs.in(mask, mn, &a.mask));
   a.rows = depth_rows, a.cols = depth_cols, a.mrows = mask_rows, a.mcols = mask_cols;
   a.T_CM_CD = rigidFromColMajor(T_CM_CD);
   a.depth_cam = *depth_cam, a.mask_cam = *mask_cam;
@@ -2752,7 +2786,7 @@ int32_t nvb_mapper_split_depth_image(NvbMapper* m, const float* depth, int32_t d
 
 int32_t nvb_mapper_split_output(NvbMapper* m, int32_t which, void* out, int32_t memory, int32_t* rows, int32_t* cols) {
   if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   const size_t n = (size_t)m->msk_rows * m->msk_cols;
   const void* src;
   size_t bytes;
@@ -2762,7 +2796,7 @@ int32_t nvb_mapper_split_output(NvbMapper* m, int32_t which, void* out, int32_t 
   else return fail(NVB_ERR_INVALID_ARGUMENT, "bad split output");
   *rows = bytes ? m->msk_rows : 0, *cols = bytes ? m->msk_cols : 0;
   NVB_CUDA(cudaSetDevice(m->device));
-  return copyDynamicsOut(m, out, src, bytes, memory);
+  return copyToCaller(m, out, src, bytes, memory);
 }
 
 int32_t nvb_mapper_split_device_buffers(NvbMapper* m, NvbSplitBuffers* out) {
@@ -2776,31 +2810,23 @@ int32_t nvb_mapper_split_device_buffers(NvbMapper* m, NvbSplitBuffers* out) {
 int32_t nvb_mapper_split_color_image(NvbMapper* m, const uint8_t* rgb, const uint8_t* mask, int32_t memory, int32_t rows,
                                      int32_t cols, uint8_t* unmasked_out, uint8_t* masked_out, uint8_t* overlay_out) {
   if (!m || !rgb || !mask || !unmasked_out || !masked_out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   if (rows <= 0 || cols <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "image must have positive size");
   if ((long long)rows * cols > kMaxDynamicsPixels) return fail(NVB_ERR_INVALID_ARGUMENT, "image too large");
   NVB_CUDA(cudaSetDevice(m->device));
   const size_t n = (size_t)rows * cols;
   ColorSplitArgs a{};
   a.pixels = (long long)n;
-  a.rgb = rgb, a.mask = mask, a.unmasked = unmasked_out, a.masked = masked_out, a.overlay = overlay_out;
-  unsigned char* s = nullptr;
-  if (memory == NVB_MEM_HOST) {  // [rgb | mask | unmasked | masked | overlay]
-    NVB_CUDA(m->msk_color.grow(m, 13 * n, 13 * n));
-    s = m->msk_color.get();
-    NVB_CUDA(cudaMemcpyAsync(s, rgb, 3 * n, cudaMemcpyHostToDevice, m->stream));
-    NVB_CUDA(cudaMemcpyAsync(s + 3 * n, mask, n, cudaMemcpyHostToDevice, m->stream));
-    a.rgb = s, a.mask = s + 3 * n, a.unmasked = s + 4 * n, a.masked = s + 7 * n, a.overlay = overlay_out ? s + 10 * n : nullptr;
-  }
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  NVB_CUDA(bufs.in(rgb, 3 * n, &a.rgb));
+  NVB_CUDA(bufs.in(mask, n, &a.mask));
+  NVB_CUDA(bufs.out(unmasked_out, 3 * n, &a.unmasked));
+  NVB_CUDA(bufs.out(masked_out, 3 * n, &a.masked));
+  NVB_CUDA(bufs.out(overlay_out, 3 * n, &a.overlay));
   launchSplitColor(a, m->stream);
   NVB_CUDA(cudaGetLastError());
   m->launches++;
-  if (memory == NVB_MEM_HOST) {
-    NVB_CUDA(cudaMemcpyAsync(unmasked_out, a.unmasked, 3 * n, cudaMemcpyDeviceToHost, m->stream));
-    NVB_CUDA(cudaMemcpyAsync(masked_out, a.masked, 3 * n, cudaMemcpyDeviceToHost, m->stream));
-    if (overlay_out) NVB_CUDA(cudaMemcpyAsync(overlay_out, a.overlay, 3 * n, cudaMemcpyDeviceToHost, m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-  }
+  NVB_CUDA(bufs.finish());
   return NVB_OK;
 }
 
@@ -3121,17 +3147,16 @@ int32_t nvb_layer_get_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
   if (n <= 0) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
-  DeviceArray<int> xyz_dev;
-  DeviceArray<unsigned char> out_dev, found_dev;
-  NVB_CUDA(xyz_dev.grow(m, (size_t)n * 3, (size_t)n * 3));
-  NVB_CUDA(out_dev.grow(m, (size_t)n * L->block_bytes, (size_t)n * L->block_bytes));
-  NVB_CUDA(found_dev.grow(m, n, n));
-  NVB_CUDA(cudaMemcpyAsync(xyz_dev.get(), xyz_host, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  launchGatherBlocks(*L, xyz_dev.get(), n, out_dev.get(), found_dev.get(), m->stream);
+  std::vector<uint8_t> found_tmp(found_host ? 0 : n);  // the gather writes every block's flag
+  CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
+  const int* xyz_dev;
+  unsigned char *out_dev, *found_dev;
+  NVB_CUDA(host.in(xyz_host, (size_t)n * 3 * sizeof(int), &xyz_dev));
+  NVB_CUDA(host.out(static_cast<unsigned char*>(out_host), (size_t)n * L->block_bytes, &out_dev));
+  NVB_CUDA(host.out(found_host ? found_host : found_tmp.data(), (size_t)n, &found_dev));
+  launchGatherBlocks(*L, xyz_dev, n, out_dev, found_dev, m->stream);
   m->launches++;
-  NVB_CUDA(cudaMemcpyAsync(out_host, out_dev.get(), (size_t)n * L->block_bytes, cudaMemcpyDeviceToHost, m->stream));
-  if (found_host) NVB_CUDA(cudaMemcpyAsync(found_host, found_dev.get(), (size_t)n, cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(syncAll(m));
+  NVB_CUDA(host.finish());
   return NVB_OK;
 }
 
@@ -3155,13 +3180,12 @@ int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
   }
   L = layerOf(m, layer);
   NVB_CUDA(syncAll(m));
-  DeviceArray<int> xyz_dev;
-  DeviceArray<unsigned char> in_dev;
-  NVB_CUDA(xyz_dev.grow(m, (size_t)n * 3, (size_t)n * 3));
-  NVB_CUDA(in_dev.grow(m, (size_t)n * L->block_bytes, (size_t)n * L->block_bytes));
-  NVB_CUDA(cudaMemcpyAsync(xyz_dev.get(), xyz_host, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  NVB_CUDA(cudaMemcpyAsync(in_dev.get(), in_host, (size_t)n * L->block_bytes, cudaMemcpyHostToDevice, m->stream));
-  launchScatterBlocks(*L, xyz_dev.get(), n, in_dev.get(), m->error_dev, m->stream);
+  CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
+  const int* xyz_dev;
+  const unsigned char* in_dev;
+  NVB_CUDA(host.in(xyz_host, (size_t)n * 3 * sizeof(int), &xyz_dev));
+  NVB_CUDA(host.in(static_cast<const unsigned char*>(in_host), (size_t)n * L->block_bytes, &in_dev));
+  launchScatterBlocks(*L, xyz_dev, n, in_dev, m->error_dev, m->stream);
   m->launches++;
   if (layer == NVB_LAYER_ESDF) m->prune_ok = false;  // voxels written from outside: the parent boxes are no longer bounds
   NVB_CUDA(syncAll(m));
@@ -3316,7 +3340,7 @@ int32_t nvb_layer_export_points(NvbMapper* m, int32_t layer, int32_t memory, flo
   if (!m || !n) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (layer != NVB_LAYER_TSDF && layer != NVB_LAYER_OCCUPANCY && layer != NVB_LAYER_FREESPACE && layer != NVB_LAYER_ESDF)
     return fail(NVB_ERR_INVALID_ARGUMENT, "points are exported from a TSDF, occupancy, freespace or ESDF layer");
-  if (!validMemory(memory)) return fail(NVB_ERR_INVALID_ARGUMENT, "unknown memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   DevLayer* L = layerOf(m, layer);
   if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper does not hold that layer");
   NVB_CUDA(cudaSetDevice(m->device));
@@ -3349,14 +3373,12 @@ int32_t nvb_layer_export_points(NvbMapper* m, int32_t layer, int32_t memory, flo
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   *n = total;
   if (!xyzi || cap < total || total == 0) return NVB_OK;
-  DeviceArray<float4> staged;
-  if (memory == NVB_MEM_HOST) NVB_CUDA(staged.grow(m, total, total));
-  a.out = memory == NVB_MEM_HOST ? staged.get() : reinterpret_cast<float4*>(xyzi);
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  NVB_CUDA(bufs.out(reinterpret_cast<float4*>(xyzi), (size_t)total * sizeof(float4), &a.out));
   launchExportEmit(a, m->stream);
   m->launches++;
-  if (memory == NVB_MEM_HOST)
-    NVB_CUDA(cudaMemcpyAsync(xyzi, staged.get(), (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  NVB_CUDA(bufs.finish());
+  if (memory == NVB_MEM_DEVICE) NVB_CUDA(cudaStreamSynchronize(m->stream));
   return NVB_OK;
 }
 
@@ -3641,10 +3663,11 @@ int32_t nvb_mesh_block_sizes(NvbMapper* m, const int32_t* blocks_xyz_host, int32
   for (int i = 0; i < 3 * num_blocks; i++) sizes_out[i] = -1;
   if (!m->mesh.blocks) return NVB_OK;
   NVB_CUDA(syncAll(m));
-  DeviceArray<int> dev;  // headers[4n] (int4-aligned) | xyz[3n]
-  NVB_CUDA(dev.grow(m, (size_t)num_blocks * 7, (size_t)num_blocks * 7));
-  int* xyz_dev = dev.get() + 4 * (size_t)num_blocks;
-  NVB_CUDA(cudaMemcpy(xyz_dev, blocks_xyz_host, (size_t)num_blocks * 3 * sizeof(int), cudaMemcpyHostToDevice));
+  DeviceArray<int> dev;  // headers[4n] (int4-aligned)
+  NVB_CUDA(dev.grow(m, (size_t)num_blocks * 4, (size_t)num_blocks * 4));
+  CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
+  const int* xyz_dev;
+  NVB_CUDA(host.in(blocks_xyz_host, (size_t)num_blocks * 3 * sizeof(int), &xyz_dev));
   launchMeshHeaders(makeMeshCtx(m), xyz_dev, num_blocks, dev.get(), m->stream);
   std::vector<int> h((size_t)num_blocks * 4);
   NVB_CUDA(cudaMemcpyAsync(h.data(), dev.get(), h.size() * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
@@ -3661,11 +3684,13 @@ int32_t nvb_mesh_get_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   const size_t n = (size_t)num_blocks;
-  DeviceArray<int> dev;  // headers[4n] (int4-aligned) | xyz[3n] | dst[3n]
-  NVB_CUDA(dev.grow(m, n * 10, n * 10));
-  NVB_CUDA(cudaMemcpy(dev.get() + 4 * n, blocks_xyz_host, n * 3 * sizeof(int), cudaMemcpyHostToDevice));
+  DeviceArray<int> dev;  // headers[4n] (int4-aligned)
+  NVB_CUDA(dev.grow(m, n * 4, n * 4));
+  CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
+  const int *xyz_dev, *dst_dev;
+  NVB_CUDA(host.in(blocks_xyz_host, n * 3 * sizeof(int), &xyz_dev));
   MeshCtx c = makeMeshCtx(m);
-  launchMeshHeaders(c, dev.get() + 4 * n, num_blocks, dev.get(), m->stream);
+  launchMeshHeaders(c, xyz_dev, num_blocks, dev.get(), m->stream);
   std::vector<int> h(n * 4), dst(n * 3);
   NVB_CUDA(cudaMemcpyAsync(h.data(), dev.get(), h.size() * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
@@ -3684,8 +3709,8 @@ int32_t nvb_mesh_get_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_
   NVB_CUDA(pn.grow(m, std::max<size_t>(1, (size_t)tv * 3), std::max<size_t>(1, (size_t)tv * 3)));
   NVB_CUDA(pt.grow(m, std::max<size_t>(1, (size_t)tt), std::max<size_t>(1, (size_t)tt)));
   NVB_CUDA(pc.grow(m, std::max<size_t>(1, (size_t)tc * 4), std::max<size_t>(1, (size_t)tc * 4)));
-  NVB_CUDA(cudaMemcpyAsync(dev.get() + 7 * n, dst.data(), n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  launchMeshPack(c, dev.get(), dev.get() + 7 * n, num_blocks, pv.get(), pn.get(), pt.get(), pc.get(), m->num_sms, m->stream);
+  NVB_CUDA(host.in(dst.data(), n * 3 * sizeof(int), &dst_dev));
+  launchMeshPack(c, dev.get(), dst_dev, num_blocks, pv.get(), pn.get(), pt.get(), pc.get(), m->num_sms, m->stream);
   if (vertices_out && tv) NVB_CUDA(cudaMemcpyAsync(vertices_out, pv.get(), (size_t)tv * 12, cudaMemcpyDeviceToHost, m->stream));
   if (normals_out && tv) NVB_CUDA(cudaMemcpyAsync(normals_out, pn.get(), (size_t)tv * 12, cudaMemcpyDeviceToHost, m->stream));
   if (triangles_out && tt) NVB_CUDA(cudaMemcpyAsync(triangles_out, pt.get(), (size_t)tt * 4, cudaMemcpyDeviceToHost, m->stream));
@@ -3756,27 +3781,23 @@ template <typename Launch>
 int runLayerQuery(NvbMapper* m, const float* xyz, int32_t memory, long long n, void* out, size_t out_bytes_per_point,
                   uint8_t* flags, Launch launch) {
   NVB_CUDA(cudaSetDevice(m->device));
-  if (memory == NVB_MEM_DEVICE) return runOrdered(&m, 1, m->stream, [&](cudaStream_t st) { launch(xyz, out, flags, st); });
-  const size_t out_bytes = (size_t)n * out_bytes_per_point;
-  DeviceArray<float> xyz_dev;
-  DeviceArray<unsigned char> out_dev, flags_dev;
-  NVB_CUDA(xyz_dev.grow(m, (size_t)n * 3, (size_t)n * 3));
-  NVB_CUDA(out_dev.grow(m, out_bytes, out_bytes));
-  NVB_CUDA(flags_dev.grow(m, n, n));
-  NVB_CUDA(cudaMemcpyAsync(xyz_dev.get(), xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, m->stream));
-  // the caller's buffer goes down too: the outputs the kernel does not write come back unchanged
-  NVB_CUDA(cudaMemcpyAsync(out_dev.get(), out, out_bytes, cudaMemcpyHostToDevice, m->stream));
-  const int rc = runOrdered(&m, 1, m->stream, [&](cudaStream_t st) { launch(xyz_dev.get(), out_dev.get(), flags_dev.get(), st); });
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  const float* xyz_dev;
+  void* out_dev;
+  uint8_t* flags_dev;
+  NVB_CUDA(bufs.in(xyz, (size_t)n * 3 * sizeof(float), &xyz_dev));
+  // the outputs the kernel does not write come back unchanged
+  NVB_CUDA(bufs.out(out, (size_t)n * out_bytes_per_point, &out_dev, true));
+  NVB_CUDA(bufs.out(flags, (size_t)n, &flags_dev));
+  const int rc = runOrdered(&m, 1, m->stream, [&](cudaStream_t st) { launch(xyz_dev, out_dev, flags_dev, st); });
   if (rc) return rc;
-  NVB_CUDA(cudaMemcpyAsync(out, out_dev.get(), out_bytes, cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaMemcpyAsync(flags, flags_dev.get(), (size_t)n, cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  NVB_CUDA(bufs.finish());
   return NVB_OK;
 }
 
 int checkLayerQueryArgs(NvbMapper* m, const float* xyz, int32_t memory, int64_t n, const void* out, const void* flags) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
-  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   if (n < 0 || n > kMaxQueryPoints) return fail(NVB_ERR_INVALID_ARGUMENT, "bad number of query points");
   if (n > 0 && (!xyz || !out || !flags)) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   return NVB_OK;
@@ -3891,7 +3912,7 @@ int renderImpl(NvbMapper* m, const NvbSphereTracerParams* p, const float* T_L_C,
     return fail(NVB_ERR_INVALID_ARGUMENT, "the sphere tracer needs a TSDF layer");
   if (p->maximum_steps <= 0 || !(p->maximum_ray_length_m > 0.0f) || !(p->surface_distance_epsilon_vox > 0.0f))
     return fail(NVB_ERR_INVALID_ARGUMENT, "sphere tracer parameter out of range");  // CHECK_GT, sphere_tracer.cu:319-333
-  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if (int rc = checkMemoryKind(memory)) return rc;
   if (cam->width <= 0 || cam->height <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "the camera must have a positive size");
   if (f <= 0 || cam->width % f != 0 || cam->height % f != 0)
     return fail(NVB_ERR_INVALID_ARGUMENT, "the ray subsampling factor must divide the image size");  // CHECK_EQ, :432-433
@@ -3911,20 +3932,12 @@ int renderImpl(NvbMapper* m, const NvbSphereTracerParams* p, const float* T_L_C,
   a.drows = cam->height / f, a.dcols = cam->width / f;  // getSubsampledImageSize (:335-339)
   const size_t n = (size_t)a.drows * a.dcols;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  DeviceArray<float> depth_dev;
-  DeviceArray<unsigned char> rgb_dev;
-  if (memory == NVB_MEM_DEVICE) {
-    a.depth = out_depth, a.rgb = out_rgb;
-  } else {
-    NVB_CUDA(depth_dev.grow(m, n, n));
-    if (out_rgb) NVB_CUDA(rgb_dev.grow(m, 3 * n, 3 * n));
-    a.depth = depth_dev.get(), a.rgb = out_rgb ? rgb_dev.get() : nullptr;
-  }
+  CallerBuffers bufs(memory, st, m->stage_pool);
+  NVB_CUDA(bufs.out(out_depth, n * sizeof(float), &a.depth));
+  NVB_CUDA(bufs.out(out_rgb, 3 * n, &a.rgb));
   const int rc = runOrdered(&m, 1, st, [&](cudaStream_t s) { launchRender(a, s); });
-  if (rc || memory == NVB_MEM_DEVICE) return rc;
-  NVB_CUDA(cudaMemcpyAsync(out_depth, a.depth, n * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (out_rgb) NVB_CUDA(cudaMemcpyAsync(out_rgb, a.rgb, 3 * n, cudaMemcpyDeviceToHost, st));
-  NVB_CUDA(cudaStreamSynchronize(st));
+  if (rc) return rc;
+  NVB_CUDA(bufs.finish());
   return NVB_OK;
 }
 
@@ -3976,25 +3989,11 @@ int validateScene(const NvbScene* s) {
   return NVB_OK;
 }
 
-// The scene with its primitives copied into stream-ordered device memory, released (stream-ordered) by the destructor: the
-// copy and the free are enqueued on the stream after the caller's work, and the host does not wait for either.
-struct DeviceScene {
-  NvbScene s{};
-  cudaStream_t st = nullptr;
-  ~DeviceScene() {
-    if (s.primitives) cudaFreeAsync(const_cast<NvbPrimitive*>(s.primitives), st);
-  }
-  cudaError_t upload(const NvbScene& host, cudaStream_t stream) {
-    s = host, s.primitives = nullptr, st = stream;
-    if (host.num_primitives == 0) return cudaSuccess;
-    const size_t bytes = (size_t)host.num_primitives * sizeof(NvbPrimitive);
-    NvbPrimitive* d = nullptr;
-    cudaError_t e = cudaMallocAsync(&d, bytes, stream);
-    if (e != cudaSuccess) return e;
-    s.primitives = d;
-    return cudaMemcpyAsync(d, host.primitives, bytes, cudaMemcpyHostToDevice, stream);
-  }
-};
+// The scene with its primitives staged on the device by `host`, a CallerBuffers of host memory.
+cudaError_t deviceScene(const NvbScene& scene, CallerBuffers* host, NvbScene* out) {
+  *out = scene;
+  return host->in(scene.primitives, (size_t)scene.num_primitives * sizeof(NvbPrimitive), &out->primitives);
+}
 
 int deviceSms() {
   int dev = 0, sms = kHelperCtas;
@@ -4036,9 +4035,8 @@ int generateLayerImpl(NvbMapper* m, DevLayer* L, int layer_id, const NvbScene* s
   }
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(joinEsdf(m));  // an update_esdf_async may still be reading the layer
-  DeviceScene ds;
-  NVB_CUDA(ds.upload(*scene, m->stream));
-  a.scene = ds.s;
+  CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
+  NVB_CUDA(deviceScene(*scene, &host, &a.scene));
   a.layer = *L;
   a.layer_id = layer_id;
   a.block_size = m->block_size;
@@ -4112,7 +4110,7 @@ int32_t nvb_scene_render_depth(const NvbScene* scene, const NvbCamera* cam, cons
   int rc;
   if ((rc = validateScene(scene))) return rc;
   if (!cam || !T_S_C || !out_depth) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if ((rc = checkMemoryKind(memory))) return rc;
   if (cam->width <= 0 || cam->height <= 0) return fail(NVB_ERR_INVALID_ARGUMENT, "the camera must have a positive size");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   SceneDepthArgs a{};
@@ -4121,24 +4119,12 @@ int32_t nvb_scene_render_depth(const NvbScene* scene, const NvbCamera* cam, cons
   a.T_C_S = invertRigid(a.T_S_C);
   a.max_dist = max_dist, a.invalid_depth = invalid_depth;
   a.rows = cam->height, a.cols = cam->width;
-  const size_t n = (size_t)a.rows * a.cols;
-  float* staged = nullptr;
-  if (memory == NVB_MEM_HOST) NVB_CUDA(cudaMallocAsync(&staged, n * sizeof(float), st));
-  a.depth = memory == NVB_MEM_HOST ? staged : out_depth;
-  cudaError_t e;
-  {
-    DeviceScene ds;
-    e = ds.upload(*scene, st);
-    a.scene = ds.s;
-    if (e == cudaSuccess) {
-      launchSceneDepth(a, st);
-      e = cudaGetLastError();
-    }
-  }
-  if (e == cudaSuccess && staged) e = cudaMemcpyAsync(out_depth, staged, n * sizeof(float), cudaMemcpyDeviceToHost, st);
-  if (staged) cudaFreeAsync(staged, st);
-  if (e == cudaSuccess && staged) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) return fail(NVB_ERR_CUDA, std::string("nvb_scene_render_depth: ") + cudaGetErrorString(e));
+  CallerBuffers host(NVB_MEM_HOST, st, nullptr), bufs(memory, st, nullptr);  // no mapper: the device's default pool
+  NVB_CUDA(deviceScene(*scene, &host, &a.scene));
+  NVB_CUDA(bufs.out(out_depth, (size_t)a.rows * a.cols * sizeof(float), &a.depth));
+  launchSceneDepth(a, st);
+  NVB_CUDA(cudaGetLastError());
+  NVB_CUDA(bufs.finish());
   return NVB_OK;
 }
 
@@ -4147,30 +4133,19 @@ int32_t nvb_scene_signed_distance(const NvbScene* scene, const float* xyz, int32
   int rc;
   if ((rc = validateScene(scene))) return rc;
   if (n < 0 || (n > 0 && (!xyz || !out))) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (memory != NVB_MEM_HOST && memory != NVB_MEM_DEVICE) return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
+  if ((rc = checkMemoryKind(memory))) return rc;
   if (n == 0) return NVB_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const float* in_dev = xyz;
-  float* out_dev = out;
-  float* staged = nullptr;  // host memory: 3 n input floats, then n outputs
-  cudaError_t e = cudaSuccess;
-  if (memory == NVB_MEM_HOST) {
-    NVB_CUDA(cudaMallocAsync(&staged, (size_t)n * 4 * sizeof(float), st));
-    in_dev = staged, out_dev = staged + 3 * n;
-    e = cudaMemcpyAsync(staged, xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, st);
-  }
-  {
-    DeviceScene ds;
-    if (e == cudaSuccess) e = ds.upload(*scene, st);
-    if (e == cudaSuccess) {
-      launchSceneDistance(ds.s, in_dev, n, max_dist, out_dev, deviceSms(), st);
-      e = cudaGetLastError();
-    }
-  }
-  if (e == cudaSuccess && staged) e = cudaMemcpyAsync(out, out_dev, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, st);
-  if (staged) cudaFreeAsync(staged, st);
-  if (e == cudaSuccess && staged) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) return fail(NVB_ERR_CUDA, std::string("nvb_scene_signed_distance: ") + cudaGetErrorString(e));
+  CallerBuffers host(NVB_MEM_HOST, st, nullptr), bufs(memory, st, nullptr);  // no mapper: the device's default pool
+  NvbScene s;
+  const float* in_dev;
+  float* out_dev;
+  NVB_CUDA(deviceScene(*scene, &host, &s));
+  NVB_CUDA(bufs.in(xyz, (size_t)n * 3 * sizeof(float), &in_dev));
+  NVB_CUDA(bufs.out(out, (size_t)n * sizeof(float), &out_dev));
+  launchSceneDistance(s, in_dev, n, max_dist, out_dev, deviceSms(), st);
+  NVB_CUDA(cudaGetLastError());
+  NVB_CUDA(bufs.finish());
   return NVB_OK;
 }
 

@@ -191,14 +191,23 @@ def test_argument_checks(gpu):
     from isaac_ros_nvblox_b200 import _lib
     m = _mapper()
     masker = nvb.ImageMasker(m)
+    import torch
     d, mk = np.ones((4, 6), np.float32), np.ones((4, 6), np.uint8)
     cam = nvb.Camera(5.0, 5.0, 3.0, 2.0, 6, 4)
+    # device buffers for the kind 2 cases: a call that took the kind for device memory would succeed on them
+    td, tb = torch.ones((4, 6), dtype=torch.float32, device="cuda"), torch.ones((4, 6, 3), dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    r, c = C.c_int32(0), C.c_int32(0)
     bad = [
         lambda: masker.split_depth(np.ones((4, 5), np.float32), mk, I4, cam, cam),       # depth size != depth camera
         lambda: masker.split_depth(d, np.ones((5, 6), np.uint8), I4, cam, cam),            # mask size != mask camera
         lambda: masker.split_depth(np.ones((0, 6), np.float32), mk, I4, nvb.Camera(5, 5, 3, 2, 6, 0), cam),  # empty
         lambda: masker.split_depth(d, np.ones((0, 6), np.uint8), I4, cam, nvb.Camera(5, 5, 3, 2, 6, 0)),
         lambda: masker._split(d.ctypes.data, 4, 6, mk.ctypes.data, 4, 6, 7, I4, cam, cam, False),  # memory kind
+        lambda: masker._split(td.data_ptr(), 4, 6, tb.data_ptr(), 4, 6, 2, I4, cam, cam, False),
+        lambda: _lib.check(m._L.nvb_mapper_split_output(m._h, _lib.NVB_SPLIT_BACKGROUND, td.data_ptr(), 2, C.byref(r), C.byref(c))),
+        lambda: _lib.check(m._L.nvb_mapper_split_color_image(m._h, tb.data_ptr(), tb.data_ptr(), 2, 4, 6, tb.data_ptr(), tb.data_ptr(),
+                                                             None)),
         lambda: masker._split(None, 4, 6, mk.ctypes.data, 4, 6, _lib.NVB_MEM_HOST, I4, cam, cam, False),
         lambda: masker._split(d.ctypes.data, 4, 6, None, 4, 6, _lib.NVB_MEM_HOST, I4, cam, cam, False),
         lambda: masker._split(d.ctypes.data, 1 << 15, 1 << 14, mk.ctypes.data, 4, 6, _lib.NVB_MEM_HOST, I4,

@@ -309,6 +309,11 @@ def test_argument_errors(gpu):
     assert L.nvb_render_rgbd(m._h, C.byref(p), T, C.byref(cam.c), 0.4, 1, H, None, c.ctypes.data, None) == bad
     assert L.nvb_render_depth(m._h, None, T, C.byref(cam.c), 0.4, 1, H, d.ctypes.data, None) == bad
     assert L.nvb_render_depth(m._h, C.byref(p), T, C.byref(cam.c), 0.4, 1, 7, d.ctypes.data, None) == bad  # memory kind
+    import torch
+    td, tc = torch.zeros((240, 320), dtype=torch.float32, device="cuda"), torch.zeros((240, 320, 3), dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    assert L.nvb_render_depth(m._h, C.byref(p), T, C.byref(cam.c), 0.4, 1, 2, td.data_ptr(), None) == bad
+    assert L.nvb_render_rgbd(m._h, C.byref(p), T, C.byref(cam.c), 0.4, 1, 2, td.data_ptr(), tc.data_ptr(), None) == bad
     occ = nvb.Mapper(0.1, projective_layer_type=nvb.ProjectiveLayerType.kOccupancy)
     assert L.nvb_render_depth(occ._h, C.byref(p), T, C.byref(cam.c), 0.4, 1, H, d.ctypes.data, None) == bad
     assert L.nvb_render_rgbd(occ._h, C.byref(p), T, C.byref(cam.c), 0.4, 1, H, d.ctypes.data, c.ctypes.data, None) == bad

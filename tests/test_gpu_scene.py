@@ -452,6 +452,11 @@ def test_invalid_arguments(gpu):
     assert L.nvb_scene_signed_distance(C.byref(good), None, H, 4, 1.0, d.ctypes.data, None) == bad
     assert L.nvb_scene_signed_distance(C.byref(good), xyz.ctypes.data, 9, 4, 1.0, d.ctypes.data, None) == bad
     assert L.nvb_scene_signed_distance(C.byref(bad_normal), xyz.ctypes.data, H, 4, 1.0, d.ctypes.data, None) == bad
+    import torch
+    tx, td = torch.zeros((24, 32), dtype=torch.float32, device="cuda"), torch.zeros((24, 32), dtype=torch.float32, device="cuda")
+    torch.cuda.synchronize()
+    assert L.nvb_scene_render_depth(C.byref(good), C.byref(cam.c), fp, 5.0, 0.0, 2, td.data_ptr(), None) == bad
+    assert L.nvb_scene_signed_distance(C.byref(good), tx.data_ptr(), 2, 4, 1.0, td.data_ptr(), None) == bad
     m = nvb.Mapper(0.1)
     for lid in (lib.NVB_LAYER_ESDF, lib.NVB_LAYER_COLOR, lib.NVB_LAYER_FREESPACE, lib.NVB_LAYER_OCCUPANCY, 42):
         assert L.nvb_scene_generate_layer(m._h, lid, C.byref(good), 0.4) == bad, lid
