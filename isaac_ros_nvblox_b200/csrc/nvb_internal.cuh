@@ -837,7 +837,7 @@ struct MapFileLayerOut {
   int block_bytes;
 };
 struct PinnedFree {
-  void operator()(unsigned char* p) const { cudaFreeHost(p); }
+  void operator()(void* p) const { cudaFreeHost(p); }
 };
 // One layer read: present = the file has its tables; n blocks in (x, y, z) order, their voxels in pinned memory.
 struct MapFileLayerIn {

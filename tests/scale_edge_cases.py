@@ -169,14 +169,14 @@ def far_parent_voxels(esdf_layer):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# Deallocation, slot reuse and slab growth (nvb_api.cu nvb_mapper_decay / ensureTsdfCapacity / growLayer, nvb_util.cu
+# Deallocation, slot reuse and slab growth (nvb_api.cu nvb_mapper_decay / ensureTsdfCapacity / LayerSlab::grow, nvb_util.cu
 # removeBlocksKernel, nvb_esdf.cu esdfRemoveBlocksKernel, nvb_internal.cuh hashFindOrInsert):
 #   * REMOVE_GRID: the remove kernels launch at most 1184 CTAs, one dead block per CTA and round; more dead blocks than
 #     that take several rounds;
 #   * a frame that allocates more new blocks than the free stack holds empties the stack inside one allocation launch
 #     (atomicSub below zero, atomicAdd back) and continues with fresh slots;
-#   * a frame whose view AABB does not fit behind the slab's high-water mark doubles the slab (growLayer copies the free
-#     stack and rehashes up to the high-water mark), here while the stack is not empty.
+#   * a frame whose view AABB does not fit behind the slab's high-water mark doubles the slab (LayerSlab::grow copies the
+#     free stack and rehashes up to the high-water mark), here while the stack is not empty.
 # The churn sequence: 2 cm voxels, three frames at a 4 m range, a decay that removes everything outside a sphere, then one
 # frame at a 7 m range (its view AABB is ~5x larger than the 4 m frames').
 # ---------------------------------------------------------------------------------------------------------------------

@@ -161,7 +161,7 @@ def test_redwood_shape_2cm_full_size_equals_oracle(gpu):
 
 @pytest.mark.parametrize("mode", [1, 3])
 def test_async_pipeline_with_layer_growth_mid_sequence(c2, mode):
-    """A slab that is too small forces growLayer (a synchronising reallocation of both layers and of the ESDF scratch)
+    """A slab that is too small forces LayerSlab::grow (a synchronising reallocation of both layers and of the ESDF scratch)
     while wavefronts of earlier frames are in flight on the side stream."""
     nvb = _nvb()
     frames = c2["frames"][:24]

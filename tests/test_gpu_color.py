@@ -4,9 +4,10 @@ synthetic depth images. The reference's own colour-test scenes are replayed on t
 import numpy as np
 import pytest
 
-from helpers import (assert_color_equal, cameras, points_on_a_sphere, rotation_y, sphere_scene_tsdf_layer, spheres_distance,
-                     textured_image, tsdf_layer_from_distance, voxel_at_position)
+from helpers import (assert_color_equal, assert_tsdf_equal, cameras, points_on_a_sphere, rotation_y, sphere_scene_tsdf_layer,
+                     spheres_distance, textured_image, tsdf_layer_from_distance, voxel_at_position)
 from isaac_ros_nvblox_b200 import synthetic as syn
+from test_gpu_mesh import assert_mesh_equal
 
 pytestmark = pytest.mark.gpu
 
@@ -166,8 +167,21 @@ def test_color_layer_follows_decay_and_occupancy_mapper_ignores_color(gpu):
         m.integrate_depth(d, T, cam), o.integrate_depth(d, T, ocam)
         m.integrate_color(_solid(BLUE, 240, 320), T, cam), o.integrate_color(_solid(BLUE, 240, 320), T, ocam)
     assert_color_equal(m.color_layer().as_dict(), o.color_layer())
+    m.update_mesh()
+    assert m.mesh_layer().num_blocks() > 0
     m.clear()
-    assert m.color_layer().num_blocks() == 0
+    assert m.color_layer().num_blocks() == 0 and m.mesh_layer().num_blocks() == 0
+    # the cleared colour and mesh layers take a new map as a fresh mapper would
+    o = orc.OracleMap(0.1)
+    for d, T in frames:
+        m.integrate_depth(d, T, cam), o.integrate_depth(d, T, ocam)
+        m.integrate_color(_solid(RED, 240, 320), T, cam), o.integrate_color(_solid(RED, 240, 320), T, ocam)
+    m.update_mesh()
+    o.integrate_mesh()
+    o.update_mesh_color()
+    assert_tsdf_equal(m.tsdf_layer().as_dict(), o.tsdf_layer())
+    assert_color_equal(m.color_layer().as_dict(), o.color_layer())
+    assert_mesh_equal(m.mesh_layer().as_dict(), o.mesh_layer(), colors=True)
     m.close()
     mo = nvb.Mapper(0.1, projective_layer_type=nvb.ProjectiveLayerType.kOccupancy)
     d, T = frames[0]
