@@ -143,6 +143,90 @@ class LayerSlab {
   DevLayer d_{};
 };
 
+// Upper bounds of the slabs' fill levels, kept on the host so that the frame path never waits for a count (DESIGN.md §5).
+// The projective bound is the last count seen plus the cells added since; each frame reads the count back into a ring of
+// pinned slots, and the newest read-back that has landed tightens the bound. The blocks the ESDF slab and the slabs that
+// follow the projective slab (colour, mesh, freespace) may hold beyond the projective fill level are counted apart.
+class SlabBounds {
+ public:
+  ~SlabBounds() {
+    for (cudaEvent_t e : count_events_)
+      if (e) cudaEventDestroy(e);
+  }
+  int create();  // the read-back ring
+
+  // The projective bound for a launch over the projective slab's blocks: tightened, at most the slab's capacity.
+  int projectiveUpper(int capacity) {
+    for (int k = 0; k < kCountRing; k++) {
+      if (count_pending_[k] && cudaEventQuery(count_events_[k]) == cudaSuccess) {
+        count_pending_[k] = false;
+        if (count_cum_at_[k] > confirmed_cum_) {
+          confirmed_cum_ = count_cum_at_[k];
+          tsdf_count_confirmed_ = h_count_ring_[k];
+        }
+      }
+    }
+    tsdf_count_ub_ = clampToInt(tsdf_count_confirmed_ + (cells_cum_ - confirmed_cum_));
+    return std::min(tsdf_count_ub_, capacity);
+  }
+  // The slots the projective slab needs to take `cells` more blocks, and those the ESDF slab needs.
+  long long projectiveNeed(long long cells) { return (long long)projectiveUpper(0x7fffffff) + derived_extra_ub_ + cells; }
+  long long esdfNeed(int projective_capacity) const {
+    return (long long)std::min(tsdf_count_ub_, projective_capacity) + esdf_extra_ub_;
+  }
+  void add(long long projective, int esdf_extra, int derived_extra) {
+    cells_cum_ += projective;
+    tsdf_count_ub_ = clampToInt(tsdf_count_ub_ + projective);
+    esdf_extra_ub_ = clampToInt((long long)esdf_extra_ub_ + esdf_extra);
+    derived_extra_ub_ = clampToInt((long long)derived_extra_ub_ + derived_extra);
+  }
+  // After a frame's kernels on `st`: its cells join the bound, and the projective `count` is read back behind them.
+  int recordFrame(const int* count, long long cells, cudaStream_t st) {
+    cells_cum_ += cells;
+    const int k = count_ring_head_;
+    if (!count_pending_[k]) {
+      count_ring_head_ = (k + 1) % kCountRing;
+      NVB_CUDA(cudaMemcpyAsync(&h_count_ring_[k], count, sizeof(int), cudaMemcpyDeviceToHost, st));
+      NVB_CUDA(cudaEventRecord(count_events_[k], st));
+      count_pending_[k] = true;
+      count_cum_at_[k] = cells_cum_;
+    }
+    tsdf_count_ub_ = clampToInt(tsdf_count_ub_ + cells);
+    return NVB_OK;
+  }
+  // A projective count read with nothing in flight, and the ESDF's and derived slabs' blocks beyond it.
+  void reset(int projective, int esdf_extra, int derived_extra) {
+    for (bool& p : count_pending_) p = false;
+    tsdf_count_confirmed_ = tsdf_count_ub_ = projective;
+    confirmed_cum_ = cells_cum_;
+    esdf_extra_ub_ = esdf_extra, derived_extra_ub_ = derived_extra;
+  }
+  void confirm(int projective) { reset(projective, esdf_extra_ub_, derived_extra_ub_); }
+  // The explicit-list entry points are synchronous: afterwards the real fill level of the ESDF slab is known and replaces
+  // the running sum of list lengths (which would otherwise grow the slab without need in a long session).
+  int tightenEsdfBound(const LayerSlab& esdf, int projective_capacity) {
+    int count = 0;
+    NVB_CUDA(esdf.fillLevel(&count));
+    esdf_extra_ub_ = std::max(0, count - std::min(tsdf_count_ub_, projective_capacity));
+    return NVB_OK;
+  }
+
+ private:
+  static int clampToInt(long long v) { return (int)std::min<long long>(v, 0x7fffffff); }
+
+  int tsdf_count_ub_ = 0;
+  int esdf_extra_ub_ = 0;     // blocks submitted to the ESDF through explicit lists
+  int derived_extra_ub_ = 0;  // written to a derived slab, or kept there when nvb_scene_to_mapper replaced the projective layer
+  std::unique_ptr<int[], PinnedFree> h_count_ring_;
+  cudaEvent_t count_events_[kCountRing] = {};
+  bool count_pending_[kCountRing] = {};
+  long long count_cum_at_[kCountRing] = {};  // cells_cum_ when the read-back was enqueued
+  int count_ring_head_ = 0;
+  int tsdf_count_confirmed_ = 0;  // last projective count seen by the host ...
+  long long confirmed_cum_ = 0;   // ... and cells_cum_ at that moment
+  long long cells_cum_ = 0;       // cells added to the bound so far
+};
+
 // A caller's buffers are host or device memory (NvbMemory); any other kind is rejected before anything is enqueued.
 int checkMemoryKind(int32_t memory) {
   if (memory == NVB_MEM_HOST || memory == NVB_MEM_DEVICE) return NVB_OK;
@@ -260,11 +344,7 @@ struct NvbMapper {
   DeviceArray<int> cols;
   long long fs_last_update_ms = 0;  // FreespaceIntegrator::last_update_time_ms_ (freespace_integrator.h:171)
   DeviceArray<int4> fs_work;
-  int tsdf_count_ub = 0;   // host-side upper bound of *tsdf.count
-  int esdf_extra_ub = 0;   // blocks submitted to the ESDF through explicit lists
-  // Blocks the colour, mesh and freespace layers may hold beyond the projective layer's fill level: those of a projective
-  // layer that nvb_scene_to_mapper replaced. These layers are sized to the projective slab's capacity, so it keeps room for them.
-  int derived_extra_ub = 0;
+  SlabBounds bounds;
 
   DeviceArray<int4> union_list;  // nvb_blocks_union's own output list
   DeviceArray<int> union_list_count;
@@ -423,14 +503,6 @@ struct NvbMapper {
   std::unique_ptr<int[], PinnedFree> h_ints;  // [0] frame count, [1] error, [2..] misc, [8], [9] prefetched error words
   std::unique_ptr<int4[], PinnedFree> h_list;  // the last frame's block list lands here (readFrameList)
   int last_frame_n = 0;
-  std::unique_ptr<int[], PinnedFree> h_count_ring;
-  cudaEvent_t count_events[kCountRing];
-  bool count_pending[kCountRing];
-  long long count_cum_at[kCountRing];  // cells_cum when the read-back was enqueued
-  int count_ring_head = 0;
-  int tsdf_count_confirmed = 0;        // last *tsdf.count seen by the host ...
-  long long confirmed_cum = 0;         // ... and cells_cum at that moment
-  long long cells_cum = 0;             // sum of the view-AABB cells of every frame enqueued so far
 
   long long launches = 0;
   bool profiling = false;
@@ -541,6 +613,12 @@ cudaError_t allocPinned(std::unique_ptr<T[], PinnedFree>* out, size_t n) {
   const cudaError_t e = cudaMallocHost(&p, n * sizeof(T));
   if (e == cudaSuccess) out->reset(static_cast<T*>(p));
   return e;
+}
+
+int SlabBounds::create() {
+  NVB_CUDA(allocPinned(&h_count_ring_, kCountRing));
+  for (cudaEvent_t& e : count_events_) NVB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  return NVB_OK;
 }
 
 // Candidate records of the exchange-slab wavefront: one segment per CTA of the launch, by ring parity. In a ring a CTA
@@ -813,59 +891,56 @@ void collectStages(NvbMapper* m) {
   m->stage_events.clear();
 }
 
-// Poll the asynchronous read-backs of *tsdf.count to tighten the host-side bound.
-// count <= confirmed + (cells enqueued since the confirmed read-back).
-void pollCounts(NvbMapper* m) {
-  for (int k = 0; k < kCountRing; k++) {
-    if (m->count_pending[k] && cudaEventQuery(m->count_events[k]) == cudaSuccess) {
-      m->count_pending[k] = false;
-      if (m->count_cum_at[k] > m->confirmed_cum) {
-        m->confirmed_cum = m->count_cum_at[k];
-        m->tsdf_count_confirmed = m->h_count_ring[k];
-      }
-    }
-  }
-  const long long ub = (long long)m->tsdf_count_confirmed + (m->cells_cum - m->confirmed_cum);
-  m->tsdf_count_ub = (int)std::min<long long>(ub, 0x7fffffff);
-}
-
-int ensureTsdfCapacity(NvbMapper* m, long long new_cells) {
-  pollCounts(m);
-  new_cells += m->derived_extra_ub;
-  if ((long long)m->tsdf_count_ub + new_cells <= m->tsdf.capacity()) return NVB_OK;
-  // refine the bound with a synchronous read
-  NVB_CUDA(syncAll(m));
-  int count = 0;
-  NVB_CUDA(m->tsdf.highWaterMark(&count));
-  for (int k = 0; k < kCountRing; k++) m->count_pending[k] = false;
-  m->tsdf_count_confirmed = count;
-  m->confirmed_cum = m->cells_cum;
-  m->tsdf_count_ub = count;
-  if ((long long)count + new_cells <= m->tsdf.capacity()) return NVB_OK;
-  long long cap = m->tsdf.capacity();
-  while (cap < (long long)count + new_cells) cap *= 2;
-  if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "TSDF layer would exceed 2^28 blocks");
-  NVB_CUDA(m->tsdf.grow(m, (int)cap));
-  return growTracker(m, (int)cap);
-}
-
-// The explicit-list entry points are synchronous: afterwards the real fill level of the ESDF slab is known and replaces
-// the running sum of list lengths (which would otherwise grow the slab without need in a long session).
-int tightenEsdfBound(NvbMapper* m) {
-  int count = 0;
-  NVB_CUDA(m->esdf.fillLevel(&count));
-  const int from_tsdf = std::min(m->tsdf_count_ub, m->tsdf.capacity());
-  m->esdf_extra_ub = std::max(0, count - from_tsdf);
+// The capacity a slab of `capacity` slots needs to hold `need` blocks: doubled until they fit, and at most 2^28. `what`
+// names the slab in the error.
+int grownCapacity(int capacity, long long need, const char* what, int* out) {
+  long long cap = capacity;
+  while (cap < need) cap *= 2;
+  if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, std::string(what) + " would exceed 2^28 blocks");
+  *out = (int)cap;
   return NVB_OK;
 }
 
-int ensureEsdfCapacity(NvbMapper* m, long long needed_total) {
-  if (needed_total <= m->esdf.capacity()) return NVB_OK;
-  long long cap = m->esdf.capacity();
-  while (cap < needed_total) cap *= 2;
-  if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "ESDF layer would exceed 2^28 blocks");
-  NVB_CUDA(m->esdf.grow(m, (int)cap));
-  return allocEsdfScratch(m, (int)cap);
+// Room in the projective slab for `cells` more blocks beyond its bound, without raising it. Growing to the capacity the slab
+// already has changes nothing.
+int ensureTsdfCapacity(NvbMapper* m, long long cells) {
+  if (m->bounds.projectiveNeed(cells) <= m->tsdf.capacity()) return NVB_OK;
+  // refine the bound with a synchronous read
+  NVB_CUDA(syncAll(m));
+  int count = 0, cap = 0, rc;
+  NVB_CUDA(m->tsdf.highWaterMark(&count));
+  m->bounds.confirm(count);
+  if ((rc = grownCapacity(m->tsdf.capacity(), m->bounds.projectiveNeed(cells), "TSDF layer", &cap))) return rc;
+  NVB_CUDA(m->tsdf.grow(m, cap));
+  return growTracker(m, cap);
+}
+
+int ensureEsdfCapacity(NvbMapper* m, long long need) {
+  int cap = 0, rc;
+  if (need <= m->esdf.capacity()) return NVB_OK;
+  if ((rc = grownCapacity(m->esdf.capacity(), need, "ESDF layer", &cap))) return rc;
+  NVB_CUDA(m->esdf.grow(m, cap));
+  return allocEsdfScratch(m, cap);
+}
+
+// Every call that adds blocks reserves room through its slab's kind. The projective slab (TSDF or occupancy) counts them in
+// its bound. ESDF blocks from explicit lists, and those of a slab that follows the projective slab (colour, mesh, freespace),
+// count beyond it; such a slab then follows the projective slab's capacity.
+int reserveProjective(NvbMapper* m, long long n) {
+  const int rc = ensureTsdfCapacity(m, n);
+  if (rc == NVB_OK) m->bounds.add(n, 0, 0);
+  return rc;
+}
+int reserveEsdf(NvbMapper* m, int n) {
+  m->bounds.add(0, n, 0);
+  return ensureEsdfCapacity(m, m->bounds.esdfNeed(m->tsdf.capacity()));
+}
+int reserveDerived(NvbMapper* m, LayerSlab* L, int n) {
+  m->bounds.add(0, 0, n);
+  const int rc = ensureTsdfCapacity(m, 0);
+  if (rc) return rc;
+  NVB_CUDA(followProjectiveSlab(m, L, L->dev().block_bytes));
+  return NVB_OK;
 }
 
 int ensureFrameScratch(NvbMapper* m, const ViewGrid& g) {
@@ -1124,17 +1199,7 @@ int enqueueFrame(NvbMapper* m, const float* depth, const unsigned char* mask, in
     }
     endStage(m);
     m->launches++;
-    // asynchronous read-back of the slab fill level for the host-side capacity bound
-    m->cells_cum += cells;
-    const int k = m->count_ring_head;
-    if (!m->count_pending[k]) {
-      m->count_ring_head = (k + 1) % kCountRing;
-      NVB_CUDA(cudaMemcpyAsync(&m->h_count_ring[k], m->tsdf.dev().count, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
-      NVB_CUDA(cudaEventRecord(m->count_events[k], m->stream));
-      m->count_pending[k] = true;
-      m->count_cum_at[k] = m->cells_cum;
-    }
-    m->tsdf_count_ub = (int)std::min<long long>((long long)m->tsdf_count_ub + cells, 0x7fffffff);
+    if ((rc = m->bounds.recordFrame(m->tsdf.dev().count, cells, m->stream))) return rc;
   }
   if (stage_slot >= 0) {
     NVB_CUDA(cudaEventRecord(m->stage_consumed[stage_slot], m->stream));
@@ -1194,21 +1259,13 @@ int readFrameList(NvbMapper* m, int32_t* out_xyz, int32_t cap, int32_t* out_coun
 int enqueueEsdf(NvbMapper* m, const int* in_xyz_dev, int n_explicit, bool from_tracker, bool slice = false,
                 const float* plane = nullptr) {
   int rc;
-  int upper;
   // EsdfMode: a mapper's ESDF layer is 3-D or a 2-D slice, never both (src/mapper/mapper.cpp:410-415,436-441)
   const int want_mode = slice ? 2 : 1;
   if (m->esdf_mode != 0 && m->esdf_mode != want_mode)
     return fail(NVB_ERR_INVALID_ARGUMENT, "the ESDF layer of this mapper is already in the other mode (3-D vs 2-D slice)");
   m->esdf_mode = want_mode;
-  if (from_tracker) {
-    pollCounts(m);
-    upper = std::min(m->tsdf_count_ub, m->tsdf.capacity());
-  } else {
-    upper = n_explicit;
-    m->esdf_extra_ub += n_explicit;
-  }
-  if (upper <= 0) upper = 1;
-  if ((rc = ensureEsdfCapacity(m, (long long)std::min(m->tsdf_count_ub, m->tsdf.capacity()) + m->esdf_extra_ub))) return rc;
+  const int upper = std::max(1, from_tracker ? m->bounds.projectiveUpper(m->tsdf.capacity()) : n_explicit);
+  if ((rc = reserveEsdf(m, from_tracker ? 0 : n_explicit))) return rc;
   if (slice) {
     // column set + column list sized to the projective layer
     const size_t columns = std::max(m->tsdf.capacity(), upper);
@@ -1426,12 +1483,7 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   NVB_CUDA(allocPinned(&m->h_ints, 64));
   memset(m->h_ints.get(), 0, 64 * sizeof(int));
   NVB_CUDA(allocPinned(&m->h_list, kHostListCap));
-  NVB_CUDA(allocPinned(&m->h_count_ring, kCountRing));
-  for (int k = 0; k < kCountRing; k++) {
-    NVB_CUDA(cudaEventCreateWithFlags(&m->count_events[k], cudaEventDisableTiming));
-    m->count_pending[k] = false;
-    m->count_cum_at[k] = 0;
-  }
+  if ((rc = m->bounds.create())) return rc;
   for (int k = 0; k < kStagingBuffers; k++) {
     NVB_CUDA(cudaEventCreateWithFlags(&m->stage_copied[k], cudaEventDisableTiming));
     NVB_CUDA(cudaEventCreateWithFlags(&m->stage_consumed[k], cudaEventDisableTiming));
@@ -1482,9 +1534,8 @@ void nvb_mapper_destroy(NvbMapper* m) {
   if (m->dyn_event) cudaEventDestroy(m->dyn_event);
   if (m->query_event) cudaEventDestroy(m->query_event);
   if (m->stage_pool) cudaMemPoolDestroy(m->stage_pool);  // a render's staging freed on a caller's stream is released once that free completes
-  for (int k = 0; k < kCountRing; k++) cudaEventDestroy(m->count_events[k]);
   cudaStreamDestroy(m->stream), cudaStreamDestroy(m->copy_stream);
-  delete m;  // the layers, device buffers and pinned buffers free themselves
+  delete m;  // the layers, device buffers, pinned buffers and the bounds' read-back ring free themselves
 }
 
 // Empties the layers and the state derived from their blocks: the slabs and hashes, the tracker (every consumer's next
@@ -1507,9 +1558,7 @@ static int resetLayers(NvbMapper* m) {
   NVB_CUDA(cudaMemsetAsync(m->nbr27.get(), 0xFE, (size_t)m->esdf.capacity() * 27 * sizeof(int), m->stream));
   NVB_CUDA(cudaMemsetAsync(m->error_dev, 0, sizeof(int), m->stream));
   if (m->mesh.exists()) NVB_CUDA(cudaMemsetAsync(m->mesh_state.get(), 0, kArenaInts * sizeof(int), m->stream));
-  m->tsdf_count_ub = 0, m->tsdf_count_confirmed = 0, m->esdf_extra_ub = 0, m->derived_extra_ub = 0;
-  m->cells_cum = 0, m->confirmed_cum = 0;
-  for (int k = 0; k < kCountRing; k++) m->count_pending[k] = false;
+  m->bounds.reset(0, 0, 0);
   NVB_CUDA(syncAll(m));
   return NVB_OK;
 }
@@ -1806,9 +1855,7 @@ int freespaceUpdateImpl(NvbMapper* m, const int* in_xyz_dev, int n_explicit, lon
                         int rows, int cols, const float* T_L_C, const NvbCamera* cam, float max_view_distance_m,
                         float truncation_distance_m) {
   NVB_CUDA(followProjectiveSlab(m, &m->freespace, kFreespaceBlockBytes));
-  int upper = in_xyz_dev ? n_explicit : std::min(m->tsdf_count_ub, m->tsdf.capacity());
-  if (!in_xyz_dev) pollCounts(m), upper = std::min(m->tsdf_count_ub, m->tsdf.capacity());
-  if (upper < 1) upper = 1;
+  const int upper = std::max(1, in_xyz_dev ? n_explicit : m->bounds.projectiveUpper(m->tsdf.capacity()));
   NVB_CUDA(m->fs_work.grow(m, upper, 2 * (size_t)upper));
   FreespaceArgs a{};
   a.tsdf = m->tsdf.dev(), a.fs = m->freespace.dev();
@@ -2064,9 +2111,7 @@ int32_t nvb_mapper_mark_unobserved_free_inside_radius(NvbMapper* m, const float 
     return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
   a.cells = (int)cells;
   int rc;
-  if ((rc = ensureTsdfCapacity(m, cells))) return rc;
-  m->cells_cum += cells;
-  m->tsdf_count_ub += (int)cells;
+  if ((rc = reserveProjective(m, cells))) return rc;
   NVB_CUDA(syncAll(m));  // rare, synchronous call: the ESDF side stream may still be reading the projective layer
   a.layer = m->tsdf.dev();
   a.occupancy = m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY ? 1 : 0;
@@ -2361,7 +2406,7 @@ int32_t nvb_esdf_integrate_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, 
   int rc = enqueueEsdf(m, m->xyz_upload.get(), n, false);
   if (rc) return rc;
   if ((rc = nvb_mapper_synchronize(m))) return rc;
-  return tightenEsdfBound(m);
+  return m->bounds.tightenEsdfBound(m->esdf, m->tsdf.capacity());
 }
 
 void nvb_default_esdf_slice_params(NvbEsdfSliceParams* p) {
@@ -2426,7 +2471,7 @@ static int32_t integrateSliceBlocksImpl(NvbMapper* m, const float* plane, const 
   int rc = enqueueEsdf(m, m->xyz_upload.get(), num_blocks, false, true, plane);
   if (rc) return rc;
   if ((rc = nvb_mapper_synchronize(m))) return rc;
-  return tightenEsdfBound(m);
+  return m->bounds.tightenEsdfBound(m->esdf, m->tsdf.capacity());
 }
 
 void nvb_default_ground_plane_params(NvbGroundPlaneParams* p) {
@@ -3174,23 +3219,16 @@ int32_t nvb_layer_get_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
 
 int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_host, int32_t n, const void* in_host) {
   if (!m || (n > 0 && (!xyz_host || !in_host))) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  const LayerSlab* L = layerOf(m, layer);
+  LayerSlab* L = layerOf(m, layer);
   if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "unknown layer");
   if (n <= 0) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   for (int i = 0; i < n; i++)
     if (!indexInRange(xyz_host[3 * i], xyz_host[3 * i + 1], xyz_host[3 * i + 2]))
       return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
-  int rc;
-  if (layer == NVB_LAYER_TSDF) {
-    if ((rc = ensureTsdfCapacity(m, n))) return rc;
-    m->cells_cum += n;
-    m->tsdf_count_ub += n;
-  } else {
-    m->esdf_extra_ub += n;
-    if ((rc = ensureEsdfCapacity(m, (long long)std::min(m->tsdf_count_ub, m->tsdf.capacity()) + m->esdf_extra_ub))) return rc;
-  }
-  L = layerOf(m, layer);
+  const bool projective = L == &m->tsdf, esdf = L == &m->esdf;
+  const int rc = projective ? reserveProjective(m, n) : esdf ? reserveEsdf(m, n) : reserveDerived(m, L, n);
+  if (rc) return rc;
   NVB_CUDA(syncAll(m));
   CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
   const int* xyz_dev;
@@ -3199,13 +3237,13 @@ int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
   NVB_CUDA(host.in(static_cast<const unsigned char*>(in_host), (size_t)n * L->dev().block_bytes, &in_dev));
   launchScatterBlocks(L->dev(), xyz_dev, n, in_dev, m->error_dev, m->stream);
   m->launches++;
-  if (layer == NVB_LAYER_ESDF) m->prune_ok = false;  // voxels written from outside: the parent boxes are no longer bounds
+  if (esdf) m->prune_ok = false;  // voxels written from outside: the parent boxes are no longer bounds
   NVB_CUDA(syncAll(m));
-  if (layer == NVB_LAYER_TSDF) {
+  if (projective) {
     // a later updateEsdf must see these blocks: the ESDF consumer's next update covers every block. Only the ESDF is
     // told; the freespace and mesh consumers keep their lists.
     m->tracker[kEsdfBlocks].initialized = false;
-  } else {
+  } else if (esdf) {
     // blocks created outside the ESDF update path are not linked: forget the neighbour table,
     // it is re-resolved lazily through the hash
     NVB_CUDA(cudaMemsetAsync(m->nbr.get(), 0xFE, (size_t)m->esdf.capacity() * 6 * sizeof(int), m->stream));
@@ -3312,10 +3350,10 @@ int32_t nvb_mapper_load_map(NvbMapper* m, const char* path, int32_t loaded_block
   // the slabs' growth, checked before the map changes (colour and freespace follow the projective slab)
   const int n_proj = in[proj].n, n_esdf = in[NVB_LAYER_ESDF].n;
   const long long need_t = std::max({n_proj, in[NVB_LAYER_COLOR].n, in[NVB_LAYER_FREESPACE].n});
-  long long cap_t = m->tsdf.capacity(), cap_e = m->esdf.capacity();
-  while (cap_t < need_t) cap_t *= 2;
-  while (cap_e < n_esdf) cap_e *= 2;
-  if (cap_t > (1ll << 28) || cap_e > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "the map would exceed 2^28 blocks");
+  int cap_t = 0, cap_e = 0;
+  if ((rc = grownCapacity(m->tsdf.capacity(), need_t, "the map", &cap_t)) ||
+      (rc = grownCapacity(m->esdf.capacity(), n_esdf, "the map", &cap_e)))
+    return rc;
 
   // Mapper::loadMap: the file's voxel size, a new cake and a fresh tracker (mapper.cpp:661-671)
   if ((rc = resetLayers(m))) return rc;
@@ -3337,9 +3375,7 @@ int32_t nvb_mapper_load_map(NvbMapper* m, const char* path, int32_t loaded_block
   launchEsdfParentBoxes(m->esdf.dev(), n_esdf, m->psum.get(), m->stream);
   m->launches++;
   // the fill-level bounds from the real counts (tightenEsdfBound)
-  m->tsdf_count_ub = m->tsdf_count_confirmed = n_proj;
-  m->confirmed_cum = m->cells_cum;
-  m->esdf_extra_ub = std::max(0, n_esdf - n_proj);
+  m->bounds.reset(n_proj, std::max(0, n_esdf - n_proj), 0);
   NVB_CUDA(syncAll(m));
   if ((rc = checkDeviceError(m))) return rc;
   // a new colour mesh layer and a full mesh update (mapper.cpp:673-678)
@@ -3620,8 +3656,7 @@ int32_t nvb_mapper_update_mesh(NvbMapper* m, int32_t update_full_layer) {
   NVB_CUDA(cudaSetDevice(m->device));
   int rc;
   if ((rc = ensureMeshLayer(m))) return rc;
-  pollCounts(m);
-  const int upper = std::min(m->tsdf_count_ub, m->tsdf.capacity());
+  const int upper = m->bounds.projectiveUpper(m->tsdf.capacity());
   if ((rc = startTrackerUpdate(m, kColorMeshBlocks, update_full_layer))) return rc;
   // integrateBlocksGPU + updateAppearance over the tracker's blocks, then markBlocksAsUpdated (mapper.cpp:385-395)
   const TrackerList todo = m->tracker[kColorMeshBlocks].list();
@@ -4028,17 +4063,14 @@ int generateLayerImpl(NvbMapper* m, LayerSlab* L, int layer_id, const NvbScene* 
   int rc;
   if ((rc = sceneBlockBox(m, scene, &a.box_lo, &a.box_size, &a.cells))) return rc;
   if (L == &m->tsdf) {
-    if ((rc = ensureTsdfCapacity(m, a.cells))) return rc;
-    m->cells_cum += a.cells;
-    m->tsdf_count_ub = (int)std::min<long long>((long long)m->tsdf_count_ub + a.cells, 0x7fffffff);
+    if ((rc = reserveProjective(m, a.cells))) return rc;
   } else {  // the freespace slab: at least the TSDF slab's capacity, doubled until the AABB's blocks fit
     NVB_CUDA(syncAll(m));
-    int count = 0;
+    int count = 0, cap = 0;
     NVB_CUDA(L->fillLevel(&count));
-    long long cap = std::max(L->capacity(), m->tsdf.capacity());
-    while (cap < (long long)count + a.cells) cap *= 2;
-    if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "the freespace layer would exceed 2^28 blocks");
-    NVB_CUDA(L->grow(m, (int)cap));
+    if ((rc = grownCapacity(std::max(L->capacity(), m->tsdf.capacity()), count + a.cells, "the freespace layer", &cap)))
+      return rc;
+    NVB_CUDA(L->grow(m, cap));
   }
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(joinEsdf(m));  // an update_esdf_async may still be reading the layer
@@ -4062,12 +4094,12 @@ int generateLayerImpl(NvbMapper* m, LayerSlab* L, int layer_id, const NvbScene* 
 
 // The projective layer as VoxelBlockLayer::copyFrom leaves it before the copy: no blocks, with room for `cells` new ones. Its
 // slots are zeroed and handed out again from 0, so every consumer's dirty words are cleared too. The ESDF, colour, mesh and
-// freespace layers keep their blocks, so the capacity bounds count them as extra: the ESDF's through esdf_extra_ub, the others'
-// (which follow the projective slab) through derived_extra_ub. Both slabs are grown first, keeping their contents, so that a
-// failed growth leaves the map as it was.
+// freespace layers keep their blocks, so the slab bounds count them as extra: the ESDF's on its own, the others' (which
+// follow the projective slab) as the derived slabs' extra blocks. Both slabs are grown first, keeping their contents, so that
+// a failed growth leaves the map as it was.
 int emptyProjectiveLayer(NvbMapper* m, long long cells) {
   NVB_CUDA(syncAll(m));
-  int esdf_n = 0, derived = 0, rc;  // derived: the most blocks a layer that follows the projective slab holds
+  int esdf_n = 0, derived = 0, cap = 0, rc;  // derived: the most blocks a layer that follows the projective slab holds
   for (const LayerSlab* L : m->layers()) {
     if (L == &m->tsdf) continue;
     int n = 0;
@@ -4075,11 +4107,9 @@ int emptyProjectiveLayer(NvbMapper* m, long long cells) {
     if (L == &m->esdf) esdf_n = n;
     else derived = std::max(derived, n);
   }
-  long long cap = m->tsdf.capacity();
-  while (cap < cells + derived) cap *= 2;
-  if (cap > (1ll << 28)) return fail(NVB_ERR_CAPACITY, "TSDF layer would exceed 2^28 blocks");
-  NVB_CUDA(m->tsdf.grow(m, (int)cap));
-  if ((rc = growTracker(m, (int)cap)) || (rc = ensureEsdfCapacity(m, cells + esdf_n))) return rc;
+  if ((rc = grownCapacity(m->tsdf.capacity(), cells + derived, "TSDF layer", &cap))) return rc;
+  NVB_CUDA(m->tsdf.grow(m, cap));
+  if ((rc = growTracker(m, cap)) || (rc = ensureEsdfCapacity(m, cells + esdf_n))) return rc;
   NVB_CUDA(m->tsdf.empty(m->stream));
   m->launches++;
   for (TrackedBlocks& t : m->tracker) {
@@ -4087,11 +4117,7 @@ int emptyProjectiveLayer(NvbMapper* m, long long cells) {
     NVB_CUDA(cudaMemsetAsync(t.dirty.get(), 0, t.dirty.size() * sizeof(int), m->stream));
     NVB_CUDA(cudaMemsetAsync(t.count, 0, sizeof(int), m->stream));
   }
-  m->tsdf_count_ub = m->tsdf_count_confirmed = 0;
-  m->confirmed_cum = m->cells_cum;
-  for (int k = 0; k < kCountRing; k++) m->count_pending[k] = false;
-  m->esdf_extra_ub = esdf_n;
-  m->derived_extra_ub = derived;
+  m->bounds.reset(0, esdf_n, derived);
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   return NVB_OK;
 }
