@@ -227,7 +227,7 @@ typedef struct NvbOccupancyDecayParams {
 } NvbOccupancyDecayParams;
 /* DecayBlockExclusionOptions (C/include/nvblox/integrators/internal/decayer.h:31-44): blocks that are spared. */
 typedef struct NvbDecayExclusion {
-  const int32_t* excluded_blocks_xyz_host; /* may be NULL */
+  const int32_t* excluded_blocks_xyz_host; /* may be NULL when the count is 0; a negative count is NVB_ERR_INVALID_ARGUMENT */
   int32_t num_excluded_blocks;
   int32_t has_exclusion_sphere;            /* blocks whose origin is within the sphere are spared */
   float exclusion_center[3];
@@ -726,11 +726,12 @@ NVB_API int32_t nvb_mesh_integrate_blocks(NvbMapper* m, const int32_t* blocks_xy
 /* MeshIntegrator::updateAppearance(colour layer, block list, mesh layer) (mesh_integrator_appearance.cu:71-96,281-380). */
 NVB_API int32_t nvb_mesh_update_color(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks);
 /* Sizes of the listed mesh blocks: sizes_out[3 i ..] = {vertices, triangle indices, colours}, or -1s if block i has no mesh
- * block. The block indices of the layer: nvb_layer_block_indices(m, NVB_LAYER_MESH, ...). */
+ * block. The block indices of the layer: nvb_layer_block_indices(m, NVB_LAYER_MESH, ...). A negative num_blocks is
+ * NVB_ERR_INVALID_ARGUMENT. */
 NVB_API int32_t nvb_mesh_block_sizes(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks, int32_t* sizes_out);
 /* The listed mesh blocks packed back to back in list order into host buffers (any of them may be NULL): 3 floats per
  * vertex / normal, one int32 per triangle index (relative to the block's first vertex), 4 bytes RGBA per colour.
- * caps = capacities of the buffers in {vertices, triangle indices, colours}. */
+ * caps = capacities of the buffers in {vertices, triangle indices, colours}. A negative num_blocks is NVB_ERR_INVALID_ARGUMENT. */
 NVB_API int32_t nvb_mesh_get_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks, float* vertices_out,
                                     float* normals_out, int32_t* triangles_out, uint8_t* colors_out, const int64_t caps[3]);
 /* out = {arena capacity, fill level, vertices emitted by the last update, reserved} in vertices. */
@@ -781,10 +782,13 @@ NVB_API int32_t nvb_layer_block_indices(NvbMapper* m, int32_t layer, int32_t* ou
 NVB_API int32_t nvb_layer_slab_stats(NvbMapper* m, int32_t layer, int64_t out[4]);
 /* getBlockAtIndex(...)->voxels copied to host: out_host receives n blocks of
  * block_bytes (4096 TSDF / 10240 ESDF); found[i] = 0 for unallocated indices
- * (their output bytes are zero). block_bytes: 4096 TSDF / 10240 ESDF / 2048 occupancy. */
+ * (their output bytes are zero). block_bytes: 4096 TSDF / 10240 ESDF / 2048 occupancy. A negative n is
+ * NVB_ERR_INVALID_ARGUMENT. */
 NVB_API int32_t nvb_layer_get_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_host,
                                      int32_t n, void* out_host, uint8_t* found_host);
-/* allocateBlockAtIndex + host->device copy of the voxels (tests, map loading). */
+/* allocateBlockAtIndex + host->device copy of the voxels (tests, map loading). Each index carries its own block, so an
+ * index listed twice is NVB_ERR_INVALID_ARGUMENT, as is a negative n; an index outside +-2^20 is NVB_ERR_INDEX_RANGE.
+ * Either way nothing is written. */
 NVB_API int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_host,
                                      int32_t n, const void* in_host);
 /* getBlockAtIndex(index).get(): raw device pointer of a block, NULL if absent.

@@ -233,6 +233,54 @@ int checkMemoryKind(int32_t memory) {
   return fail(NVB_ERR_INVALID_ARGUMENT, "bad memory kind");
 }
 
+// What a call does with a caller's list of block indices, and so how much of it is checked.
+enum class BlockList {
+  kLookup,     // looked up only: the hash rejects an index it cannot hold
+  kInsert,     // inserted in the caller's order: every index must be in range
+  kInsertSet,  // inserted as a set, since find-or-insert needs unique keys per launch: in range, then sorted in (x, y, z)
+               // order with repeats dropped
+};
+
+// Checks the caller's list `*xyz` of `*n` block indices (xyz triples in host memory) by `kind` before anything is enqueued:
+// a negative count or a null list with a positive count is NVB_ERR_INVALID_ARGUMENT, an index outside +-2^20 is
+// NVB_ERR_INDEX_RANGE. A set is built in `set`, and *xyz and *n then name it.
+int takeBlockList(BlockList kind, const int32_t** xyz, int32_t* n, std::vector<std::array<int, 3>>* set = nullptr) {
+  if (*n < 0 || (*n > 0 && !*xyz)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad block list");
+  if (kind == BlockList::kLookup) return NVB_OK;
+  const int32_t* p = *xyz;
+  for (int i = 0; i < *n; i++)
+    if (!indexInRange(p[3 * i], p[3 * i + 1], p[3 * i + 2])) return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
+  if (kind == BlockList::kInsert) return NVB_OK;
+  static_assert(sizeof(std::array<int, 3>) == 3 * sizeof(int32_t), "a set entry is one xyz triple");
+  set->assign(reinterpret_cast<const std::array<int, 3>*>(p), reinterpret_cast<const std::array<int, 3>*>(p) + *n);
+  std::sort(set->begin(), set->end());  // std::array compares lexicographically: (x, y, z) order
+  set->erase(std::unique(set->begin(), set->end()), set->end());
+  *xyz = set->data()->data(), *n = (int32_t)set->size();
+  return NVB_OK;
+}
+
+// Where a block-list record keeps its block index.
+enum class Record {
+  kXyzFirst,  // {x, y, z, ·}: the frame, colour and mark-free lists
+  kXyzLast,   // {slot, x, y, z}: the dead and shape-selection lists
+};
+
+// Returns a list of n block-index records to the caller: *out_count = n, and the first min(n, cap) indices as xyz triples
+// to out_xyz. `sorted` puts all n records in (x, y, z) order before the cut; unsorted, only the first min(n, cap) are read.
+void writeBlockList(int4* rec, int n, Record at, bool sorted, int32_t* out_xyz, int32_t cap, int32_t* out_count) {
+  if (out_count) *out_count = n;
+  if (!out_xyz || cap <= 0 || n <= 0) return;
+  const auto xyz = [at](const int4& r) {
+    return at == Record::kXyzFirst ? std::array<int, 3>{r.x, r.y, r.z} : std::array<int, 3>{r.y, r.z, r.w};
+  };
+  if (sorted) std::sort(rec, rec + n, [&](const int4& a, const int4& b) { return xyz(a) < xyz(b); });
+  const int k = std::min(n, (int)cap);
+  for (int i = 0; i < k; i++) {
+    const std::array<int, 3> b = xyz(rec[i]);
+    out_xyz[3 * i] = b[0], out_xyz[3 * i + 1] = b[1], out_xyz[3 * i + 2] = b[2];
+  }
+}
+
 // The device side of one call's caller buffers, all of one memory kind, for work on `st`. Device buffers are used in place.
 // Host buffers are staged in stream-ordered allocations on `st` from `pool` (the device's default pool when null): an input
 // is copied down when it is staged, the outputs are copied back by finish(), and the destructor frees the staging on `st`
@@ -1241,18 +1289,32 @@ int readFrameList(NvbMapper* m, int32_t* out_xyz, int32_t cap, int32_t* out_coun
   NVB_CUDA(syncAll(m));
   const int n = m->h_ints[0];
   m->last_frame_n = n;
-  if (out_count) *out_count = n;
-  if (out_xyz && cap > 0 && n > 0) {
-    const int k = std::min(n, cap);
-    const int4* src = m->h_list.get();
-    std::vector<int4> tmp;
-    if (k > want) {  // the frame has more blocks than the speculative prefix: one more copy
-      tmp.resize((size_t)k);
-      NVB_CUDA(cudaMemcpy(tmp.data(), m->frame_blocks.get(), (size_t)k * sizeof(int4), cudaMemcpyDeviceToHost));
-      src = tmp.data();
-    }
-    for (int i = 0; i < k; i++) out_xyz[3 * i] = src[i].x, out_xyz[3 * i + 1] = src[i].y, out_xyz[3 * i + 2] = src[i].z;
+  const int k = std::min(n, cap);
+  int4* src = m->h_list.get();
+  std::vector<int4> tmp;
+  if (out_xyz && cap > 0 && k > want) {  // the frame has more blocks than the speculative prefix: one more copy
+    tmp.resize((size_t)k);
+    NVB_CUDA(cudaMemcpy(tmp.data(), m->frame_blocks.get(), (size_t)k * sizeof(int4), cudaMemcpyDeviceToHost));
+    src = tmp.data();
   }
+  writeBlockList(src, n, Record::kXyzFirst, false, out_xyz, cap, out_count);
+  return NVB_OK;
+}
+
+// writeBlockList for a list on the device, its count at `count_dev` and its records at `rec_dev`. The count is read first,
+// then only the records the output needs.
+int readBlockList(NvbMapper* m, const int* count_dev, const int4* rec_dev, Record at, bool sorted, int32_t* out_xyz,
+                  int32_t cap, int32_t* out_count) {
+  int n = 0;
+  NVB_CUDA(cudaMemcpyAsync(&n, count_dev, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  std::vector<int4> rec;
+  if (out_xyz && cap > 0 && n > 0) {
+    rec.resize((size_t)(sorted ? n : std::min(n, (int)cap)));
+    NVB_CUDA(cudaMemcpyAsync(rec.data(), rec_dev, rec.size() * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+  }
+  writeBlockList(rec.data(), n, at, sorted, out_xyz, cap, out_count);
   return NVB_OK;
 }
 
@@ -1727,16 +1789,6 @@ int removeDeadBlocks(NvbMapper* m, int n_dead, std::vector<int4>* removed) {
   for (const int4& d : *removed) m->cleared_blocks.insert({d.y, d.z, d.w});
   return NVB_OK;
 }
-
-// Removed or touched blocks {slot, x, y, z} -> xyz triples in (x, y, z) order.
-void writeSortedTriples(std::vector<int4>& v, int32_t* out_xyz_host, int32_t cap) {
-  if (!out_xyz_host || cap <= 0) return;
-  std::sort(v.begin(), v.end(), [](const int4& a, const int4& b) {
-    return a.y != b.y ? a.y < b.y : (a.z != b.z ? a.z < b.z : a.w < b.w);
-  });
-  const int k = std::min((int)v.size(), (int)cap);
-  for (int i = 0; i < k; i++) out_xyz_host[3 * i] = v[i].y, out_xyz_host[3 * i + 1] = v[i].z, out_xyz_host[3 * i + 2] = v[i].w;
-}
 }  // namespace
 
 int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const float* depth, int32_t depth_memory,
@@ -1748,8 +1800,9 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
     int rc = validateFrameArgs(m, depth, depth_memory, rows, cols, T_L_C, cam);
     if (rc) return rc;
   }
-  if (exclusion && exclusion->num_excluded_blocks > 0 && !exclusion->excluded_blocks_xyz_host)
-    return fail(NVB_ERR_INVALID_ARGUMENT, "exclusion list is null");
+  const int32_t* excl_xyz = exclusion ? exclusion->excluded_blocks_xyz_host : nullptr;
+  int32_t ne = exclusion ? exclusion->num_excluded_blocks : 0;
+  if (int rc = takeBlockList(BlockList::kLookup, &excl_xyz, &ne)) return rc;
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));  // the decay touches both layers: nothing of the ESDF chain may be in flight
   const bool occupancy = m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY;
@@ -1781,10 +1834,9 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
   }
   // block exclusion
   CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
-  if (exclusion && exclusion->num_excluded_blocks > 0) {
-    const int ne = exclusion->num_excluded_blocks;
+  if (ne > 0) {
     const int* excl_dev;
-    NVB_CUDA(host.in(exclusion->excluded_blocks_xyz_host, (size_t)ne * 3 * sizeof(int), &excl_dev));
+    NVB_CUDA(host.in(excl_xyz, (size_t)ne * 3 * sizeof(int), &excl_dev));
     m->skip_seq++;
     launchMarkSkipped(P, excl_dev, ne, m->skip_stamp.get(), m->skip_seq, m->stream);
     a.skip_stamp = m->skip_stamp.get();
@@ -1814,12 +1866,7 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
   if (n_dead > 0) {
     std::vector<int4> removed;
     if ((rc = removeDeadBlocks(m, n_dead, &removed))) return rc;
-    if (out_count) *out_count = n_dead;
-    if (removed_xyz_host && cap > 0) {
-      const int k = std::min(n_dead, (int)cap);
-      for (int i = 0; i < k; i++)
-        removed_xyz_host[3 * i] = removed[i].y, removed_xyz_host[3 * i + 1] = removed[i].z, removed_xyz_host[3 * i + 2] = removed[i].w;
-    }
+    writeBlockList(removed.data(), n_dead, Record::kXyzLast, false, removed_xyz_host, cap, out_count);
   }
   // BlocksToUpdateTracker::addAllBlocksToUpdate (mapper_impl.h:208-211): the next ESDF update covers every block. The
   // reset also zeroes the dirty words of the deallocated slots, so a block that gets one of them is told again.
@@ -1913,28 +1960,17 @@ int32_t nvb_freespace_update_blocks(NvbMapper* m, const int32_t* blocks_xyz_host
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
   if (m->projective_layer_type != NVB_PROJECTIVE_TSDF_WITH_FREESPACE)
     return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper has no freespace layer");
-  if (num_blocks < 0 || (num_blocks > 0 && !blocks_xyz_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad block list");
+  std::vector<std::array<int, 3>> set;  // a set, like every caller's list in the reference
+  int rc = takeBlockList(BlockList::kInsertSet, &blocks_xyz_host, &num_blocks, &set);
+  if (rc) return rc;
   if (num_blocks == 0) return NVB_OK;  // early return (:337-339)
   if (depth) {
-    int rc = validateFrameArgs(m, depth, depth_memory, rows, cols, T_L_C, cam);
-    if (rc) return rc;
+    if ((rc = validateFrameArgs(m, depth, depth_memory, rows, cols, T_L_C, cam))) return rc;
   }
   NVB_CUDA(cudaSetDevice(m->device));
-  for (int i = 0; i < num_blocks; i++)
-    if (!indexInRange(blocks_xyz_host[3 * i], blocks_xyz_host[3 * i + 1], blocks_xyz_host[3 * i + 2]))
-      return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
-  // a set, like every caller's list in the reference (find-or-insert needs unique keys per launch)
-  struct K3 {
-    int x, y, z;
-  };
-  std::vector<K3> v((size_t)num_blocks);
-  memcpy(v.data(), blocks_xyz_host, (size_t)num_blocks * sizeof(K3));
-  std::sort(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x != b.x ? a.x < b.x : (a.y != b.y ? a.y < b.y : a.z < b.z); });
-  v.erase(std::unique(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x == b.x && a.y == b.y && a.z == b.z; }), v.end());
-  num_blocks = (int)v.size();
   CallerBuffers host(NVB_MEM_HOST, m->stream, m->stage_pool);
   const int* xyz_dev;
-  NVB_CUDA(host.in(&v[0].x, (size_t)num_blocks * 3 * sizeof(int), &xyz_dev));
+  NVB_CUDA(host.in(blocks_xyz_host, (size_t)num_blocks * 3 * sizeof(int), &xyz_dev));
   return freespaceUpdateImpl(m, xyz_dev, num_blocks, update_time_ms, depth, depth_memory, rows, cols, T_L_C, cam,
                              max_view_distance_m, truncation_distance_m);
 }
@@ -1972,8 +2008,7 @@ int32_t nvb_mapper_clear_outside_radius(NvbMapper* m, const float center[3], flo
   forgetDeadSlots(m, dead_count, n);  // no switch to update-all (unlike the decay)
   std::vector<int4> removed;
   if ((rc = removeDeadBlocks(m, n, &removed))) return rc;
-  if (out_count) *out_count = n;
-  writeSortedTriples(removed, removed_xyz_host, cap);
+  writeBlockList(removed.data(), n, Record::kXyzLast, true, removed_xyz_host, cap, out_count);
   return checkDeviceError(m);
 }
 
@@ -2006,17 +2041,8 @@ int clearShapesImpl(NvbMapper* m, const LayerSlab* L, int voxel_kind, bool track
   launchShapeSelect(a, m->stream);
   launchShapeClear(a, m->num_sms, m->stream);
   m->launches += 2;
-  int n = 0;
-  NVB_CUDA(cudaMemcpyAsync(&n, a.sel_count, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
-  if (out_count) *out_count = n;
-  if (updated_xyz_host && cap > 0 && n > 0) {
-    std::vector<int4> sel((size_t)n);
-    NVB_CUDA(cudaMemcpyAsync(sel.data(), a.sel, (size_t)n * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    writeSortedTriples(sel, updated_xyz_host, cap);
-  }
-  return checkDeviceError(m);
+  const int rc = readBlockList(m, a.sel_count, a.sel, Record::kXyzLast, true, updated_xyz_host, cap, out_count);
+  return rc ? rc : checkDeviceError(m);
 }
 }  // namespace
 
@@ -2043,7 +2069,7 @@ int32_t nvb_layer_clear_shapes(NvbMapper* m, int32_t layer, const NvbBoundingSha
 int32_t nvb_mapper_get_cleared_blocks(NvbMapper* m, const int32_t* ignore_xyz, int32_t n_ignore, int32_t* out_xyz_host,
                                       int32_t cap, int32_t* out_count) {
   if (!m || !out_count) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (n_ignore < 0 || (n_ignore > 0 && !ignore_xyz)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad ignore list");
+  if (int rc = takeBlockList(BlockList::kLookup, &ignore_xyz, &n_ignore)) return rc;
   if (!out_xyz_host) {
     *out_count = (int32_t)m->cleared_blocks.size();
     return NVB_OK;
@@ -2051,8 +2077,7 @@ int32_t nvb_mapper_get_cleared_blocks(NvbMapper* m, const int32_t* ignore_xyz, i
   for (int i = 0; i < n_ignore; i++) m->cleared_blocks.erase({ignore_xyz[3 * i], ignore_xyz[3 * i + 1], ignore_xyz[3 * i + 2]});
   *out_count = (int32_t)m->cleared_blocks.size();
   if (*out_count > cap) return fail(NVB_ERR_CAPACITY, "more cleared blocks than the output holds");
-  int i = 0;
-  for (const auto& k : m->cleared_blocks) out_xyz_host[3 * i] = k[0], out_xyz_host[3 * i + 1] = k[1], out_xyz_host[3 * i + 2] = k[2], i++;
+  for (const auto& k : m->cleared_blocks) out_xyz_host = std::copy(k.begin(), k.end(), out_xyz_host);
   m->cleared_blocks.clear();
   return NVB_OK;
 }
@@ -2128,18 +2153,7 @@ int32_t nvb_mapper_mark_unobserved_free_inside_radius(NvbMapper* m, const float 
   NVB_CUDA(cudaMemsetAsync(out_dev.get(), 0, sizeof(int4), m->stream));
   launchMarkFreeSphere(a, m->num_sms, m->stream);
   m->launches++;
-  int n = 0;
-  NVB_CUDA(cudaMemcpyAsync(&n, a.out_count, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
-  if (out_count) *out_count = n;
-  if (updated_xyz_host && cap > 0 && n > 0) {
-    const int k = std::min(n, (int)cap);
-    std::vector<int4> tmp((size_t)k);
-    NVB_CUDA(cudaMemcpyAsync(tmp.data(), a.out, (size_t)k * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    for (int i = 0; i < k; i++)
-      updated_xyz_host[3 * i] = tmp[i].x, updated_xyz_host[3 * i + 1] = tmp[i].y, updated_xyz_host[3 * i + 2] = tmp[i].z;
-  }
+  if ((rc = readBlockList(m, a.out_count, a.out, Record::kXyzFirst, false, updated_xyz_host, cap, out_count))) return rc;
   return checkDeviceError(m);
 }
 
@@ -2340,19 +2354,8 @@ int32_t nvb_mapper_last_color_blocks(NvbMapper* m, int32_t* out_xyz_host, int32_
   if (out_count) *out_count = 0;
   if (!m->color.exists() || !m->color_work.get()) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
-  int n = 0;
-  NVB_CUDA(cudaMemcpyAsync(&n, m->esdf_ints.get() + kColorWorkCount, sizeof(int), cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
-  if (out_count) *out_count = n;
-  if (out_xyz_host && cap > 0 && n > 0) {
-    const int k = std::min(n, (int)cap);
-    std::vector<int4> tmp((size_t)k);
-    NVB_CUDA(cudaMemcpyAsync(tmp.data(), m->color_work.get(), (size_t)k * sizeof(int4), cudaMemcpyDeviceToHost, m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    for (int i = 0; i < k; i++)
-      out_xyz_host[3 * i] = tmp[i].x, out_xyz_host[3 * i + 1] = tmp[i].y, out_xyz_host[3 * i + 2] = tmp[i].z;
-  }
-  return NVB_OK;
+  return readBlockList(m, m->esdf_ints.get() + kColorWorkCount, m->color_work.get(), Record::kXyzFirst, false, out_xyz_host,
+                       cap, out_count);
 }
 
 int32_t nvb_mapper_integrate_depth(NvbMapper* m, const float* depth, const uint8_t* mask, int32_t mask_mode,
@@ -2379,32 +2382,19 @@ int32_t nvb_mapper_update_esdf(NvbMapper* m, int32_t update_full_layer) {
 
 int32_t nvb_esdf_integrate_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
-  if (num_blocks < 0 || (num_blocks > 0 && !blocks_xyz_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad block list");
+  // The list is a set for every caller of the reference (Mapper::getBlocksToUpdate); make it one.
+  std::vector<std::array<int, 3>> set;
+  int rc = takeBlockList(BlockList::kInsertSet, &blocks_xyz_host, &num_blocks, &set);
+  if (rc) return rc;
   if (num_blocks == 0) return NVB_OK;  // early return, esdf_integrator.cu:226-228
   NVB_CUDA(cudaSetDevice(m->device));
-  // The list is a set for every caller of the reference (Mapper::getBlocksToUpdate); make it one.
-  struct K {
-    int x, y, z;
-  };
-  std::vector<K> v((size_t)num_blocks);
-  memcpy(v.data(), blocks_xyz_host, (size_t)num_blocks * sizeof(K));
-  std::sort(v.begin(), v.end(), [](const K& a, const K& b) {
-    if (a.x != b.x) return a.x < b.x;
-    if (a.y != b.y) return a.y < b.y;
-    return a.z < b.z;
-  });
-  v.erase(std::unique(v.begin(), v.end(), [](const K& a, const K& b) { return a.x == b.x && a.y == b.y && a.z == b.z; }),
-          v.end());
-  for (const K& k : v)
-    if (!indexInRange(k.x, k.y, k.z)) return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
-  const int n = (int)v.size();
+  const int n = num_blocks;
   NVB_CUDA(m->xyz_upload.grow(m, 3 * (size_t)n, 6 * (size_t)n));
   // Stream-ordered upload: a blocking cudaMemcpy from pageable memory may return before the DMA has landed,
   // and the mapper's stream is non-blocking (not ordered against the legacy default stream).
-  NVB_CUDA(cudaMemcpyAsync(m->xyz_upload.get(), v.data(), (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));  // v is pageable and about to go out of scope
-  int rc = enqueueEsdf(m, m->xyz_upload.get(), n, false);
-  if (rc) return rc;
+  NVB_CUDA(cudaMemcpyAsync(m->xyz_upload.get(), blocks_xyz_host, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));  // the set is pageable and about to go out of scope
+  if ((rc = enqueueEsdf(m, m->xyz_upload.get(), n, false))) return rc;
   if ((rc = nvb_mapper_synchronize(m))) return rc;
   return m->bounds.tightenEsdfBound(m->esdf, m->tsdf.capacity());
 }
@@ -2459,17 +2449,14 @@ int32_t nvb_esdf_integrate_slice_planar_blocks(NvbMapper* m, const float plane[4
 }
 static int32_t integrateSliceBlocksImpl(NvbMapper* m, const float* plane, const int32_t* blocks_xyz_host, int32_t num_blocks) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
-  if (num_blocks < 0 || (num_blocks > 0 && !blocks_xyz_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad block list");
+  int rc = takeBlockList(BlockList::kInsert, &blocks_xyz_host, &num_blocks);  // the column set dedupes on the device
+  if (rc) return rc;
   if (num_blocks == 0) return NVB_OK;  // early return (:289-291)
   NVB_CUDA(cudaSetDevice(m->device));
-  for (int i = 0; i < num_blocks; i++)
-    if (!indexInRange(blocks_xyz_host[3 * i], blocks_xyz_host[3 * i + 1], blocks_xyz_host[3 * i + 2]))
-      return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
   NVB_CUDA(m->xyz_upload.grow(m, 3 * (size_t)num_blocks, 6 * (size_t)num_blocks));
   NVB_CUDA(cudaMemcpyAsync(m->xyz_upload.get(), blocks_xyz_host, (size_t)num_blocks * 3 * sizeof(int), cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  int rc = enqueueEsdf(m, m->xyz_upload.get(), num_blocks, false, true, plane);
-  if (rc) return rc;
+  if ((rc = enqueueEsdf(m, m->xyz_upload.get(), num_blocks, false, true, plane))) return rc;
   if ((rc = nvb_mapper_synchronize(m))) return rc;
   return m->bounds.tightenEsdfBound(m->esdf, m->tsdf.capacity());
 }
@@ -3198,10 +3185,11 @@ int32_t nvb_layer_block_indices(NvbMapper* m, int32_t layer, int32_t* out_xyz_ho
 
 int32_t nvb_layer_get_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_host, int32_t n, void* out_host,
                              uint8_t* found_host) {
-  if (!m || (n > 0 && (!xyz_host || !out_host))) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (!m || (n > 0 && !out_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (int rc = takeBlockList(BlockList::kLookup, &xyz_host, &n)) return rc;
   const LayerSlab* L = layerOf(m, layer);
   if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "unknown layer");
-  if (n <= 0) return NVB_OK;
+  if (n == 0) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   std::vector<uint8_t> found_tmp(found_host ? 0 : n);  // the gather writes every block's flag
@@ -3218,14 +3206,17 @@ int32_t nvb_layer_get_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
 }
 
 int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_host, int32_t n, const void* in_host) {
-  if (!m || (n > 0 && (!xyz_host || !in_host))) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (!m || (n > 0 && !in_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  // Each index carries its own payload, so a repeat cannot be dropped; find-or-insert needs unique keys per launch.
+  std::vector<std::array<int, 3>> set;
+  const int32_t* unique = xyz_host;
+  int32_t n_unique = n;
+  if (int rc = takeBlockList(BlockList::kInsertSet, &unique, &n_unique, &set)) return rc;
+  if (n_unique != n) return fail(NVB_ERR_INVALID_ARGUMENT, "repeated block index");
   LayerSlab* L = layerOf(m, layer);
   if (!L) return fail(NVB_ERR_INVALID_ARGUMENT, "unknown layer");
-  if (n <= 0) return NVB_OK;
+  if (n == 0) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
-  for (int i = 0; i < n; i++)
-    if (!indexInRange(xyz_host[3 * i], xyz_host[3 * i + 1], xyz_host[3 * i + 2]))
-      return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
   const bool projective = L == &m->tsdf, esdf = L == &m->esdf;
   const int rc = projective ? reserveProjective(m, n) : esdf ? reserveEsdf(m, n) : reserveDerived(m, L, n);
   if (rc) return rc;
@@ -3607,27 +3598,6 @@ int meshUpdateImpl(NvbMapper* m, const int* xyz_dev, const TrackerList& todo, in
   return NVB_OK;
 }
 
-int uploadMeshList(NvbMapper* m, const int32_t* xyz_host, int n, int* out_unique) {
-  for (int i = 0; i < n; i++)
-    if (!indexInRange(xyz_host[3 * i], xyz_host[3 * i + 1], xyz_host[3 * i + 2]))
-      return fail(NVB_ERR_INDEX_RANGE, "block index outside +-2^20");
-  // a set, like the tracker's list in the reference (the mesh layer's find-or-insert needs unique keys per launch)
-  struct K3 {
-    int x, y, z;
-  };
-  std::vector<K3> v((size_t)n);
-  memcpy(v.data(), xyz_host, (size_t)n * sizeof(K3));
-  std::sort(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x != b.x ? a.x < b.x : (a.y != b.y ? a.y < b.y : a.z < b.z); });
-  v.erase(std::unique(v.begin(), v.end(), [](const K3& a, const K3& b) { return a.x == b.x && a.y == b.y && a.z == b.z; }), v.end());
-  const int u = (int)v.size();
-  const size_t ints = 3 * (size_t)u;
-  NVB_CUDA(m->mesh_xyz_dev.grow(m, ints, std::max(ints, 2 * m->mesh_xyz_dev.size())));
-  NVB_CUDA(cudaMemcpyAsync(m->mesh_xyz_dev.get(), v.data(), (size_t)u * sizeof(K3), cudaMemcpyHostToDevice, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));  // v dies with this scope
-  *out_unique = u;
-  return NVB_OK;
-}
-
 }  // namespace
 
 extern "C" {
@@ -3669,38 +3639,46 @@ int32_t nvb_mapper_update_mesh(NvbMapper* m, int32_t update_full_layer) {
 int32_t nvb_mesh_integrate_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks, int32_t update_color) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
   if (m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY) return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper has no TSDF layer");
-  if (num_blocks < 0 || (num_blocks > 0 && !blocks_xyz_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad block list");
+  // a set, like the tracker's list in the reference
+  std::vector<std::array<int, 3>> set;
+  int rc = takeBlockList(BlockList::kInsertSet, &blocks_xyz_host, &num_blocks, &set);
+  if (rc) return rc;
   NVB_CUDA(cudaSetDevice(m->device));
-  int rc;
   if ((rc = ensureMeshLayer(m))) return rc;
   if (num_blocks == 0) return NVB_OK;  // (:73-75)
-  int u = 0;
-  if ((rc = uploadMeshList(m, blocks_xyz_host, num_blocks, &u))) return rc;
-  if ((rc = meshUpdateImpl(m, m->mesh_xyz_dev.get(), TrackerList{}, u, update_color != 0))) return rc;
+  const size_t ints = 3 * (size_t)num_blocks;
+  NVB_CUDA(m->mesh_xyz_dev.grow(m, ints, std::max(ints, 2 * m->mesh_xyz_dev.size())));
+  NVB_CUDA(cudaMemcpyAsync(m->mesh_xyz_dev.get(), blocks_xyz_host, ints * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  if ((rc = meshUpdateImpl(m, m->mesh_xyz_dev.get(), TrackerList{}, num_blocks, update_color != 0))) return rc;
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   return checkDeviceError(m);
 }
 
 int32_t nvb_mesh_update_color(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
-  if (num_blocks < 0 || (num_blocks > 0 && !blocks_xyz_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad block list");
+  std::vector<std::array<int, 3>> set;
+  int rc = takeBlockList(BlockList::kInsertSet, &blocks_xyz_host, &num_blocks, &set);
+  if (rc) return rc;
   NVB_CUDA(cudaSetDevice(m->device));
-  int rc;
   if ((rc = ensureMeshLayer(m))) return rc;
   if (num_blocks == 0 || !m->mesh_v.get()) return NVB_OK;
-  int u = 0;
-  if ((rc = uploadMeshList(m, blocks_xyz_host, num_blocks, &u))) return rc;
+  const size_t ints = 3 * (size_t)num_blocks;
+  NVB_CUDA(m->mesh_xyz_dev.grow(m, ints, std::max(ints, 2 * m->mesh_xyz_dev.size())));
+  NVB_CUDA(cudaMemcpyAsync(m->mesh_xyz_dev.get(), blocks_xyz_host, ints * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
   MeshCtx c = makeMeshCtx(m);
-  c.in_xyz = m->mesh_xyz_dev.get(), c.in_count_host = u;
-  launchMeshColor(c, u, m->num_sms, m->stream);
+  c.in_xyz = m->mesh_xyz_dev.get(), c.in_count_host = num_blocks;
+  launchMeshColor(c, num_blocks, m->num_sms, m->stream);
   m->launches++;
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   return NVB_OK;
 }
 
 int32_t nvb_mesh_block_sizes(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks, int32_t* sizes_out) {
-  if (!m || (num_blocks > 0 && (!blocks_xyz_host || !sizes_out))) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (num_blocks <= 0) return NVB_OK;
+  if (!m || (num_blocks > 0 && !sizes_out)) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (int rc = takeBlockList(BlockList::kLookup, &blocks_xyz_host, &num_blocks)) return rc;
+  if (num_blocks == 0) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   for (int i = 0; i < 3 * num_blocks; i++) sizes_out[i] = -1;
   if (!m->mesh.exists()) return NVB_OK;
@@ -3721,8 +3699,9 @@ int32_t nvb_mesh_block_sizes(NvbMapper* m, const int32_t* blocks_xyz_host, int32
 
 int32_t nvb_mesh_get_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_t num_blocks, float* vertices_out,
                             float* normals_out, int32_t* triangles_out, uint8_t* colors_out, const int64_t caps[3]) {
-  if (!m || !caps || (num_blocks > 0 && !blocks_xyz_host)) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  if (num_blocks <= 0 || !m->mesh.exists()) return NVB_OK;
+  if (!m || !caps) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (int rc = takeBlockList(BlockList::kLookup, &blocks_xyz_host, &num_blocks)) return rc;
+  if (num_blocks == 0 || !m->mesh.exists()) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   const size_t n = (size_t)num_blocks;

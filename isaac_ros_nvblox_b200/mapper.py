@@ -108,12 +108,16 @@ def _shape_array(shapes):
     return arr, len(shapes)
 
 
-def _clear_shapes_call(fn, cap, *args):
-    """Run a shape-clearing entry point and return the touched (n, 3) block indices in (x, y, z) order."""
+def _block_list(fn, cap, *args, reread=None):
+    """Call fn(*args, out, cap, &n), which returns a list of n block indices with at most `cap` of them in `out`, and return
+    the (n, 3) int32 indices it wrote. A list longer than `cap` is read again in full through `reread`, (fn, *args) of an
+    entry point that returns the same list without changing the map; without one, the first `cap` indices are returned."""
     cap = max(int(cap), 1)
-    out = np.zeros((cap, 3), dtype=np.int32)
+    out = np.empty((cap, 3), dtype=np.int32)
     n = C.c_int32(0)
     check(fn(*args, _ip(out), cap, C.byref(n)))
+    if n.value > cap and reread is not None:
+        return _block_list(reread[0], n.value, *reread[1:])
     return out[:n.value].copy()
 
 
@@ -129,11 +133,7 @@ class _Layer:
         return n.value
 
     def get_all_block_indices(self):
-        n = self.num_blocks()
-        out = np.zeros((max(n, 1), 3), dtype=np.int32)
-        cnt = C.c_int32(0)
-        check(self._m._L.nvb_layer_block_indices(self._m._h, self._id, _ip(out), n, C.byref(cnt)))
-        return out[:n].copy()
+        return _block_list(self._m._L.nvb_layer_block_indices, self.num_blocks(), self._m._h, self._id)
 
     def slab_stats(self):
         """Storage of the layer: slab capacity, high-water mark and free-stack size in blocks, and the hash-table size."""
@@ -168,7 +168,7 @@ class _Layer:
         voxels whose centre lies in a BoundingSphere / AxisAlignedBoundingBox are reset. The tracker is not told. Returns the
         touched (n, 3) block indices in (x, y, z) order."""
         arr, n = _shape_array(shapes)
-        return _clear_shapes_call(self._m._L.nvb_layer_clear_shapes, self.num_blocks(), self._m._h, self._id, arr, n)
+        return _block_list(self._m._L.nvb_layer_clear_shapes, self.num_blocks(), self._m._h, self._id, arr, n)
 
     def block_device_ptr(self, index):
         k = np.asarray(index, dtype=np.int32)
@@ -585,11 +585,9 @@ class _MeshLayer:
 
     def get_all_block_indices(self):
         n = self.num_blocks()
-        out = np.zeros((max(n, 1), 3), dtype=np.int32)
-        if n:
-            cnt = C.c_int32(0)
-            check(self._m._L.nvb_layer_block_indices(self._m._h, _lib.NVB_LAYER_MESH, _ip(out), n, C.byref(cnt)))
-        return out[:n].copy()
+        if not n:  # no mesh update yet: the layer does not exist
+            return np.zeros((0, 3), dtype=np.int32)
+        return _block_list(self._m._L.nvb_layer_block_indices, n, self._m._h, _lib.NVB_LAYER_MESH)
 
     def block_sizes(self, indices):
         """(n,3) -> (n,3) int32 {vertices, triangle indices, colours}; -1 where there is no mesh block."""
@@ -1046,13 +1044,12 @@ class Mapper:
     def mark_unobserved_tsdf_free_inside_radius(self, center, radius):
         """Mapper::markUnobservedTsdfFreeInsideRadius(center, radius) (mapper.h:352-356) -> the blocks inside the radius."""
         c = np.ascontiguousarray(center, dtype=np.float32).reshape(3)
-        n = C.c_int32(0)
-        cap = 1 << 16
-        out = np.empty((cap, 3), dtype=np.int32)
-        check(self._L.nvb_mapper_mark_unobserved_free_inside_radius(self._h, _fp(c), float(radius), _ip(out), cap, C.byref(n)))
-        if n.value > cap:
-            raise RuntimeError("more than %d blocks inside the radius" % cap)
-        return out[:n.value].copy()
+        # room for every block of the sphere's block box, computed in float32 as the library bounds its own list; the call
+        # fails for a box of more than 2^26 blocks or a radius that is not positive
+        r, bs = np.float32(radius), np.float32(self.block_size())
+        cells = np.prod(np.floor((c + r) / bs) - np.floor((c - r) / bs) + 1, dtype=np.float64)
+        cap = int(cells) if 1 <= cells <= (1 << 26) else 1
+        return _block_list(self._L.nvb_mapper_mark_unobserved_free_inside_radius, cap, self._h, _fp(c), float(radius))
 
     def color_layer(self):
         return self._color
@@ -1089,17 +1086,13 @@ class Mapper:
             if mk.shape != c.shape[:2]:
                 raise ValueError("mask must have the colour image's size")
         T = colmajor(T_L_C)
-        cap = 1 << 14 if return_blocks else 0
-        n = C.c_int32(0)
-        out = np.empty((max(cap, 1), 3), dtype=np.int32)
-        check(self._L.nvb_mapper_integrate_color(self._h, c.ctypes.data, None if mk is None else mk.ctypes.data, mask_mode,
-                                                 _lib.NVB_MEM_HOST, c.shape[0], c.shape[1], _fp(T), C.byref(camera.c),
-                                                 _ip(out) if return_blocks else None, cap, C.byref(n)))
+        args = (self._h, c.ctypes.data, None if mk is None else mk.ctypes.data, mask_mode, _lib.NVB_MEM_HOST, c.shape[0],
+                c.shape[1], _fp(T), C.byref(camera.c))
         if not return_blocks:
+            check(self._L.nvb_mapper_integrate_color(*args, None, 0, None))
             return None
-        if n.value > cap:
-            raise RuntimeError("more than %d colour blocks in one frame" % cap)
-        return out[:n.value].copy()
+        return _block_list(self._L.nvb_mapper_integrate_color, 1 << 14, *args,
+                           reread=(self._L.nvb_mapper_last_color_blocks, self._h))
 
     def integrate_color_device(self, color_ptr, rows, cols, T_L_C, camera, mask_ptr=0, mask_mode=0):
         """Same, for an RGB frame already resident in HBM (raw device pointers); enqueued without synchronising."""
@@ -1111,9 +1104,7 @@ class Mapper:
         """updated_blocks of the last colour frame (after synchronize())."""
         n = C.c_int32(0)
         check(self._L.nvb_mapper_last_color_blocks(self._h, None, 0, C.byref(n)))
-        out = np.empty((max(n.value, 1), 3), dtype=np.int32)
-        check(self._L.nvb_mapper_last_color_blocks(self._h, _ip(out), n.value, C.byref(n)))
-        return out[:n.value].copy()
+        return _block_list(self._L.nvb_mapper_last_color_blocks, n.value, self._h)
 
     def freespace_integrator(self):
         return _FreespaceIntegrator(self)
@@ -1166,28 +1157,21 @@ class Mapper:
             x.has_exclusion_sphere = 1
             x.exclusion_center = (C.c_float * 3)(*[float(v) for v in exclusion_center])
             x.exclusion_radius_m = float(exclusion_radius_m)
-        n = C.c_int32(0)
-        cap = max(self._occupancy.num_blocks() if self._projective_layer_type == 1 else self._tsdf.num_blocks(), 1)
-        out = np.zeros((cap, 3), dtype=np.int32)
         if depth is not None:
             depth = np.ascontiguousarray(depth, dtype=np.float32)
             T = colmajor(T_L_C)
-            check(self._L.nvb_mapper_decay(self._h, C.byref(x), depth.ctypes.data, _lib.NVB_MEM_HOST, depth.shape[0],
-                                           depth.shape[1], _fp(T), C.byref(camera.c), _ip(out), cap, C.byref(n)))
+            view = (depth.ctypes.data, _lib.NVB_MEM_HOST, depth.shape[0], depth.shape[1], _fp(T), C.byref(camera.c))
         else:
-            check(self._L.nvb_mapper_decay(self._h, C.byref(x), None, 0, 0, 0, None, None, _ip(out), cap, C.byref(n)))
-        return out[:n.value].copy()
+            view = (None, 0, 0, 0, None, None)
+        return _block_list(self._L.nvb_mapper_decay, self._projective_num_blocks(), self._h, C.byref(x), *view)
 
     def clear_outside_radius(self, center, radius):
         """Mapper::clearOutsideRadius(center, radius) (mapper.h; src/mapper/mapper.cpp:473-492): deallocates every projective
         block farther than `radius` from `center`, with its ESDF, freespace, colour and mesh twins. Returns the removed (n, 3)
         block indices in (x, y, z) order."""
         c = np.ascontiguousarray(center, dtype=np.float32).reshape(3)
-        cap = max(self._occupancy.num_blocks() if self._projective_layer_type == 1 else self._tsdf.num_blocks(), 1)
-        out = np.zeros((cap, 3), dtype=np.int32)
-        n = C.c_int32(0)
-        check(self._L.nvb_mapper_clear_outside_radius(self._h, _fp(c), float(radius), _ip(out), cap, C.byref(n)))
-        return out[:n.value].copy()
+        return _block_list(self._L.nvb_mapper_clear_outside_radius, self._projective_num_blocks(), self._h, _fp(c),
+                           float(radius))
 
     def clear_tsdf_inside_shapes(self, shapes):
         """Mapper::clearTsdfInsideShapes(shapes) (src/mapper/mapper.cpp:364-368): TSDF voxels inside the shapes are reset and
@@ -1195,7 +1179,7 @@ class Mapper:
         mapper)."""
         arr, n = _shape_array(shapes)
         cap = self._tsdf.num_blocks() if self._projective_layer_type != ProjectiveLayerType.kOccupancy else 0
-        return _clear_shapes_call(self._L.nvb_mapper_clear_tsdf_inside_shapes, cap, self._h, arr, n)
+        return _block_list(self._L.nvb_mapper_clear_tsdf_inside_shapes, cap, self._h, arr, n)
 
     def get_cleared_blocks(self, blocks_to_ignore=()):
         """Mapper::getClearedBlocks(blocks_to_ignore) (src/mapper/mapper.cpp:509-521): the blocks deallocated by
@@ -1203,19 +1187,16 @@ class Mapper:
         ign = np.ascontiguousarray(np.asarray(blocks_to_ignore, dtype=np.int32).reshape(-1, 3))
         n = C.c_int32(0)
         check(self._L.nvb_mapper_get_cleared_blocks(self._h, None, 0, None, 0, C.byref(n)))
-        cap = max(n.value, 1)
-        out = np.zeros((cap, 3), dtype=np.int32)
-        check(self._L.nvb_mapper_get_cleared_blocks(self._h, _ip(ign) if len(ign) else None, len(ign), _ip(out), cap, C.byref(n)))
-        return out[:n.value].copy()
+        return _block_list(self._L.nvb_mapper_get_cleared_blocks, n.value, self._h, _ip(ign) if len(ign) else None, len(ign))
 
     def decay_exclude_last_view(self):
         """Mapper::decayTsdfExcludeLastView / decayOccupancyExcludeLastView with the view kept by the mapper
         (Mapper(..., keep_last_view=True))."""
-        n = C.c_int32(0)
-        cap = max(self._occupancy.num_blocks() if self._projective_layer_type == 1 else self._tsdf.num_blocks(), 1)
-        out = np.zeros((cap, 3), dtype=np.int32)
-        check(self._L.nvb_mapper_decay_exclude_last_view(self._h, None, _ip(out), cap, C.byref(n)))
-        return out[:n.value].copy()
+        return _block_list(self._L.nvb_mapper_decay_exclude_last_view, self._projective_num_blocks(), self._h, None)
+
+    def _projective_num_blocks(self):
+        """Blocks of the projective layer: a bound on what a decay or a clear removes."""
+        return (self._occupancy if self._projective_layer_type == ProjectiveLayerType.kOccupancy else self._tsdf).num_blocks()
 
     def decay_tsdf(self, **kw):
         assert self._projective_layer_type != ProjectiveLayerType.kOccupancy
@@ -1308,22 +1289,13 @@ class Mapper:
         """Mapper::integrateDepth. depth: (rows, cols) float32 host array. Returns updated_blocks (n,3)."""
         d, mk = self._frame_args(depth, mask)
         T = colmajor(T_L_C)
-        cap = 0
-        out = None
-        if return_blocks:
-            cap = 1 << 14
-            out = np.empty((cap, 3), dtype=np.int32)
-        n = C.c_int32(0)
-        check(self._L.nvb_mapper_integrate_depth(
-            self._h, d.ctypes.data, None if mk is None else mk.ctypes.data, mask_mode, _lib.NVB_MEM_HOST,
-            d.shape[0], d.shape[1], _fp(T), C.byref(camera.c), None if out is None else _ip(out), cap,
-            C.byref(n)))
-        if out is not None and n.value > cap:
-            # list longer than the buffer: the frame IS integrated; read the full list back
-            cap = n.value
-            out = np.empty((cap, 3), dtype=np.int32)
-            check(self._L.nvb_mapper_last_frame_blocks(self._h, _ip(out), cap, C.byref(n)))
-        return None if out is None else out[:n.value].copy()
+        args = (self._h, d.ctypes.data, None if mk is None else mk.ctypes.data, mask_mode, _lib.NVB_MEM_HOST, d.shape[0],
+                d.shape[1], _fp(T), C.byref(camera.c))
+        if not return_blocks:
+            check(self._L.nvb_mapper_integrate_depth(*args, None, 0, None))
+            return None
+        return _block_list(self._L.nvb_mapper_integrate_depth, 1 << 14, *args,
+                           reread=(self._L.nvb_mapper_last_frame_blocks, self._h))
 
     def integrate_depth_device(self, depth_ptr, rows, cols, T_L_C, camera, mask_ptr=0, mask_mode=0, sync=False):
         """Same, for a frame already resident in HBM (raw device pointers). Asynchronous unless sync."""
@@ -1401,14 +1373,7 @@ class ViewCalculator:
                                          max_integration_distance_behind_surface_m, max_integration_distance_m):
         d = np.ascontiguousarray(depth, dtype=np.float32)
         T = colmajor(T_L_C)
-        cap = 1 << 16
-        while True:
-            out = np.zeros((cap, 3), dtype=np.int32)
-            n = C.c_int32(0)
-            check(self._m._L.nvb_view_raycast(self._m._h, d.ctypes.data, _lib.NVB_MEM_HOST, d.shape[0], d.shape[1],
-                                              _fp(T), C.byref(camera.c), float(block_size),
-                                              float(max_integration_distance_behind_surface_m),
-                                              float(max_integration_distance_m), _ip(out), cap, C.byref(n)))
-            if n.value <= cap:
-                return out[:n.value].copy()
-            cap = n.value
+        L, h = self._m._L, self._m._h
+        return _block_list(L.nvb_view_raycast, 1 << 16, h, d.ctypes.data, _lib.NVB_MEM_HOST, d.shape[0], d.shape[1], _fp(T),
+                           C.byref(camera.c), float(block_size), float(max_integration_distance_behind_surface_m),
+                           float(max_integration_distance_m), reread=(L.nvb_mapper_last_frame_blocks, h))
