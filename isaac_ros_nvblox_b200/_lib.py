@@ -43,7 +43,7 @@ EXPORTED_SYMBOLS = [
     "nvb_mapper_stream", "nvb_mapper_join_streams", "nvb_blocks_union",
     "nvb_layer_num_blocks", "nvb_layer_block_indices", "nvb_layer_slab_stats", "nvb_layer_get_blocks",
     "nvb_layer_set_blocks", "nvb_layer_block_device_ptr", "nvb_layer_block_bytes",
-    "nvb_mapper_last_esdf_stats", "nvb_mapper_set_cache_last_viewpoint", "nvb_mapper_get_cache_last_viewpoint", "nvb_mapper_set_depth_preprocessing", "nvb_mapper_get_depth_preprocessing", "nvb_depth_dilate_invalid", "nvb_esdf_slice_aabb", "nvb_esdf_slice_distance_image_in_aabb", "nvb_mapper_set_esdf_reserved_sms", "nvb_mapper_get_esdf_reserved_sms", "nvb_default_mesh_params", "nvb_mapper_set_mesh_params", "nvb_mapper_get_mesh_params", "nvb_mapper_update_mesh", "nvb_mesh_integrate_blocks", "nvb_mesh_update_color", "nvb_mesh_block_sizes", "nvb_mesh_get_blocks", "nvb_mesh_arena_stats", "nvb_mapper_append_frame_blocks", "nvb_blocks_union_segments", "nvb_blocks_union_status", "nvb_mapper_esdf_time_split", "nvb_mapper_esdf_clear_blocks_read", "nvb_mapper_debug_phase_max", "nvb_mapper_enable_profiling", "nvb_mapper_stage_times",
+    "nvb_mapper_last_esdf_stats", "nvb_mapper_set_cache_last_viewpoint", "nvb_mapper_get_cache_last_viewpoint", "nvb_mapper_set_depth_preprocessing", "nvb_mapper_get_depth_preprocessing", "nvb_depth_dilate_invalid", "nvb_esdf_slice_aabb", "nvb_esdf_dense_grid_in_aabb", "nvb_esdf_slice_distance_image_in_aabb", "nvb_mapper_set_esdf_reserved_sms", "nvb_mapper_get_esdf_reserved_sms", "nvb_default_mesh_params", "nvb_mapper_set_mesh_params", "nvb_mapper_get_mesh_params", "nvb_mapper_update_mesh", "nvb_mesh_integrate_blocks", "nvb_mesh_update_color", "nvb_mesh_block_sizes", "nvb_mesh_get_blocks", "nvb_mesh_arena_stats", "nvb_mapper_append_frame_blocks", "nvb_blocks_union_segments", "nvb_blocks_union_status", "nvb_mapper_esdf_time_split", "nvb_mapper_esdf_clear_blocks_read", "nvb_mapper_debug_phase_max", "nvb_mapper_enable_profiling", "nvb_mapper_stage_times",
     "nvb_mapper_kernel_launches", "nvb_mapper_esdf_split_stats",
     "nvb_mapper_clear_outside_radius", "nvb_mapper_clear_tsdf_inside_shapes", "nvb_layer_clear_shapes",
     "nvb_mapper_get_cleared_blocks",
@@ -302,6 +302,7 @@ def load(path=None):
     L.nvb_mapper_get_depth_preprocessing.argtypes = [vp, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     L.nvb_depth_dilate_invalid.argtypes = [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float]
     L.nvb_esdf_slice_aabb.argtypes = [vp, C.c_float, C.POINTER(C.c_float), C.POINTER(C.c_int32)]
+    L.nvb_esdf_dense_grid_in_aabb.argtypes = [vp, C.POINTER(C.c_float), C.c_float, i32, vp, C.c_int64, ip, ip]
     L.nvb_esdf_slice_distance_image_in_aabb.argtypes = [vp, C.c_float, C.c_float, C.POINTER(C.c_float), vp, vp, C.c_int32,
                                                         C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     L.nvb_mapper_set_esdf_reserved_sms.argtypes = [vp, C.c_int32]

@@ -12,7 +12,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libnvblox_b200.so")
 SOURCES = ["nvb_api.cu", "nvb_view.cu", "nvb_tsdf.cu", "nvb_esdf.cu", "nvb_esdf_wave.cu", "nvb_esdf_wavex.cu", "nvb_util.cu", "nvb_merge.cu", "nvb_color.cu", "nvb_mesh.cu", "nvb_clear.cu", "nvb_ground.cu", "nvb_dynamics.cu", "nvb_query.cu", "nvb_masker.cu", "nvb_map_io.cu", "nvb_scene.cu"]
-HEADERS = [os.path.join(CSRC, "nvb_internal.cuh"), os.path.join(CSRC, "nvb_esdf_common.cuh"), os.path.join(CSRC, "nvb_esdf_wave_common.cuh"), os.path.join(CSRC, "nvb_tma.cuh"), os.path.join(CSRC, "nvb_mc_table.h"), os.path.join(ROOT, "include", "nvblox_b200.h")]
+HEADERS = [os.path.join(CSRC, "nvb_internal.cuh"), os.path.join(CSRC, "nvb_esdf_block.cuh"), os.path.join(CSRC, "nvb_esdf_common.cuh"), os.path.join(CSRC, "nvb_esdf_wave_common.cuh"), os.path.join(CSRC, "nvb_tma.cuh"), os.path.join(CSRC, "nvb_mc_table.h"), os.path.join(ROOT, "include", "nvblox_b200.h")]
 
 
 def nvcc_path():

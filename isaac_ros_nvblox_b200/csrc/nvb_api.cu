@@ -17,7 +17,7 @@
 #include <string>
 #include <vector>
 
-#include "nvb_internal.cuh"
+#include "nvb_esdf_block.cuh"
 
 using namespace nvb;
 
@@ -2934,6 +2934,46 @@ int32_t nvb_esdf_slice_distance_image_in_aabb(NvbMapper* m, float slice_height_m
   return NVB_OK;
 }
 
+// robustFloor (nvblox map/internal/cuda/impl/layer_to_3d_grid_impl.cuh): an integer stored as a float with a rounding error
+// below 1e-4 is that integer, anything else floors.
+static int robustFloor(float x) {
+  const int nearest = (int)std::round(x);
+  return std::abs(x - (float)nearest) < 1e-4f ? nearest : (int)std::floor(x);
+}
+
+int32_t nvb_esdf_dense_grid_in_aabb(NvbMapper* m, const float aabb[6], float default_value, int32_t memory, float* out,
+                                    int64_t cap, int32_t min_index_out[3], int32_t dims_out[3]) {
+  if (!m || !aabb || !min_index_out || !dims_out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
+  if (int rc = checkMemoryKind(memory)) return rc;
+  for (int a = 0; a < 3; a++) min_index_out[a] = 0, dims_out[a] = 0;
+  for (int a = 0; a < 6; a++)
+    if (!std::isfinite(aabb[a])) return fail(NVB_ERR_INVALID_ARGUMENT, "non-finite AABB");
+  const float inv_voxel_size = 1.0f / m->voxel_size;
+  int mn[3], dims[3];
+  long long cells = 1;
+  for (int a = 0; a < 3; a++) {
+    mn[a] = robustFloor(aabb[a] * inv_voxel_size);
+    const long long d = (long long)robustFloor(aabb[3 + a] * inv_voxel_size) - mn[a] + 1;
+    if (d <= 0) return NVB_OK;  // an empty box: no cells
+    if (d > 65535ll * kVps) return fail(NVB_ERR_CAPACITY, "dense grid longer than 65535 blocks along an axis");
+    dims[a] = (int)d, cells *= d;
+  }
+  if (cells > 0x7fffffffll) return fail(NVB_ERR_CAPACITY, "dense grid with more than 2^31 cells");
+  for (int a = 0; a < 3; a++) min_index_out[a] = mn[a], dims_out[a] = dims[a];
+  if (!out || cap < cells) return NVB_OK;  // the size only
+  NVB_CUDA(cudaSetDevice(m->device));
+  NVB_CUDA(syncAll(m));
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  float* out_dev;
+  NVB_CUDA(bufs.out(out, (size_t)cells * sizeof(float), &out_dev));
+  launchEsdfDenseGrid(m->esdf.dev(), make_int3(mn[0], mn[1], mn[2]), make_int3(dims[0], dims[1], dims[2]), m->voxel_size,
+                      default_value, out_dev, m->stream);
+  m->launches++;
+  NVB_CUDA(bufs.finish());
+  if (memory == NVB_MEM_DEVICE) NVB_CUDA(cudaStreamSynchronize(m->stream));
+  return NVB_OK;
+}
+
 int32_t nvb_esdf_slice_distance_image(NvbMapper* m, float slice_height_m, float unobserved_value, float aabb_out[6],
                                       float* image_host, int8_t* grid_host, int32_t cap_pixels, int32_t* rows_out,
                                       int32_t* cols_out) {
@@ -3199,7 +3239,7 @@ int32_t nvb_layer_get_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
   NVB_CUDA(host.in(xyz_host, (size_t)n * 3 * sizeof(int), &xyz_dev));
   NVB_CUDA(host.out(static_cast<unsigned char*>(out_host), (size_t)n * L->dev().block_bytes, &out_dev));
   NVB_CUDA(host.out(found_host ? found_host : found_tmp.data(), (size_t)n, &found_dev));
-  launchGatherBlocks(L->dev(), xyz_dev, n, out_dev, found_dev, m->stream);
+  launchGatherBlocks(L->dev(), L == &m->esdf, xyz_dev, n, out_dev, found_dev, m->stream);
   m->launches++;
   NVB_CUDA(host.finish());
   return NVB_OK;
@@ -3226,7 +3266,7 @@ int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
   const unsigned char* in_dev;
   NVB_CUDA(host.in(xyz_host, (size_t)n * 3 * sizeof(int), &xyz_dev));
   NVB_CUDA(host.in(static_cast<const unsigned char*>(in_host), (size_t)n * L->dev().block_bytes, &in_dev));
-  launchScatterBlocks(L->dev(), xyz_dev, n, in_dev, m->error_dev, m->stream);
+  launchScatterBlocks(L->dev(), esdf, xyz_dev, n, in_dev, m->error_dev, m->stream);
   m->launches++;
   if (esdf) m->prune_ok = false;  // voxels written from outside: the parent boxes are no longer bounds
   NVB_CUDA(syncAll(m));
@@ -3299,6 +3339,7 @@ int32_t nvb_mapper_save_map(NvbMapper* m, const char* path) {
     voxels[k].resize((size_t)hw * L->block_bytes);
     NVB_CUDA(cudaMemcpy(xyz[k].data(), L->block_index, xyz[k].size() * sizeof(int), cudaMemcpyDeviceToHost));
     NVB_CUDA(cudaMemcpy(voxels[k].data(), L->blocks, voxels[k].size(), cudaMemcpyDeviceToHost));
+    if (S == &m->esdf) esdfBlocksToRecords(voxels[k].data(), (size_t)hw);  // the file holds EsdfVoxel records
     const int* b = xyz[k].data();
     for (int sl = 0; sl < hw; sl++)
       if (b[3 * sl] != kDeadSlotX) order[k].push_back(sl);
@@ -3317,6 +3358,7 @@ int32_t nvb_mapper_save_map(NvbMapper* m, const char* path) {
 static int uploadLoadedLayer(NvbMapper* m, LayerSlab* S, const MapFileLayerIn& in) {
   if (in.n == 0) return NVB_OK;
   const DevLayer& L = S->dev();
+  if (S == &m->esdf) esdfBlocksFromRecords(in.voxels.get(), (size_t)in.n);  // the file holds EsdfVoxel records
   NVB_CUDA(cudaMemcpyAsync(L.blocks, in.voxels.get(), (size_t)in.n * L.block_bytes, cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaMemcpyAsync(L.block_index, in.xyz.data(), in.xyz.size() * sizeof(int), cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaMemcpyAsync(L.count, &in.n, sizeof(int), cudaMemcpyHostToDevice, m->stream));
@@ -3866,7 +3908,7 @@ int32_t nvb_layer_query_voxels(NvbMapper* m, int32_t layer, const float* xyz, in
   const int voxel_bytes = q.layer.block_bytes / kVpb;
   return runLayerQuery(m, xyz, memory, n, out_voxels, (size_t)voxel_bytes, out_success,
                        [&](const float* x, void* o, uint8_t* f, cudaStream_t st) {
-                         launchQueryVoxels(q, voxel_bytes, x, n, o, f, m->num_sms, st);
+                         launchQueryVoxels(q, voxel_bytes, L == &m->esdf, x, n, o, f, m->num_sms, st);
                        });
 }
 

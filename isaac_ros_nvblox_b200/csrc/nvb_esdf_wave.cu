@@ -398,24 +398,28 @@ __global__ void __maxnreg__(NVB_WAVE_MAXREG) esdfWaveGesKernel(EsdfCtx c) {
             int pos = -1;
             {
               const int a = lane64 >> 3, b = lane64 & 7;
-              sweepLineRegs(R, regionWord(1, a + 1, b + 1), 400, 0, a, b, 0, c.max_sq);
+              sweepLineRegs(R, kRegionFlagWord0, regionVox(1, a + 1, b + 1), 80, 0, a, b, 0, c.max_sq);
               groupSync(group);
               // the exchange is back by now; the position fetch overlaps the other two axes
               if (nb >= 0 && old != ring + 1) pos = atomicAdd(ccount + ni, 1);
-              sweepLineRegs(R, regionWord(a + 1, 1, b + 1), 40, a, 0, b, 1, c.max_sq);
+              sweepLineRegs(R, kRegionFlagWord0, regionVox(a + 1, 1, b + 1), 8, a, 0, b, 1, c.max_sq);
               groupSync(group);
-              sweepLineRegs(R, regionWord(a + 1, b + 1, 1), kEsdfVoxelWords, a, b, 0, 2, c.max_sq);
+              sweepLineRegs(R, kRegionFlagWord0, regionVox(a + 1, b + 1, 1), 1, a, b, 0, 2, c.max_sq);
               groupSync(group);
             }
             if (pos >= 0) clist[ni][pos] = nb;
             // inner 8x8x8 -> shadow slab
-            uint4* dst = reinterpret_cast<uint4*>(c.shadow + (size_t)slot * kEsdfBlockBytes);
+            unsigned int* dst = reinterpret_cast<unsigned int*>(c.shadow + (size_t)slot * kEsdfBlockBytes);
 #pragma unroll
             for (int it = 0; it < 2; it++) {
-              const int r = it * 32 + (lane64 >> 1);  // block row (lx, ly); two lanes share a row
-              const unsigned int* srow = R + (((r >> 3) + 1) * 10 + (r & 7) + 1) * 40 + (lane64 & 1) * 4;
+              const int r = it * 32 + (lane64 >> 1), half = lane64 & 1;  // block z-row (lx, ly); two lanes share a row
+              const int zr = ((r >> 3) + 1) * 10 + (r & 7) + 1;
 #pragma unroll
-              for (int j = 0; j < 5; j++) __stcg(dst + r * 10 + (lane64 & 1) + 2 * j, *reinterpret_cast<const uint4*>(srow + j * 8));
+              for (int j = 0; j < 4; j++)
+                __stcg(reinterpret_cast<uint4*>(esdfCell(dst, r * 8 + 2 * j + half)),
+                       *reinterpret_cast<const uint4*>(esdfCell(R, zr * 8 + 2 * j + half)));
+              __stcg(reinterpret_cast<uint4*>(esdfFlag(dst, r * 8 + 4 * half)),
+                     *reinterpret_cast<const uint4*>(R + kRegionFlagWord0 + zr * 8 + 4 * half));
             }
           }
           groupSync(group);

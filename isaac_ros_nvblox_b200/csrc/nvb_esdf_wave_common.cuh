@@ -92,20 +92,21 @@ __device__ __forceinline__ void prefetchNeighbors(const EsdfCtx& c, WaveShared<W
 // The line's 8 voxels are loaded once, walked forward, the register image is reversed and walked again
 // (= the backward pass); changed voxels are written back. `axis` and `pass` are run-time values so that
 // ONE copy of the 8-step body serves all six passes.
-// `sm` is the block image in shared memory, base_w the word offset of the line's first voxel, stride_w the word
-// stride along the line; (c0,c1,c2) are the voxel coordinates at position 0.
-__device__ __forceinline__ bool sweepLineRegs(unsigned int* sm, int base_w, int stride_w, int c0, int c1, int c2,
+// `sm` is a split image in shared memory (a block: nvb_esdf_block.cuh, or a gather region): voxel u's cell at words
+// [4 u, 4 u + 4), its flag word at flag_w + u. v0 is the line's first voxel, stride the voxel stride along the line;
+// (c0,c1,c2) are the voxel coordinates at position 0.
+__device__ __forceinline__ bool sweepLineRegs(unsigned int* sm, int flag_w, int v0, int stride, int c0, int c1, int c2,
                                               int axis, float max_sq) {
   int T[kVps];  // ceil(squared distance): sq > n  <=>  T > n for every integer n
   int p0[kVps], p1[kVps], p2[kVps];
   unsigned int obs = 0, site = 0, valid = 0, dirty = 0;
 #pragma unroll
   for (int i = 0; i < kVps; i++) {
-    const unsigned int* e = sm + base_w + i * stride_w;
-    const float sq = __uint_as_float(e[0]);
+    const uint4 e = *reinterpret_cast<const uint4*>(sm + kEsdfCellWords * (v0 + i * stride));
+    const float sq = __uint_as_float(e.x);
     T[i] = __float2int_ru(sq);
-    p0[i] = (int)e[1], p1[i] = (int)e[2], p2[i] = (int)e[3];
-    const unsigned int fl = e[4];
+    p0[i] = (int)e.y, p1[i] = (int)e.z, p2[i] = (int)e.w;
+    const unsigned int fl = sm[flag_w + v0 + i * stride];
     if (flagObserved(fl)) obs |= 1u << i;
     if (flagSite(fl)) site |= 1u << i;
     if (sq < max_sq) valid |= 1u << i;
@@ -152,9 +153,8 @@ __device__ __forceinline__ bool sweepLineRegs(unsigned int* sm, int base_w, int 
 #pragma unroll
   for (int i = 0; i < kVps; i++) {
     if ((dirty >> i) & 1u) {
-      unsigned int* e = sm + base_w + i * stride_w;
-      e[0] = __float_as_uint((float)T[i]);
-      e[1] = (unsigned)p0[i], e[2] = (unsigned)p1[i], e[3] = (unsigned)p2[i];
+      *reinterpret_cast<uint4*>(sm + kEsdfCellWords * (v0 + i * stride)) =
+          make_uint4(__float_as_uint((float)T[i]), (unsigned)p0[i], (unsigned)p1[i], (unsigned)p2[i]);
     }
   }
   return dirty != 0;
@@ -185,7 +185,7 @@ __device__ NVB_WAVE_FN void sweepMembers(const EsdfCtx& c, WaveShared<WT>& sh, i
       const int c1 = (axis == 0) ? a : ((axis == 1) ? 0 : b);
       const int c2 = (axis == 2) ? 0 : b;
       if (slot >= 0)
-        ch |= sweepLineRegs(sm, v0 * kEsdfVoxelWords, stride * kEsdfVoxelWords, c0, c1, c2, axis, c.max_sq);
+        ch |= sweepLineRegs(sm, kEsdfFlagWord0, v0, stride, c0, c1, c2, axis, c.max_sq);
       __syncthreads();
     }
     if (ch) sh.changed[group] = 1;
@@ -223,23 +223,23 @@ __device__ NVB_WAVE_FN void axisMembers(const EsdfCtx& c, WaveShared<WT>& sh, in
       unsigned int* blkA = esdfBlockPtr(c.esdf, side == 0 ? mine : other);
       unsigned int* blkB = esdfBlockPtr(c.esdf, side == 0 ? other : mine);
       VoxelRegs A[2], B[2];
-      unsigned int *gHi[2], *gLo[2];
+      int vHi[2], vLo[2];
 #pragma unroll
       for (int h = 0; h < 2; h++) {
         const int f = lane + 32 * h, u = f >> 3, w = f & 7;
         const int faceBase = (axis == 0) ? (u * 8 + w) : ((axis == 1) ? (u * 64 + w) : (u * 64 + w * 8));
-        gHi[h] = blkA + (faceBase + (kVps - 1) * strideA) * kEsdfVoxelWords;
-        gLo[h] = blkB + faceBase * kEsdfVoxelWords;
-        A[h] = loadVoxel(gHi[h]);
-        B[h] = loadVoxel(gLo[h]);
+        vHi[h] = faceBase + (kVps - 1) * strideA;
+        vLo[h] = faceBase;
+        A[h] = loadVoxel(blkA, vHi[h]);
+        B[h] = loadVoxel(blkB, vLo[h]);
       }
 #pragma unroll
       for (int h = 0; h < 2; h++) {
         if (side == 0) {
-          updB |= updateSingleNeighbor(A[h], B[h], gLo[h], axis, +1, c.max_sq);  // P: mine -> mine + d
-          if (other_stamp == ring) updA |= updateSingleNeighbor(B[h], A[h], gHi[h], axis, -1, c.max_sq);  // Q
+          updB |= updateSingleNeighbor(A[h], B[h], blkB, vLo[h], axis, +1, c.max_sq);  // P: mine -> mine + d
+          if (other_stamp == ring) updA |= updateSingleNeighbor(B[h], A[h], blkA, vHi[h], axis, -1, c.max_sq);  // Q
         } else if (other_stamp != ring) {
-          updA |= updateSingleNeighbor(B[h], A[h], gHi[h], axis, -1, c.max_sq);  // Q: mine -> mine - d
+          updA |= updateSingleNeighbor(B[h], A[h], blkA, vHi[h], axis, -1, c.max_sq);  // Q: mine -> mine - d
         }
       }
     }
@@ -344,15 +344,14 @@ __device__ NVB_WAVE_FN int flushLocal(WaveShared<WT>& sh, int* stamp_nxt, int ri
 // shadow slab until every CTA has finished reading the old state (barrier), then copied over the layer while
 // the next ring's candidates and their neighbour rows are fetched (barrier).
 // =====================================================================================================
-// Region layout (words): "core" = the 10 x 10 z-rows (rx, ry) of the 8 voxels rz = 1..8, 40 words each, in
-// the same order as in a block -- so runs of rows that are contiguous in their source block are contiguous here
-// and move with ONE TMA bulk copy (30 copies per region); then the two z-halo planes rz = 0 and rz = 9, one
-// 8-word cell per voxel, padded so that four of the five voxel words are a 16-byte aligned chunk on both sides.
-constexpr int kCoreWords = 100 * 40;
-constexpr int kZCell = 8;
-constexpr int kZLoBase = kCoreWords;                 // cell: [pad x3][w0][w1 w2 w3 w4]
-constexpr int kZHiBase = kCoreWords + 100 * kZCell;  // cell: [w0 w1 w2 w3][w4][pad x3]
-constexpr int kRegionWords = kCoreWords + 200 * kZCell;  // 5600
+// Region layout: split like a block (nvb_esdf_block.cuh), a plane of 16-byte cells then a plane of flag words, over 1 000
+// region voxels: "core" = the 10 x 10 z-rows zr = rx * 10 + ry of the 8 voxels rz = 1..8 (voxel zr * 8 + rz - 1), so a
+// z-row's cells (128 bytes) and flags (32 bytes) are contiguous here as in their source block; then the two z-halo planes
+// rz = 0 and rz = 9 (voxels 800 + zr and 900 + zr).
+constexpr int kZLoVox = 800;
+constexpr int kZHiVox = 900;
+constexpr int kRegionFlagWord0 = 1000 * kEsdfCellWords;  // word offset of the flag plane
+constexpr int kRegionWords = kRegionFlagWord0 + 1000;   // 5000
 constexpr int kGesMaxCand = 32;                 // candidates of one CTA per chunk
 constexpr int kGesDoneMax = 64;                 // changed blocks remembered per 64-thread group and ring
 template <int WT>
@@ -361,9 +360,9 @@ constexpr size_t gesSmemBytes() { return (size_t)(WT / 64) * kRegionWords * size
 template <int WT>
 struct GesShared {
   // per-lane constants of the gather and of the pass replay (the same for every candidate): packed descriptors
-  unsigned int tz[4][64];  // z-halo voxel copies:  d27 | hi << 5 | zr << 6 | src_off << 13 | valid << 27
-  unsigned int tc[4][64];  // core row copies:      d27 | zr << 6 | src_off << 13 | valid << 27
-  unsigned int te[6][4][64];  // boundary pairs per pass: src word | dst word << 13 | d27 << 26 | inner << 31; 0 = none
+  unsigned int tz[4][64];  // z-halo voxel copies:  d27 | hi << 5 | zr << 6 | src voxel << 13 | valid << 27
+  unsigned int tc[4][64];  // core row copies:      d27 | zr << 6 | src z-row << 13 | valid << 27
+  unsigned int te[6][4][64];  // boundary pairs per pass: src voxel | dst voxel << 13 | d27 << 26 | inner << 31; 0 = none
   int cand[kGesMaxCand];
   int rows[kGesMaxCand * 27];
   int done_slots[(WT / 64)][kGesDoneMax];
@@ -381,20 +380,18 @@ __device__ __forceinline__ void cpAsync16(unsigned int* smem_dst, const void* gs
 }
 __device__ __forceinline__ void cpAsyncWaitAll() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-__device__ __forceinline__ int regionWord(int rx, int ry, int rz) {
+__device__ __forceinline__ int regionVox(int rx, int ry, int rz) {
   const int zr = rx * 10 + ry;
-  return rz == 0 ? (kZLoBase + zr * kZCell + 3) : (rz == 9 ? (kZHiBase + zr * kZCell) : (zr * 40 + (rz - 1) * kEsdfVoxelWords));
+  return rz == 0 ? (kZLoVox + zr) : (rz == 9 ? (kZHiVox + zr) : (zr * 8 + rz - 1));
 }
 // region coordinate (0..9) -> block offset (-1, 0, +1) and voxel coordinate inside that block
 __device__ __forceinline__ int regOff(int r) { return r == 0 ? -1 : (r == 9 ? 1 : 0); }
 __device__ __forceinline__ int regLoc(int r) { return r == 0 ? 7 : (r == 9 ? 0 : r - 1); }
 
 // Region of a candidate block <- the 27 blocks of `row` (slots; < 0 = not allocated -> zeros = unobserved voxels).
-// All bulk traffic is 16-byte cp.async.cg (L2 -> shared, no L1, no registers). Core: a z-row is 160 contiguous,
-// 16-byte aligned bytes on both sides; two neighbouring lanes take alternate chunks of one row, so every request
-// of a warp covers whole 32-byte sectors, and the row is decoded once per five copies. z-halo planes: per voxel one
-// aligned chunk plus one word. (A TMA bulk-copy version would issue 30 copies per region from 30 lanes; the expectation that the
-// per-lane issue of those copies costs more than the address arithmetic it saves is design reasoning, not measured on the H100.)
+// All bulk traffic is 16-byte cp.async.cg (L2 -> shared, no L1, no registers). Core: a z-row is 8 cells (128 bytes) and 8
+// flag words (32 bytes), contiguous and 16-byte aligned on both sides; two neighbouring lanes take alternate chunks of one
+// row, and the row is decoded once per five copies. z-halo planes: per voxel one cell plus one flag word.
 template <int WT>
 __device__ __forceinline__ void gesInitTables(GesShared<WT>& gs, int tid) {
   if (tid < 64) {
@@ -406,7 +403,7 @@ __device__ __forceinline__ void gesInitTables(GesShared<WT>& gs, int tid) {
           const int zr = t >> 1, hi = t & 1;  // hi: rz = 9 <- block +z, voxel z = 0; lo: rz = 0 <- block -z, voxel z = 7
           const int rx = zr / 10, ry = zr % 10;
           const int d = (regOff(rx) + 1) * 9 + (regOff(ry) + 1) * 3 + (hi ? 2 : 0);
-          const int off = ((regLoc(rx) * 8 + regLoc(ry)) * 8 + (hi ? 0 : 7)) * 20;
+          const int off = (regLoc(rx) * 8 + regLoc(ry)) * 8 + (hi ? 0 : 7);  // source voxel
           v = (unsigned)d | ((unsigned)hi << 5) | ((unsigned)zr << 6) | ((unsigned)off << 13) | (1u << 27);
         }
         gs.tz[j][tid] = v;
@@ -417,7 +414,7 @@ __device__ __forceinline__ void gesInitTables(GesShared<WT>& gs, int tid) {
         if (zr < 100) {
           const int rx = zr / 10, ry = zr % 10;
           const int d = (regOff(rx) + 1) * 9 + (regOff(ry) + 1) * 3 + 1;
-          const int off = (regLoc(rx) * 8 + regLoc(ry)) * 160 + (tid & 1) * 16;
+          const int off = regLoc(rx) * 8 + regLoc(ry);  // source z-row
           v = (unsigned)d | ((unsigned)zr << 6) | ((unsigned)off << 13) | (1u << 27);
         }
         gs.tc[j][tid] = v;
@@ -434,8 +431,8 @@ __device__ __forceinline__ void gesInitTables(GesShared<WT>& gs, int tid) {
           const int da = sa + dir;
           const int d = 13 + so * A + regOff(u) * U + regOff(w) * W;
           const int inner = da >= 1 && da <= 8 && u >= 1 && u <= 8 && w >= 1 && w <= 8;
-          const int sw = axis == 0 ? regionWord(sa, u, w) : (axis == 1 ? regionWord(u, sa, w) : regionWord(u, w, sa));
-          const int dw = axis == 0 ? regionWord(da, u, w) : (axis == 1 ? regionWord(u, da, w) : regionWord(u, w, da));
+          const int sw = axis == 0 ? regionVox(sa, u, w) : (axis == 1 ? regionVox(u, sa, w) : regionVox(u, w, sa));
+          const int dw = axis == 0 ? regionVox(da, u, w) : (axis == 1 ? regionVox(u, da, w) : regionVox(u, w, da));
           v = (unsigned)sw | ((unsigned)dw << 13) | ((unsigned)d << 26) | ((unsigned)inner << 31);
         }
         gs.te[pass][j][tid] = v;
@@ -453,15 +450,10 @@ __device__ __forceinline__ void gesGather(const EsdfCtx& c, const GesShared<WT>&
     const unsigned int t = gs.tz[j][lane64];
     zw[j] = 0;
     if (t >> 27) {
-      const int slot = row[t & 31u], hi = (t >> 5) & 1u, zr = (t >> 6) & 127u;
-      const unsigned char* vox = c.esdf.blocks + (size_t)(slot < 0 ? 0 : slot) * kEsdfBlockBytes + ((t >> 13) & 16383u);
-      if (hi) {
-        cpAsync16(R + kZHiBase + zr * kZCell, vox, slot >= 0);  // words 0..3
-        if (slot >= 0) zw[j] = __ldcg(reinterpret_cast<const unsigned int*>(vox + 16));
-      } else {
-        cpAsync16(R + kZLoBase + zr * kZCell + 4, vox + 4, slot >= 0);  // words 1..4
-        if (slot >= 0) zw[j] = __ldcg(reinterpret_cast<const unsigned int*>(vox));
-      }
+      const int slot = row[t & 31u], hi = (t >> 5) & 1u, zr = (t >> 6) & 127u, v = (t >> 13) & 511u;
+      const unsigned int* blk = esdfBlockPtr(c.esdf, slot < 0 ? 0 : slot);
+      cpAsync16(esdfCell(R, (hi ? kZHiVox : kZLoVox) + zr), esdfCell(blk, v), slot >= 0);
+      if (slot >= 0) zw[j] = __ldcg(esdfFlag(blk, v));
     }
   }
   const int half = lane64 & 1;
@@ -469,11 +461,12 @@ __device__ __forceinline__ void gesGather(const EsdfCtx& c, const GesShared<WT>&
   for (int it = 0; it < 4; it++) {
     const unsigned int t = gs.tc[it][lane64];
     if (t >> 27) {
-      const int slot = row[t & 31u], zr = (t >> 6) & 127u;
-      const unsigned char* src = c.esdf.blocks + (size_t)(slot < 0 ? 0 : slot) * kEsdfBlockBytes + ((t >> 13) & 16383u);
-      unsigned int* dst = R + zr * 40 + half * 4;
+      const int slot = row[t & 31u], zr = (t >> 6) & 127u, r = (t >> 13) & 63u;
+      const unsigned int* blk = esdfBlockPtr(c.esdf, slot < 0 ? 0 : slot);
+      // chunks 2 j + half of the row: cells 0..7, then the two 16-byte halves of its flag words
 #pragma unroll
-      for (int j = 0; j < 5; j++) cpAsync16(dst + j * 8, src + j * 32, slot >= 0);
+      for (int j = 0; j < 4; j++) cpAsync16(esdfCell(R, zr * 8 + 2 * j + half), esdfCell(blk, r * 8 + 2 * j + half), slot >= 0);
+      cpAsync16(R + kRegionFlagWord0 + zr * 8 + 4 * half, esdfFlag(blk, r * 8 + 4 * half), slot >= 0);
     }
   }
 #pragma unroll
@@ -481,7 +474,7 @@ __device__ __forceinline__ void gesGather(const EsdfCtx& c, const GesShared<WT>&
     const unsigned int t = gs.tz[j][lane64];
     if (t >> 27) {
       const int hi = (t >> 5) & 1u, zr = (t >> 6) & 127u;
-      R[hi ? (kZHiBase + zr * kZCell + 4) : (kZLoBase + zr * kZCell + 3)] = zw[j];
+      R[kRegionFlagWord0 + (hi ? kZHiVox : kZLoVox) + zr] = zw[j];
     }
   }
   cpAsyncWaitAll();
@@ -497,12 +490,13 @@ struct PairOps {
 __device__ __forceinline__ PairOps pairLoad(unsigned int* R, unsigned int desc, bool act) {
   PairOps q;
   q.act = act;
-  q.nb = R + ((desc >> 13) & 8191u);
-  // unconditional fetch (the addresses of an inactive descriptor are valid words of the region): no branch, so the
+  const int sv = desc & 8191u, dv = (desc >> 13) & 8191u;
+  q.nb = esdfCell(R, dv);
+  // unconditional fetch (the addresses of an inactive descriptor are valid voxels of the region): no branch, so the
   // operands of the lane's four pairs are in flight together
-  const unsigned int* e = R + (desc & 8191u);
-  q.e0 = e[0], q.e1 = e[1], q.e2 = e[2], q.e3 = e[3], q.e4 = e[4];
-  q.n0 = q.nb[0], q.n4 = q.nb[4];
+  const unsigned int* e = esdfCell(R, sv);
+  q.e0 = e[0], q.e1 = e[1], q.e2 = e[2], q.e3 = e[3], q.e4 = R[kRegionFlagWord0 + sv];
+  q.n0 = q.nb[0], q.n4 = R[kRegionFlagWord0 + dv];
   return q;
 }
 __device__ __forceinline__ bool pairApply(const PairOps& q, int axis, int direction, float max_sq) {

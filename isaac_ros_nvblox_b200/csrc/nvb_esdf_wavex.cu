@@ -25,9 +25,11 @@
 //     blocks that are in no live pair are not fetched (they would miss L2: nobody wrote them lately). The halo travels by
 //     cp.async from the exchange slab straight into the region planes, so no registers are held across its round trip.
 //   * Region layout in shared memory: a plane of 16-byte cells {squared distance, parent} and a plane of flag words, voxel
-//     index rx*110 + ry*11 + rz. Every line of the three sweeps and every pair of the replay is ONE conflict-free 128-bit
-//     access per voxel (the 20-byte array-of-structures layout of the layer costs five 32-bit accesses with up to 8-way bank
-//     conflicts on z lines; with eight groups per SM the kernel is bound by shared-memory instructions, not by latency).
+//     index rx*110 + ry*11 + rz, the split the layer's blocks (nvb_esdf_block.cuh) and the exchange slab use too. Every line
+//     of the three sweeps and every pair of the replay is ONE conflict-free 128-bit access per voxel (a 20-byte array-of-
+//     structures layout costs five 32-bit accesses with up to 8-way bank conflicts on z lines; with eight groups per SM the
+//     kernel is bound by shared-memory instructions, not by latency), and the own block moves between the layer and the
+//     region in aligned 16-byte cells and flag words, with no reshuffling.
 //   * The sweep keeps, per line, the running site as (offset along the line, squared perpendicular offset, the two
 //     perpendicular components): the loop-carried chain per voxel is one subtract, one multiply-add, one compare, one select.
 //   * No hot words. Candidates of ring r+1 are registered by the owners of the blocks that changed in ring r (unique by an
@@ -99,7 +101,7 @@ constexpr int kMaxCtas = 192;     // per-CTA flags
 constexpr int kRX = 110, kRY = 11;  // region voxel index = rx * 110 + ry * 11 + rz, rx, ry, rz in 0..9 (block voxel + 1)
 constexpr int kRegionVox = 1100;
 constexpr int kFlagBase = 4 * kRegionVox;        // word offset of the flag plane
-constexpr int kXRegionWords = 5 * kRegionVox;    // 5 500 words = 22 000 bytes per group
+constexpr int kXRegionWords = (kEsdfCellWords + 1) * kRegionVox;  // the two planes: 5 500 words = 22 000 bytes per group
 constexpr size_t kXSmemBytes = (size_t)kXG * kXRegionWords * sizeof(unsigned int);
 // Exchange-slab slot: the block's six faces (+x,-x,+y,-y,+z,-z), 64 voxels each in the order of the halo batches (face f, voxel
 // (c1, c2) of the two other axes in axis order at index f * 64 + c1 * 8 + c2), as a plane of 16-byte cells {squared distance,
@@ -317,44 +319,46 @@ __device__ __forceinline__ LiveMasks liveMasks(unsigned int mask, unsigned int* 
   return L;
 }
 
-// ---- the candidate's own block: one z-row (8 voxels, 160 contiguous bytes) per lane, through registers into the two planes
+// ---- the candidate's own block: one z-row per lane (its 8 cells and its 8 flag words as two 16-byte vectors), through
+// registers into the two planes
 struct OwnRegs {
-  uint4 q[10];
+  uint4 cell[8];
+  uint4 flag[2];
 };
 __device__ __forceinline__ OwnRegs ownLoad(const unsigned char* blk, int lane64) {
   OwnRegs o;
-  const uint4* src = reinterpret_cast<const uint4*>(blk) + lane64 * 10;
+  const unsigned int* b = reinterpret_cast<const unsigned int*>(blk);
 #pragma unroll
-  for (int i = 0; i < 10; i++) o.q[i] = __ldcg(src + i);
+  for (int z = 0; z < 8; z++) o.cell[z] = __ldcg(reinterpret_cast<const uint4*>(esdfCell(b, lane64 * 8 + z)));
+#pragma unroll
+  for (int h = 0; h < 2; h++) o.flag[h] = __ldcg(reinterpret_cast<const uint4*>(esdfFlag(b, lane64 * 8 + 4 * h)));
   return o;
 }
 __device__ __forceinline__ unsigned int liveAxes(const unsigned int* live) {  // bit a: a pass along axis a is live
   return ((live[0] | live[1]) ? 1u : 0u) | ((live[2] | live[3]) ? 2u : 0u) | ((live[4] | live[5]) ? 4u : 0u);
 }
-__device__ __forceinline__ unsigned int ownWord(const OwnRegs& o, int w) {  // w is a compile-time constant after unrolling
-  const uint4& v = o.q[w >> 2];
-  return (w & 3) == 0 ? v.x : ((w & 3) == 1 ? v.y : ((w & 3) == 2 ? v.z : v.w));
-}
 __device__ __forceinline__ void ownToShared(unsigned int* R, const OwnRegs& o, int lane64) {
   uint4* A = reinterpret_cast<uint4*>(R);
   const int v0 = rvox((lane64 >> 3) + 1, (lane64 & 7) + 1, 1);
 #pragma unroll
-  for (int z = 0; z < 8; z++) {
-    A[v0 + z] = make_uint4(ownWord(o, 5 * z), ownWord(o, 5 * z + 1), ownWord(o, 5 * z + 2), ownWord(o, 5 * z + 3));
-    R[kFlagBase + v0 + z] = ownWord(o, 5 * z + 4);
+  for (int z = 0; z < 8; z++) A[v0 + z] = o.cell[z];
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    R[kFlagBase + v0 + 4 * h] = o.flag[h].x, R[kFlagBase + v0 + 4 * h + 1] = o.flag[h].y;
+    R[kFlagBase + v0 + 4 * h + 2] = o.flag[h].z, R[kFlagBase + v0 + 4 * h + 3] = o.flag[h].w;
   }
 }
-// inner 8x8x8 of the region -> the block in the layer (if `to_layer`), half a z-row (four voxels = 80 bytes = five 16-byte words)
-// at a time, and its six faces -> its slot in an exchange slab, one cell and one flag word per lane and face. On the way the box
-// of the BLOCK OFFSETS the voxels' parents point into is collected and published in c.psum (EsdfCtx::psum; one word per warp of
-// the group, so no barrier is needed): the clear pass of later updates reads a candidate block only if that box contains a
-// to-clear block.
+// inner 8x8x8 of the region -> the block in the layer (if `to_layer`), and its six faces -> its slot in an exchange slab, one
+// cell and one flag word per lane and face. The block goes in eight steps of one cell and one flag word per lane, warp w of
+// the group taking voxels 256 w + 32 k + lane (x = 4 w + k / 2): each warp store is 512 contiguous bytes of cells and 128 of
+// flags. On the way the box of the BLOCK OFFSETS the voxels' parents point into is collected and published in c.psum
+// (EsdfCtx::psum; one word per warp of the group, so no barrier is needed): the clear pass of later updates reads a
+// candidate block only if that box contains a to-clear block.
 __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer, unsigned char* x_slot, const unsigned int* R,
                                          unsigned int* psum_slot, int lane64) {
   const uint4* A = reinterpret_cast<const uint4*>(R);
   const int x = lane64 >> 3, y = lane64 & 7;
-  const int v0 = rvox(x + 1, y + 1, 1);
-  uint4* dl = reinterpret_cast<uint4*>(layer_blk) + lane64 * 10;
+  unsigned int* dl = reinterpret_cast<unsigned int*>(layer_blk);
   uint4* xc = reinterpret_cast<uint4*>(x_slot) + lane64;
   unsigned int* xf = reinterpret_cast<unsigned int*>(x_slot + kXFlagOff) + lane64;
 #pragma unroll
@@ -365,22 +369,20 @@ __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer
     __stcg(xf + f * 64, R[kFlagBase + v]);
   }
   int lo0 = 99, lo1 = 99, lo2 = 99, hi0 = -99, hi1 = -99, hi2 = -99;
+  const int w = lane64 >> 5, l = lane64 & 31;
 #pragma unroll
-  for (int h = 0; h < 2; h++) {
-    unsigned int w[20];
-#pragma unroll
-    for (int z = 0; z < 4; z++) {
-      const uint4 a = A[v0 + 4 * h + z];
-      w[5 * z] = a.x, w[5 * z + 1] = a.y, w[5 * z + 2] = a.z, w[5 * z + 3] = a.w;
-      w[5 * z + 4] = R[kFlagBase + v0 + 4 * h + z];
-      if ((a.y | a.z | a.w) != 0u) {
-        const int b0 = (x + (int)a.y) >> 3, b1 = (y + (int)a.z) >> 3, b2 = (4 * h + z + (int)a.w) >> 3;  // floor: arithmetic shift
-        lo0 = min(lo0, b0), hi0 = max(hi0, b0), lo1 = min(lo1, b1), hi1 = max(hi1, b1), lo2 = min(lo2, b2), hi2 = max(hi2, b2);
-      }
+  for (int k = 0; k < 8; k++) {
+    const int vx = 4 * w + (k >> 1), vy = ((k & 1) << 2) + (l >> 3), vz = l & 7;
+    const int v = (vx * kVps + vy) * kVps + vz, rv = rvox(vx + 1, vy + 1, vz + 1);
+    const uint4 a = A[rv];
+    if (to_layer) {
+      __stcg(reinterpret_cast<uint4*>(esdfCell(dl, v)), a);
+      __stcg(esdfFlag(dl, v), R[kFlagBase + rv]);
     }
-#pragma unroll
-    for (int i = 0; i < 5; i++)
-      if (to_layer) __stcg(dl + 5 * h + i, make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]));
+    if ((a.y | a.z | a.w) != 0u) {
+      const int b0 = (vx + (int)a.y) >> 3, b1 = (vy + (int)a.z) >> 3, b2 = (vz + (int)a.w) >> 3;  // floor: arithmetic shift
+      lo0 = min(lo0, b0), hi0 = max(hi0, b0), lo1 = min(lo1, b1), hi1 = max(hi1, b1), lo2 = min(lo2, b2), hi2 = max(hi2, b2);
+    }
   }
   if (psum_slot) {
     lo0 = __reduce_min_sync(0xffffffffu, lo0), lo1 = __reduce_min_sync(0xffffffffu, lo1), lo2 = __reduce_min_sync(0xffffffffu, lo2);
@@ -392,7 +394,7 @@ __device__ __forceinline__ void ownStore(unsigned char* layer_blk, bool to_layer
 // ---- halo voxels, as cp.async copies straight into the two region planes -- the 16-byte cell and the flag word of a voxel
 // from its block's exchange-slab slot: no registers are held across the wait (the register version held up to 20 words per
 // lane and spilled at 96 registers). Only the batches of the members in a live pair are fetched, after the stamps. The cells
-// travel .cg, through L2 only. The flag words and the own block's words (ownAsync) are 4-byte copies, which have no .cg form,
+// travel .cg, through L2 only. The flag words (here and in ownAsync) are 4-byte copies, which have no .cg form,
 // so they go .ca. The L1 lines those leave behind cannot go stale unnoticed: every grid barrier ends with an acquire
 // (gridBarrierRA), which invalidates the SM's L1, and within the single-CTA tail the writer is this SM.
 __device__ __forceinline__ void cpAsync4(unsigned int* smem_dst, const unsigned int* gsrc) {
@@ -405,24 +407,22 @@ __device__ __forceinline__ void cpAsyncCell(unsigned int* smem_dst, const void* 
 }
 // ---- the own block split in two (grid rings, processCandidate): first the voxels on the boundary planes of
 // the axes `axes` (bit a: the planes 0 and 7 along axis a), which hold every voxel of B the replay reads or writes, then -- only
-// if B changed -- the rest. 4-byte copies (the layer's 20-byte voxels are not 16-byte aligned), one voxel per
-// lane and x plane (lane = y * 8 + z: a warp's copies of one word cover 640 contiguous bytes). `planes`: copy the voxels on
-// those planes, else every other voxel. (.ca: the layer's blocks are written with .cg stores by the owners of earlier rings,
-// and the grid barrier between them and this read invalidates the SM's L1; the single-CTA tail does not fetch split.)
+// if B changed -- the rest. One voxel per lane and x plane (lane = y * 8 + z), as its 16-byte cell (.cg) and its flag word
+// (.ca): a warp's copies cover 512 contiguous bytes of cells and 128 of flags. `planes`: copy the voxels on those planes,
+// else every other voxel. (.ca: the layer's blocks are written with .cg stores by the owners of earlier rings, and the grid
+// barrier between them and this read invalidates the SM's L1; the single-CTA tail does not fetch split.)
 __device__ __forceinline__ void ownAsync(unsigned int* R, const unsigned char* blk, int lane64, unsigned int axes, bool planes) {
   const int y = lane64 >> 3, z = lane64 & 7;
   const bool lane_on = ((axes & 2u) && (y == 0 || y == 7)) || ((axes & 4u) && (z == 0 || z == 7));
-  const unsigned int* src = reinterpret_cast<const unsigned int*>(blk) + lane64 * kEsdfVoxelWords;
+  const unsigned int* b = reinterpret_cast<const unsigned int*>(blk);
   const int v0 = rvox(1, y + 1, z + 1);
 #pragma unroll
   for (int x = 0; x < 8; x++) {
     const bool on = lane_on || ((axes & 1u) && (x == 0 || x == 7));
     if (on == planes) {
-      const unsigned int* s = src + x * 64 * kEsdfVoxelWords;
-      const int v = v0 + x * kRX;
-#pragma unroll
-      for (int w = 0; w < 4; w++) cpAsync4(R + 4 * v + w, s + w);
-      cpAsync4(R + kFlagBase + v, s + 4);
+      const int v = x * 64 + lane64, rv = v0 + x * kRX;
+      cpAsyncCell(R + 4 * rv, esdfCell(b, v));
+      cpAsync4(R + kFlagBase + rv, esdfFlag(b, v));
     }
   }
 }

@@ -21,8 +21,7 @@ namespace nvb {
 constexpr int kVps = 8;                 // VoxelBlock::kVoxelsPerSide (map/blox.h:36)
 constexpr int kVpb = kVps * kVps * kVps;
 constexpr int kTsdfBlockBytes = kVpb * 8;   // 4096
-constexpr int kEsdfBlockBytes = kVpb * 20;  // 10240
-constexpr int kEsdfVoxelWords = 5;
+constexpr int kEsdfBlockBytes = kVpb * (16 + 4);  // 10240: a plane of 16-byte cells and a plane of flag words (nvb_esdf_block.cuh)
 constexpr int kColorBlockBytes = kVpb * 8;  // ColorVoxel{Color (3 bytes) + 1 pad, float weight} (map/voxels.h:77-83)
 constexpr int kOccBlockBytes = kVpb * 4;    // OccupancyVoxel{float log_odds} (map/voxels.h:92-97)
 constexpr int kHelperCtas = 132;            // grid of the small grid-stride helper kernels: one CTA per H100 SM
@@ -679,9 +678,10 @@ void launchMeshCompactMove(const MeshCtx& c, int nslots, const int* new_offsets,
                            unsigned char* c2, int num_sms, cudaStream_t stream);
 
 // nvb_util.cu
-void launchGatherBlocks(const DevLayer& layer, const int* xyz_dev, int n, unsigned char* out, unsigned char* found,
+// `esdf`: the ESDF layer, whose blocks are copied out as / in from the reference's EsdfVoxel records (nvb_esdf_block.cuh)
+void launchGatherBlocks(const DevLayer& layer, bool esdf, const int* xyz_dev, int n, unsigned char* out, unsigned char* found,
                         cudaStream_t stream);
-void launchScatterBlocks(const DevLayer& layer, const int* xyz_dev, int n, const unsigned char* in, int* error,
+void launchScatterBlocks(const DevLayer& layer, bool esdf, const int* xyz_dev, int n, const unsigned char* in, int* error,
                          cudaStream_t stream);
 void launchFillU64(unsigned long long* p, unsigned long long v, size_t n, cudaStream_t stream);
 // DepthPreprocessor::dilateInvalidRegionsAsync (src/sensors/depth_preprocessing.cpp); out must not alias in
@@ -693,6 +693,9 @@ void launchRehash(const DevLayer& layer, int count, cudaStream_t stream);
 void launchSliceAabb(const DevLayer& esdf, int zb, int* out4, cudaStream_t stream);
 void launchSliceImage(const DevLayer& esdf, float block_size, float min_x, float min_y, float slice_height, float unobserved_value,
                       int rows, int cols, float* image, signed char* grid, cudaStream_t stream);
+// the ESDF's signed distances (metres) on the voxel grid (min_vox, dims), z fastest; default_value where unknown
+void launchEsdfDenseGrid(const DevLayer& esdf, int3 min_vox, int3 dims, float voxel_size, float default_value, float* out,
+                         cudaStream_t stream);
 void launchRemoveBlocks(const DevLayer& layer, const int4* dead, const int* dead_count, int upper, cudaStream_t stream);
 void launchTodoAll(const DevLayer& tsdf, const TrackerList& t, cudaStream_t stream);
 // Drops the slots that are dead in `layer` from a list of its slots (*count entries), keeping the order of the others.
@@ -812,8 +815,8 @@ struct QueryLayers {
   int n;
 };
 enum QueryInterpKind { kInterpTsdf = 0, kInterpEsdf = 1, kInterpOccupancy = 2 };
-// out: n voxels of voxel_bytes (a multiple of 4) each, written only where found[i] = 1
-void launchQueryVoxels(const QueryLayer& q, int voxel_bytes, const float* xyz, long long n, void* out, unsigned char* found,
+// out: n voxels of voxel_bytes (a multiple of 4) each, written only where found[i] = 1 (ESDF voxels as EsdfVoxel records)
+void launchQueryVoxels(const QueryLayer& q, int voxel_bytes, bool esdf, const float* xyz, long long n, void* out, unsigned char* found,
                        int num_sms, cudaStream_t stream);
 void launchInterpolate(const QueryLayer& q, int kind, const float* xyz, long long n, float* out, unsigned char* success,
                        int num_sms, cudaStream_t stream);

@@ -14,7 +14,7 @@
 #include <cstdio>
 #include <string>
 
-#include "nvb_internal.cuh"
+#include "nvb_esdf_block.cuh"
 
 namespace nvb {
 
@@ -236,11 +236,12 @@ int readMapFile(const char* path, const bool want[kMapFileLayers], MapFileLayerI
 __global__ void esdfParentBoxesKernel(DevLayer esdf, unsigned int* psum) {
   const int slot = blockIdx.x, lane64 = threadIdx.x;
   const int x = lane64 >> 3, y = lane64 & 7;
-  const int* row = reinterpret_cast<const int*>(esdf.blocks + (size_t)slot * kEsdfBlockBytes) + lane64 * kVps * kEsdfVoxelWords;
+  const unsigned int* blk = reinterpret_cast<const unsigned int*>(esdf.blocks + (size_t)slot * kEsdfBlockBytes);
   int lo0 = 99, lo1 = 99, lo2 = 99, hi0 = -99, hi1 = -99, hi2 = -99;
 #pragma unroll
   for (int z = 0; z < kVps; z++) {
-    const int px = row[kEsdfVoxelWords * z + 1], py = row[kEsdfVoxelWords * z + 2], pz = row[kEsdfVoxelWords * z + 3];
+    const unsigned int* c = esdfCell(blk, lane64 * kVps + z);
+    const int px = (int)c[1], py = (int)c[2], pz = (int)c[3];
     if ((px | py | pz) != 0) {
       const int b0 = (x + px) >> 3, b1 = (y + py) >> 3, b2 = (z + pz) >> 3;  // floor: arithmetic shift
       lo0 = min(lo0, b0), hi0 = max(hi0, b0), lo1 = min(lo1, b1), hi1 = max(hi1, b1), lo2 = min(lo2, b2), hi2 = max(hi2, b2);
@@ -272,11 +273,12 @@ __device__ __forceinline__ bool exportVoxel(const ExportPointsArgs& a, const uns
     *intensity = blk[(size_t)v * kFreespaceVoxelBytes + 16] ? 1.0f : 0.0f;  // is_high_confidence_freespace
     return true;
   }
-  const unsigned char* e = blk + (size_t)v * kEsdfVoxelWords * 4;
-  float d = a.voxel_size * sqrtf(*reinterpret_cast<const float*>(e));
-  if (e[16]) d = -d;  // is_inside
+  const unsigned int* b = reinterpret_cast<const unsigned int*>(blk);
+  const unsigned int fl = *esdfFlag(b, v);
+  float d = a.voxel_size * sqrtf(__uint_as_float(*esdfCell(b, v)));
+  if (fl & 0xffu) d = -d;  // is_inside
   *intensity = d;
-  return e[17] != 0;  // observed
+  return (fl & 0xff00u) != 0;  // observed
 }
 
 // One CTA per listed block, one thread per voxel (v = (x * 8 + y) * 8 + z, the order of voxels[x][y][z]).

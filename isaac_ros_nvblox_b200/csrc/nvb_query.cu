@@ -12,7 +12,7 @@
 //    reference's float -> int conversion would alias it to some other block);
 //  - interpolation does not abort when the corner offsets leave [0, 1] by rounding (getQVector3D's CHECKs); it evaluates the
 //    same polynomial.
-#include "nvb_internal.cuh"
+#include "nvb_esdf_block.cuh"
 
 namespace nvb {
 
@@ -25,14 +25,16 @@ constexpr float kGradientEpsilon = 1e-6f;    // sdf_query.cu:106
 
 __device__ __forceinline__ bool finite3(const Vec3& p) { return isfinite(p.x) && isfinite(p.y) && isfinite(p.z); }
 
-// getVoxelAtPosition (gpu_hash/internal/cuda/gpu_indexing.cuh:56-64): the voxel's byte offset in the slab, or -1.
-__device__ __forceinline__ long long voxelOffsetAt(const QueryLayer& q, const Vec3& p, int voxel_bytes) {
-  if (!finite3(p)) return -1;
-  int3 b, v;
-  blockAndVoxelIndexFromPosition(q.block_size, q.voxel_size_inv, p, b, v);
+// getVoxelAtPosition (gpu_hash/internal/cuda/gpu_indexing.cuh:56-64): the block holding p (null if it is not allocated)
+// and the voxel's index v in it.
+__device__ __forceinline__ const unsigned char* voxelAt(const QueryLayer& q, const Vec3& p, int* v) {
+  if (!finite3(p)) return nullptr;
+  int3 b, vi;
+  blockAndVoxelIndexFromPosition(q.block_size, q.voxel_size_inv, p, b, vi);
   const int slot = hashFind(q.layer.hash, b.x, b.y, b.z);
-  if (slot < 0) return -1;
-  return (long long)slot * q.layer.block_bytes + (long long)((v.x * kVps + v.y) * kVps + v.z) * voxel_bytes;
+  if (slot < 0) return nullptr;
+  *v = (vi.x * kVps + vi.y) * kVps + vi.z;
+  return q.layer.blocks + (size_t)slot * q.layer.block_bytes;
 }
 
 __device__ __forceinline__ Vec3 loadPoint(const float* xyz, long long i, int stride) {
@@ -40,16 +42,22 @@ __device__ __forceinline__ Vec3 loadPoint(const float* xyz, long long i, int str
   return Vec3{p[0], p[1], p[2]};
 }
 
-__global__ void __launch_bounds__(kQueryThreads) queryVoxelsKernel(const __grid_constant__ QueryLayer q, int voxel_words,
+// ESDF voxels are returned as the reference's 20-byte records (nvb_esdf_block.cuh).
+__global__ void __launch_bounds__(kQueryThreads) queryVoxelsKernel(const __grid_constant__ QueryLayer q, int voxel_words, bool esdf,
                                                                   const float* __restrict__ xyz, long long n,
                                                                   unsigned int* __restrict__ out,
                                                                   unsigned char* __restrict__ found) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const long long off = voxelOffsetAt(q, loadPoint(xyz, i, 3), voxel_words * 4);
-    found[i] = off >= 0;
-    if (off < 0) continue;
-    const unsigned int* src = reinterpret_cast<const unsigned int*>(q.layer.blocks + off);
-    for (int w = 0; w < voxel_words; w++) out[i * voxel_words + w] = src[w];
+    int v = 0;
+    const unsigned char* blk = voxelAt(q, loadPoint(xyz, i, 3), &v);
+    found[i] = blk != nullptr;
+    if (!blk) continue;
+    const unsigned int* words = reinterpret_cast<const unsigned int*>(blk);
+    if (esdf) {
+      esdfVoxelToRecord(words, v, out + i * voxel_words);
+    } else {
+      for (int w = 0; w < voxel_words; w++) out[i * voxel_words + w] = words[(size_t)v * voxel_words + w];
+    }
   }
 }
 
@@ -61,9 +69,9 @@ __device__ __forceinline__ bool interpMember(const unsigned char* blk, int v, fl
     *value = t.x;
     return t.y > kTsdfMinWeight;
   } else if (kKind == kInterpEsdf) {
-    const unsigned int* e = reinterpret_cast<const unsigned int*>(blk) + v * kEsdfVoxelWords;
-    if ((e[4] & 0xff00u) == 0) return false;  // observed
-    *value = sqrtf(__uint_as_float(e[0]));
+    const unsigned int* b = reinterpret_cast<const unsigned int*>(blk);
+    if ((*esdfFlag(b, v) & 0xff00u) == 0) return false;  // observed
+    *value = sqrtf(__uint_as_float(*esdfCell(b, v)));
     return true;
   } else {
     const float lo = reinterpret_cast<const float*>(blk)[v];
@@ -155,10 +163,11 @@ __global__ void __launch_bounds__(kQueryThreads, 4) queryEsdfKernel(const __grid
     const int nm = kMulti ? q.n : 1;
     for (int k = 0; k < nm; k++) {
       const QueryLayer& L = q.l[k];
-      const long long off = voxelOffsetAt(L, p, kEsdfVoxelWords * 4);
-      if (off < 0) continue;
-      const unsigned int* e = reinterpret_cast<const unsigned int*>(L.layer.blocks + off);
-      const unsigned int flags = e[4];
+      int v = 0;
+      const unsigned char* blk = voxelAt(L, p, &v);
+      if (!blk) continue;
+      const unsigned int* e = esdfCell(reinterpret_cast<const unsigned int*>(blk), v);
+      const unsigned int flags = *esdfFlag(reinterpret_cast<const unsigned int*>(blk), v);
       write_d = true;
       if ((flags & 0xff00u) == 0) {  // not observed
         d = kMaxDistance;
@@ -202,18 +211,20 @@ __global__ void __launch_bounds__(kQueryThreads) queryTsdfKernel(const __grid_co
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const Vec3 p = loadPoint(xyz, i, 3);
     if (!kMulti) {
-      const long long off = voxelOffsetAt(q.l[0], p, 8);
-      if (off >= 0) {
-        const float2 t = *reinterpret_cast<const float2*>(q.l[0].layer.blocks + off);
+      int v = 0;
+      const unsigned char* blk = voxelAt(q.l[0], p, &v);
+      if (blk) {
+        const float2 t = reinterpret_cast<const float2*>(blk)[v];
         out[2 * i] = t.x, out[2 * i + 1] = t.y;
       }
       continue;
     }
     float min_distance = kMaxDistance, weight_at_min = 0.0f;
     for (int k = 0; k < q.n; k++) {
-      const long long off = voxelOffsetAt(q.l[k], p, 8);
-      if (off < 0) continue;
-      const float2 t = *reinterpret_cast<const float2*>(q.l[k].layer.blocks + off);
+      int v = 0;
+      const unsigned char* blk = voxelAt(q.l[k], p, &v);
+      if (!blk) continue;
+      const float2 t = reinterpret_cast<const float2*>(blk)[v];
       if (t.x < min_distance) min_distance = t.x, weight_at_min = t.y;
     }
     out[2 * i] = min_distance, out[2 * i + 1] = weight_at_min;
@@ -231,9 +242,10 @@ __global__ void __launch_bounds__(kQueryThreads) queryOccupancyKernel(const __gr
     float max_log_odds = initial;
     const int nm = kMulti ? q.n : 1;
     for (int k = 0; k < nm; k++) {
-      const long long off = voxelOffsetAt(q.l[k], p, 4);
-      if (off < 0) continue;
-      const float lo = *reinterpret_cast<const float*>(q.l[k].layer.blocks + off);
+      int v = 0;
+      const unsigned char* blk = voxelAt(q.l[k], p, &v);
+      if (!blk) continue;
+      const float lo = reinterpret_cast<const float*>(blk)[v];
       if (lo > max_log_odds) max_log_odds = lo;
     }
     out[i] = max_log_odds;
@@ -248,10 +260,10 @@ int queryGrid(long long n, int num_sms) {
 
 }  // namespace
 
-void launchQueryVoxels(const QueryLayer& q, int voxel_bytes, const float* xyz, long long n, void* out, unsigned char* found,
+void launchQueryVoxels(const QueryLayer& q, int voxel_bytes, bool esdf, const float* xyz, long long n, void* out, unsigned char* found,
                        int num_sms, cudaStream_t stream) {
   if (n <= 0) return;
-  queryVoxelsKernel<<<queryGrid(n, num_sms), kQueryThreads, 0, stream>>>(q, voxel_bytes / 4, xyz, n,
+  queryVoxelsKernel<<<queryGrid(n, num_sms), kQueryThreads, 0, stream>>>(q, voxel_bytes / 4, esdf, xyz, n,
                                                                          static_cast<unsigned int*>(out), found);
 }
 

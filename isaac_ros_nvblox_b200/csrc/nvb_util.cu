@@ -4,13 +4,14 @@
 // These back the BlockLayer queries the reference answers from its host-side
 // unordered_map (nvblox/include/nvblox/map/layer.h:76-217): here the map lives in
 // HBM, so host access is an explicit gather.
-#include "nvb_internal.cuh"
+#include "nvb_esdf_block.cuh"
 
 namespace nvb {
 
 namespace {
 
-__global__ void gatherBlocksKernel(DevLayer L, const int* xyz, int n, unsigned char* out, unsigned char* found) {
+// ESDF blocks (`esdf`) leave in the reference's 20-byte voxel records and come back from them (nvb_esdf_block.cuh).
+__global__ void gatherBlocksKernel(DevLayer L, bool esdf, const int* xyz, int n, unsigned char* out, unsigned char* found) {
   const int i = blockIdx.x;
   if (i >= n) return;
   __shared__ int s_slot;
@@ -22,7 +23,11 @@ __global__ void gatherBlocksKernel(DevLayer L, const int* xyz, int n, unsigned c
   const int slot = s_slot;
   uint4* dst = reinterpret_cast<uint4*>(out + (size_t)i * L.block_bytes);
   const int nvec = L.block_bytes / 16;
-  if (slot >= 0) {
+  if (slot >= 0 && esdf) {
+    const unsigned int* src = reinterpret_cast<const unsigned int*>(L.blocks + (size_t)slot * L.block_bytes);
+    unsigned int* rec = reinterpret_cast<unsigned int*>(dst);
+    for (int v = threadIdx.x; v < kVpb; v += blockDim.x) esdfVoxelToRecord(src, v, rec + kEsdfRecordWords * v);
+  } else if (slot >= 0) {
     const uint4* src = reinterpret_cast<const uint4*>(L.blocks + (size_t)slot * L.block_bytes);
     for (int k = threadIdx.x; k < nvec; k += blockDim.x) dst[k] = src[k];
   } else {
@@ -30,7 +35,7 @@ __global__ void gatherBlocksKernel(DevLayer L, const int* xyz, int n, unsigned c
   }
 }
 
-__global__ void scatterBlocksKernel(DevLayer L, const int* xyz, int n, const unsigned char* in, int* error) {
+__global__ void scatterBlocksKernel(DevLayer L, bool esdf, const int* xyz, int n, const unsigned char* in, int* error) {
   const int i = blockIdx.x;
   if (i >= n) return;
   __shared__ int s_slot;
@@ -41,6 +46,12 @@ __global__ void scatterBlocksKernel(DevLayer L, const int* xyz, int n, const uns
   __syncthreads();
   const int slot = s_slot;
   if (slot < 0) return;
+  if (esdf) {
+    const unsigned int* rec = reinterpret_cast<const unsigned int*>(in + (size_t)i * L.block_bytes);
+    unsigned int* dst = reinterpret_cast<unsigned int*>(L.blocks + (size_t)slot * L.block_bytes);
+    for (int v = threadIdx.x; v < kVpb; v += blockDim.x) esdfVoxelFromRecord(rec + kEsdfRecordWords * v, dst, v);
+    return;
+  }
   const uint4* src = reinterpret_cast<const uint4*>(in + (size_t)i * L.block_bytes);
   uint4* dst = reinterpret_cast<uint4*>(L.blocks + (size_t)slot * L.block_bytes);
   const int nvec = L.block_bytes / 16;
@@ -201,11 +212,12 @@ __global__ void sliceImageKernel(DevLayer L, float block_size, float min_x, floa
   float d = unobserved_value;
   const int slot = hashFind(L.hash, b.x, b.y, b.z);
   if (slot >= 0) {
-    const unsigned int* e = reinterpret_cast<const unsigned int*>(L.blocks + (size_t)slot * kEsdfBlockBytes) +
-                            ((v.x * kVps + v.y) * kVps + v.z) * kEsdfVoxelWords;
-    if ((e[4] & 0xff00u) != 0) {  // observed
-      d = voxel_size * sqrtf(__uint_as_float(e[0]));
-      if ((e[4] & 0xffu) != 0) d = -d;  // is_inside
+    const unsigned int* blk = reinterpret_cast<const unsigned int*>(L.blocks + (size_t)slot * kEsdfBlockBytes);
+    const int vi = (v.x * kVps + v.y) * kVps + v.z;
+    const unsigned int fl = *esdfFlag(blk, vi);
+    if ((fl & 0xff00u) != 0) {  // observed
+      d = voxel_size * sqrtf(__uint_as_float(*esdfCell(blk, vi)));
+      if ((fl & 0xffu) != 0) d = -d;  // is_inside
     }
   }
   const size_t pix = (size_t)row * cols + col;
@@ -217,7 +229,41 @@ __global__ void sliceImageKernel(DevLayer L, float block_size, float min_x, floa
   }
 }
 
+// voxelLayerToDenseVoxelGridInAABBAsync (nvblox map/internal/cuda/impl/layer_to_3d_grid_impl.cuh) with nvblox_ros's
+// SignedDistanceFunctor (conversions/esdf_and_gradients_conversions.cu): one CTA per block overlapping the grid, one thread per
+// voxel; a cell is the voxel's distance in metres (negative inside), `default_value` where the voxel is unobserved or its block
+// is not allocated. Cells in z-fastest order over the grid (min_vox, dims), as Unified3DGrid stores them.
+__global__ void __launch_bounds__(kVpb) esdfDenseGridKernel(DevLayer L, int3 min_block, int3 min_vox, int3 dims, float voxel_size,
+                                                           float default_value, float* out) {
+  __shared__ int s_slot;
+  const int bx = min_block.x + (int)blockIdx.x, by = min_block.y + (int)blockIdx.y, bz = min_block.z + (int)blockIdx.z;
+  if (threadIdx.x == 0) s_slot = hashFind(L.hash, bx, by, bz);
+  __syncthreads();
+  const int v = threadIdx.x;
+  const int gx = bx * kVps + (v >> 6) - min_vox.x, gy = by * kVps + ((v >> 3) & 7) - min_vox.y, gz = bz * kVps + (v & 7) - min_vox.z;
+  if (gx < 0 || gy < 0 || gz < 0 || gx >= dims.x || gy >= dims.y || gz >= dims.z) return;
+  float d = default_value;
+  if (s_slot >= 0) {
+    const unsigned int* blk = reinterpret_cast<const unsigned int*>(L.blocks + (size_t)s_slot * kEsdfBlockBytes);
+    const unsigned int fl = *esdfFlag(blk, v);
+    if ((fl & 0xff00u) != 0) {  // observed
+      d = sqrtf(__uint_as_float(*esdfCell(blk, v))) * voxel_size;
+      if ((fl & 0xffu) != 0) d = -d;  // is_inside
+    }
+  }
+  out[((size_t)gx * dims.y + gy) * dims.z + gz] = d;
+}
+
 }  // namespace
+
+void launchEsdfDenseGrid(const DevLayer& esdf, int3 min_vox, int3 dims, float voxel_size, float default_value, float* out,
+                         cudaStream_t stream) {
+  // the blocks holding the grid's first and last voxel (floor division)
+  const int3 lo = make_int3(min_vox.x >> 3, min_vox.y >> 3, min_vox.z >> 3);
+  const int3 hi = make_int3((min_vox.x + dims.x - 1) >> 3, (min_vox.y + dims.y - 1) >> 3, (min_vox.z + dims.z - 1) >> 3);
+  const dim3 grid(hi.x - lo.x + 1, hi.y - lo.y + 1, hi.z - lo.z + 1);
+  esdfDenseGridKernel<<<grid, kVpb, 0, stream>>>(esdf, lo, min_vox, dims, voxel_size, default_value, out);
+}
 
 void launchSliceAabb(const DevLayer& esdf, int zb, int* out4, cudaStream_t stream) {
   sliceAabbKernel<<<296, 256, 0, stream>>>(esdf, zb, out4);
@@ -239,13 +285,13 @@ void launchDropDeadSlots(const DevLayer& layer, int* list, int* count, cudaStrea
   dropDeadSlotsKernel<<<1, 1024, 0, stream>>>(layer, list, count);
 }
 
-void launchGatherBlocks(const DevLayer& layer, const int* xyz_dev, int n, unsigned char* out, unsigned char* found,
+void launchGatherBlocks(const DevLayer& layer, bool esdf, const int* xyz_dev, int n, unsigned char* out, unsigned char* found,
                         cudaStream_t stream) {
-  if (n > 0) gatherBlocksKernel<<<n, 128, 0, stream>>>(layer, xyz_dev, n, out, found);
+  if (n > 0) gatherBlocksKernel<<<n, 128, 0, stream>>>(layer, esdf, xyz_dev, n, out, found);
 }
-void launchScatterBlocks(const DevLayer& layer, const int* xyz_dev, int n, const unsigned char* in, int* error,
+void launchScatterBlocks(const DevLayer& layer, bool esdf, const int* xyz_dev, int n, const unsigned char* in, int* error,
                          cudaStream_t stream) {
-  if (n > 0) scatterBlocksKernel<<<n, 128, 0, stream>>>(layer, xyz_dev, n, in, error);
+  if (n > 0) scatterBlocksKernel<<<n, 128, 0, stream>>>(layer, esdf, xyz_dev, n, in, error);
 }
 void launchDilateInvalid(const float* in, float* out, int rows, int cols, int num_dilations, float threshold,
                          float invalid_value, cudaStream_t stream) {

@@ -1124,6 +1124,20 @@ class Mapper:
     def esdf_layer(self):
         return self._esdf
 
+    def esdf_dense_grid_in_aabb(self, aabb, default_value):
+        """voxelLayerToDenseVoxelGridInAABBAsync on the ESDF layer with the EsdfAndGradients service's conversion: aabb =
+        (6,) {min xyz, max xyz} in metres -> (min_index (3,) int32, (X, Y, Z) float32 grid of distances in metres, negative
+        inside, `default_value` where unknown). An empty box gives an empty grid."""
+        box = np.ascontiguousarray(aabb, dtype=np.float32).reshape(6)
+        mn, dims = np.zeros(3, np.int32), np.zeros(3, np.int32)
+        check(self._L.nvb_esdf_dense_grid_in_aabb(self._h, _fp(box), float(default_value), _lib.NVB_MEM_HOST, None, 0, _ip(mn),
+                                                  _ip(dims)))
+        out = np.zeros(max(int(np.prod(dims.astype(np.int64))), 1), np.float32)
+        if dims.all():
+            check(self._L.nvb_esdf_dense_grid_in_aabb(self._h, _fp(box), float(default_value), _lib.NVB_MEM_HOST,
+                                                      out.ctypes.data, out.size, _ip(mn), _ip(dims)))
+        return mn, out[:int(np.prod(dims.astype(np.int64)))].reshape(tuple(int(d) for d in dims))
+
     def projective_layer_type(self):
         return self._projective_layer_type
 
