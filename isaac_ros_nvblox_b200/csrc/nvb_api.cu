@@ -343,7 +343,7 @@ class CallerBuffers {
 };
 
 // One consumer of the block-update tracker: its dirty words and list, as large as the projective slab, and the list's
-// count in esdf_ints. Producers tell a consumer only once it is initialized, which its first all-blocks update does (the
+// count in DeviceCounters. Producers tell a consumer only once it is initialized, which its first all-blocks update does (the
 // lazy initialisation of BlocksToUpdateTracker, map/blocks_to_update_tracker.h).
 struct TrackedBlocks {
   DeviceArray<int> dirty;
@@ -352,6 +352,112 @@ struct TrackedBlocks {
   bool initialized = false;
 
   TrackerList list() const { return {dirty.get(), slots.get(), count}; }
+};
+
+// The mapper's device counter words, one zeroed allocation. Most belong to the ESDF update; the frame count, the error
+// word, the tracker consumers' list counts and the dead, colour and freespace work counts share the block.
+struct DeviceCounters {
+  int work_count;
+  int upd_count;
+  int clr_count;
+  int clr_aabb[6];
+  int cleared_count;
+  int ring_count[3];  // [2]: the mark kernel's count of finished CTAs
+  int unused_13;
+  int ring_id;
+  int todo_count;
+  int frame_count;
+  int error;
+  int cleared_seq;
+  int unused_19;
+  int tail_state[2];
+  int dead_count;
+  int dead_cleared_count;
+  int ges_counts[4];
+  int todo_fs_count;
+  int fs_work_count;
+  int cols_count;
+  int color_work_count;
+  int xtail[4];
+  int todo_mesh_count;
+  int slice_box[4];  // nvb_esdf_slice_aabb's block-column box
+};
+
+// The ESDF integrator's device state beside its layer slab (EsdfIntegrator's members, esdf_integrator.h): the per-slot
+// arrays of an update, those that carry state from one update to the next, the wavefront driver's own arrays, the
+// statistics and the switch of the clear pass's parent-box pruning. The per-slot arrays follow the ESDF slab's capacity.
+// The driver (esdf_persistent) is 0 for the host loop, 1 for the persistent wavefront, 2 for the gather-replay wavefront
+// and 3 for the exchange-slab wavefront; the shadow slab is driver 2's, the exchange slabs and records driver 3's.
+class EsdfState {
+ public:
+  // Reads the driver's switches, allocates every array for `capacity` ESDF slots and sets the first ring id.
+  int create(NvbMapper* m, int capacity, int driver);
+  // The per-slot arrays at `capacity` slots; those that carry state from one update to the next keep their contents.
+  int grow(NvbMapper* m, int capacity);
+  // SMs the exchange-slab wavefront leaves to concurrently running kernels; its records follow the launch's grid.
+  int setReservedSms(NvbMapper* m, int n);
+  // An empty ESDF layer: no cleared list, no seeds, unlinked neighbour tables and exact parent boxes, so pruning is back.
+  int reset(NvbMapper* m);
+  // Voxels written from outside the update: the parent boxes are no longer bounds, and the new blocks are not linked, so
+  // the face-neighbour table is forgotten (it is re-resolved lazily through the hash).
+  int blocksWritten(NvbMapper* m);
+  // Voxels of other blocks may keep parents inside deallocated blocks: the reference clears them when they happen to be
+  // candidates of a later clear pass, which the per-block parent boxes cannot tell. No pruning from here on.
+  void forgetParentBoxes() { prune_ok_ = false; }
+  // The parent boxes of the ESDF slots [0, n), after blocks were loaded: pruning stays exact.
+  void buildParentBoxes(const DevLayer& esdf, int n, cudaStream_t st) { launchEsdfParentBoxes(esdf, n, psum_.get(), st); }
+  // The slice update's column set and column list for `columns` columns.
+  int reserveSliceColumns(NvbMapper* m, size_t columns);
+  // The list of deallocated blocks that were on the cleared list, 3 ints per ESDF slot.
+  int reserveDeadCleared(NvbMapper* m);
+  void beginUpdate() { update_seq_++; }
+  // An EsdfCtx with the state pointers set, the counter words in `ctr`.
+  EsdfCtx ctx(DeviceCounters* ctr) const;
+  cudaError_t readStats(long long out[kNumEsdfStats]) const {
+    return cudaMemcpy(out, stats_.get(), kNumEsdfStats * sizeof(long long), cudaMemcpyDeviceToHost);
+  }
+  cudaError_t readPhaseMax(int64_t* out, int n) const {
+    return cudaMemcpy(out, phase_max_.get(), (size_t)n * sizeof(long long), cudaMemcpyDeviceToHost);
+  }
+  int driver() const { return driver_; }
+  int reservedSms() const { return reserved_sms_; }
+
+ private:
+  static constexpr int kUnlinked = 0xFE;  // neighbour-table bytes: entries 0xFEFEFEFE, "unknown" (< -1), never linked
+  template <typename F>
+  cudaError_t eachSlotArray(F f);
+  int allocRecords(NvbMapper* m, int capacity);
+
+  int driver_ = 1;
+  int reserved_sms_ = 2;
+  int split_min_k_ = 0;   // exchange-slab wavefront: smallest grid ring that fetches its candidates' blocks split
+  int ges_switch_ = 160;  // gather-replay wavefront: rings with more members run as four-phase rings
+  bool prune_default_ = false;  // driver 3 and not switched off (NVB_CLEAR_PRUNE=0)
+  bool prune_ok_ = false;       // the parent boxes are upper bounds for every block (only driver 3 keeps them)
+  int update_seq_ = 0;
+  // per ESDF slot (eachSlotArray)
+  DeviceArray<int4> work_;
+  DeviceArray<int> upd_list_, clr_list_, cleared_list_;
+  DeviceArray<int> ring_a_, ring_b_, stamp_a_, stamp_b_;
+  DeviceArray<int> seed_upd_, seed_clr_;
+  DeviceArray<unsigned int> psum_;
+  DeviceArray<int> nbr_, nbr27_;
+  DeviceArray<int> cand_stamp_, cand_a_, cand_b_;
+  // the drivers' own
+  DeviceArray<unsigned char> shadow_;  // driver 2: a second ESDF slab (contents only live inside one launch)
+  DeviceArray<unsigned char> xslab_;   // driver 3: two slabs by ring parity of six faces per slot (7.5 KiB) ...
+  DeviceArray<int> xrec_;              // ... 2 x CTAs x xseg_ candidate records of 32 ints ...
+  int xseg_ = 0;
+  int xseg_grid_ = 0;                  // ... for a launch of this many CTAs ...
+  DeviceArray<int> xcounts_;           // ... and the barrier flags
+  // the rest
+  DeviceArray<unsigned long long> colset_;  // the slice update's columns
+  DeviceArray<int> cols_;
+  DeviceArray<int> dead_cleared_xyz_;
+  DeviceArray<unsigned int> clr_bits_;  // to-clear bitmap of the current update (2048 words)
+  DeviceArray<long long> stats_;
+  DeviceArray<unsigned int> barrier_;
+  DeviceArray<unsigned long long> phase_max_;
 };
 
 }  // namespace
@@ -375,11 +481,9 @@ struct NvbMapper {
   // NVB_PROJECTIVE_TSDF or NVB_PROJECTIVE_OCCUPANCY: which voxel type the projective layer (`tsdf` below) holds
   // (ProjectiveLayerType, mapper/mapper.h:52-53).
   int projective_layer_type = 0;
-  int esdf_persistent = 1;
-  int esdf_reserved_sms = 2;  // SMs the exchange-slab wavefront leaves to concurrently running kernels (nvb_esdf_wavex.cu)
-  int esdf_split_min_k = 0;   // exchange-slab wavefront: smallest grid ring that fetches its candidates' blocks split
 
   LayerSlab tsdf, esdf;
+  EsdfState esdf_state;  // the ESDF integrator's state beside its slab
   LayerSlab freespace;  // FreespaceLayer of a NVB_PROJECTIVE_TSDF_WITH_FREESPACE mapper
   LayerSlab color;      // ColorLayer, created by the first nvb_mapper_integrate_color
   NvbColorParams cp{};
@@ -388,8 +492,6 @@ struct NvbMapper {
   NvbFreespaceParams fp;
   NvbEsdfSliceParams sp;
   int esdf_mode = 0;                // EsdfMode: 0 unset, 1 3-D, 2 2-D slice (mapper.h:61, src/mapper/mapper.cpp:408-470)
-  DeviceArray<unsigned long long> colset;
-  DeviceArray<int> cols;
   long long fs_last_update_ms = 0;  // FreespaceIntegrator::last_update_time_ms_ (freespace_integrator.h:171)
   DeviceArray<int4> fs_work;
   SlabBounds bounds;
@@ -434,12 +536,12 @@ struct NvbMapper {
   // per-frame scratch
   DeviceArray<unsigned int> bits;
   DeviceArray<int4> frame_blocks;
-  int* frame_count = nullptr;  // in esdf_ints
+  int* frame_count = nullptr;  // in counters
   DeviceArray<unsigned long long> tile_state;
   DeviceArray<unsigned int> ticket;
   unsigned int ticket_base = 0;
   unsigned int epoch = 0;
-  int* error_dev = nullptr;  // in esdf_ints
+  int* error_dev = nullptr;  // in counters
 
   // depth / mask staging for host inputs
   DeviceArray<float> depth_stage[kStagingBuffers];
@@ -451,32 +553,13 @@ struct NvbMapper {
 
   TrackedBlocks tracker[kNumBlocksToUpdateTypes];  // by BlocksToUpdateType
 
-  // esdf scratch
-  DeviceArray<int4> work;
-  DeviceArray<int> esdf_ints;  // small counters block
-  DeviceArray<int> upd_list;
-  DeviceArray<int> clr_list;
-  DeviceArray<int> cleared_list;
-  DeviceArray<int> ring_a;
-  DeviceArray<int> ring_b;
-  DeviceArray<int> stamp_a;
-  DeviceArray<int> stamp_b;
-  DeviceArray<int> nbr;
-  DeviceArray<int> nbr27;
-  DeviceArray<unsigned char> shadow;
-  DeviceArray<unsigned char> xslab;  // exchange-slab wavefront (esdf_persistent == 3): 2 x capacity slots of six faces (7.5 KiB)
-  DeviceArray<int> xrec;             // ... 2 x CTAs x xseg candidate records of 32 ints ...
-  int xseg = 0;
-  int xseg_grid = 0;                 // CTAs of the exchange-slab launch the segments were sized for
-  DeviceArray<int> xcounts;          // ... and 2 x CTAs count pairs
-  DeviceArray<int> cand_stamp;
+  DeviceArray<DeviceCounters> counters;  // one element
   // decay integrators
   NvbTsdfDecayParams tdp;
   NvbOccupancyDecayParams odp;
   DeviceArray<int4> dead;        // deallocated projective blocks of the last decay call
   DeviceArray<int> skip_stamp;   // per projective slot: == skip_seq -> block excluded from this decay call
   int skip_seq = 0;
-  DeviceArray<int> dead_cleared_xyz;
   // map clearing: Mapper::cleared_blocks_ (every clearBlocksInLayers adds to it), ShapeClearer's scratch
   std::set<std::array<int, 3>> cleared_blocks;
   DeviceArray<int4> shape_sel;
@@ -529,22 +612,9 @@ struct NvbMapper {
   float last_T_L_C[16];
   NvbCamera last_cam;
   bool has_last_view = false;
-  DeviceArray<int> cand_a;
-  DeviceArray<int> cand_b;
-  int ges_switch = 160;
-  DeviceArray<int> seed_upd;
-  DeviceArray<int> seed_clr;
   // device-resident merge of block lists (nvb_blocks_union_segments): own scratch, usable on any stream
   DeviceArray<unsigned int> union_bits;
   DeviceArray<int> union_state;           // AABB, error flag, words in use
-  DeviceArray<unsigned int> clr_bits;     // to-clear bitmap of the current update (2048 words)
-  DeviceArray<unsigned int> psum;  // per ESDF slot: box of the block offsets its voxels' parents point into (clear-pass pruning)
-  bool prune_default = false;    // esdf_persistent == 3 and not switched off (NVB_CLEAR_PRUNE=0)
-  bool prune_ok = false;         // the summaries are upper bounds for every block (only the exchange-slab wavefront keeps them)
-  int update_seq = 0;
-  DeviceArray<long long> stats;
-  DeviceArray<unsigned int> barrier;
-  DeviceArray<unsigned long long> phase_max;
   DeviceArray<int> xyz_upload;
 
   // pinned host scratch
@@ -669,61 +739,153 @@ int SlabBounds::create() {
   return NVB_OK;
 }
 
-// Candidate records of the exchange-slab wavefront: one segment per CTA of the launch, by ring parity. In a ring a CTA
-// processes at most ceil(cap / CTAs) members (seeds or candidates, dealt round-robin) and registers at most 6 face neighbours
-// for each; the single-CTA tail registers at most 6 per group. So the segment is sized for the grid the launch really uses,
-// which shrinks as SMs are reserved.
-int allocWaveXRecords(NvbMapper* m, int cap) {
-  const int grid = esdfWaveXGrid(m->num_sms, m->esdf_reserved_sms);
-  NVB_CUDA(syncAll(m));
-  m->xrec = DeviceArray<int>();  // released first: the exact size follows the grid down as well as up
-  m->xseg = 6 * ((cap + grid - 1) / grid) + 64;
-  m->xseg_grid = grid;
-  const size_t n = 2 * (size_t)grid * m->xseg * 32;
-  NVB_CUDA(m->xrec.grow(m, n, n));
+// Every per-slot array once, for f(array, elements per slot, fill byte of a new allocation, whether growth keeps the
+// contents, whether reset() refills it). The kept ones carry state from one update to the next.
+template <typename F>
+cudaError_t EsdfState::eachSlotArray(F f) {
+  cudaError_t e = cudaSuccess;
+  const auto a = [&](auto& array, size_t per_slot, int fill, bool keep, bool reset) {
+    if (e == cudaSuccess) e = f(array, per_slot, fill, keep, reset);
+  };
+  constexpr bool kReset = true;
+  a(work_, 1, kNoFill, false, false);
+  a(upd_list_, 1, kNoFill, false, false);
+  a(clr_list_, 1, kNoFill, false, false);
+  a(cleared_list_, 1, 0, kKeepContents, false);
+  a(ring_a_, 1, kNoFill, false, false);
+  a(ring_b_, 1, kNoFill, false, false);
+  a(stamp_a_, 1, 0, kKeepContents, false);
+  a(stamp_b_, 1, 0, kKeepContents, false);
+  a(seed_upd_, 1, 0, kKeepContents, kReset);
+  a(seed_clr_, 1, 0, kKeepContents, kReset);
+  a(psum_, 2, 0, kKeepContents, kReset);
+  a(nbr_, 6, kUnlinked, kKeepContents, kReset);
+  a(nbr27_, 27, kUnlinked, kKeepContents, kReset);
+  a(cand_stamp_, 1, 0, kKeepContents, false);
+  a(cand_a_, 1, kNoFill, false, false);
+  a(cand_b_, 1, kNoFill, false, false);
+  return e;
+}
+
+int EsdfState::create(NvbMapper* m, int capacity, int driver) {
+  driver_ = driver;
+  split_min_k_ = esdfWaveXSplitMinK();
+  if (const char* e = getenv("NVB_GES_SWITCH")) ges_switch_ = atoi(e);
+  const char* e = getenv("NVB_CLEAR_PRUNE");
+  prune_default_ = prune_ok_ = driver == 3 && !(e && atoi(e) == 0);
+  if (int rc = grow(m, capacity)) return rc;
+  const int one = 1;
+  NVB_CUDA(cudaMemcpyAsync(&m->counters.get()->ring_id, &one, sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(clr_bits_.grow(m, 2048, 2048));
+  NVB_CUDA(stats_.grow(m, kNumEsdfStats, kNumEsdfStats, 0));
+  NVB_CUDA(phase_max_.grow(m, kPhaseMaxEntries, kPhaseMaxEntries, 0));
+  NVB_CUDA(barrier_.grow(m, 16, 16, 0));  // 64 bytes
   return NVB_OK;
 }
 
-// The ESDF slab's companions, at `cap` slots; the ones that carry state from one update to the next keep their contents.
-int allocEsdfScratch(NvbMapper* m, int cap) {
-  const size_t n = cap;
-  NVB_CUDA(m->work.grow(m, n, n));
-  NVB_CUDA(m->upd_list.grow(m, n, n));
-  NVB_CUDA(m->clr_list.grow(m, n, n));
-  NVB_CUDA(m->cleared_list.grow(m, n, n, 0, kKeepContents));
-  NVB_CUDA(m->ring_a.grow(m, n, n));
-  NVB_CUDA(m->ring_b.grow(m, n, n));
-  NVB_CUDA(m->stamp_a.grow(m, n, n, 0, kKeepContents));
-  NVB_CUDA(m->stamp_b.grow(m, n, n, 0, kKeepContents));
-  NVB_CUDA(m->seed_upd.grow(m, n, n, 0, kKeepContents));
-  NVB_CUDA(m->seed_clr.grow(m, n, n, 0, kKeepContents));
-  NVB_CUDA(m->psum.grow(m, 2 * n, 2 * n, 0, kKeepContents));
-  // neighbour table: 0xFE bytes = "unknown" (< -1) for slots that were never linked
-  NVB_CUDA(m->nbr.grow(m, 6 * n, 6 * n, 0xFE, kKeepContents));
-  NVB_CUDA(m->nbr27.grow(m, 27 * n, 27 * n, 0xFE, kKeepContents));
-  NVB_CUDA(m->cand_stamp.grow(m, n, n, 0, kKeepContents));
-  NVB_CUDA(m->cand_a.grow(m, n, n));
-  NVB_CUDA(m->cand_b.grow(m, n, n));
-  if (m->esdf_persistent == 2) {
-    // gather-emulate-sweep wavefront: second ESDF slab (contents only live inside one launch)
-    NVB_CUDA(m->shadow.grow(m, n * kEsdfBlockBytes, n * kEsdfBlockBytes));
-  }
-  if (m->esdf_persistent == 3) {
-    // exchange-slab wavefront: two slabs by ring parity + the candidate records (contents only live inside one launch)
-    NVB_CUDA(m->xslab.grow(m, esdfWaveXSlabBytes(cap), esdfWaveXSlabBytes(cap)));
-    int rc;
-    if ((rc = allocWaveXRecords(m, cap))) return rc;
+int EsdfState::grow(NvbMapper* m, int capacity) {
+  const size_t n = capacity;
+  const auto grow_slots = [&](auto& a, size_t per_slot, int fill, bool keep, bool) {
+    return a.grow(m, per_slot * n, per_slot * n, fill, keep);
+  };
+  NVB_CUDA(eachSlotArray(grow_slots));
+  if (driver_ == 2) NVB_CUDA(shadow_.grow(m, n * kEsdfBlockBytes, n * kEsdfBlockBytes));
+  if (driver_ == 3) {
+    NVB_CUDA(xslab_.grow(m, esdfWaveXSlabBytes(capacity), esdfWaveXSlabBytes(capacity)));
+    if (int rc = allocRecords(m, capacity)) return rc;
     const size_t flags = esdfWaveXFlagBytes() / sizeof(int);
-    NVB_CUDA(m->xcounts.grow(m, flags, flags, 0));
+    NVB_CUDA(xcounts_.grow(m, flags, flags, 0));
   }
   return NVB_OK;
+}
+
+// Candidate records of the exchange-slab wavefront: one segment per CTA of the launch, by ring parity. In a ring a CTA
+// processes at most ceil(capacity / CTAs) members (seeds or candidates, dealt round-robin) and registers at most 6 face
+// neighbours for each; the single-CTA tail registers at most 6 per group. So the segment is sized for the grid the launch
+// really uses, which shrinks as SMs are reserved.
+int EsdfState::allocRecords(NvbMapper* m, int capacity) {
+  const int grid = esdfWaveXGrid(m->num_sms, reserved_sms_);
+  NVB_CUDA(syncAll(m));
+  xrec_ = DeviceArray<int>();  // released first: the exact size follows the grid down as well as up
+  xseg_ = 6 * ((capacity + grid - 1) / grid) + 64;
+  xseg_grid_ = grid;
+  const size_t n = 2 * (size_t)grid * xseg_ * 32;
+  NVB_CUDA(xrec_.grow(m, n, n));
+  return NVB_OK;
+}
+
+int EsdfState::setReservedSms(NvbMapper* m, int n) {
+  reserved_sms_ = n;
+  if (xrec_.get() && esdfWaveXGrid(m->num_sms, n) != xseg_grid_) return allocRecords(m, m->esdf.capacity());
+  return NVB_OK;
+}
+
+int EsdfState::reset(NvbMapper* m) {
+  DeviceCounters* ctr = m->counters.get();
+  NVB_CUDA(cudaMemsetAsync(&ctr->cleared_count, 0, sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(&ctr->cleared_seq, 0, sizeof(int), m->stream));
+  NVB_CUDA(cudaMemsetAsync(&ctr->dead_cleared_count, 0, sizeof(int), m->stream));
+  const auto refill = [&](auto& a, size_t, int fill, bool, bool reset) {
+    return reset ? cudaMemsetAsync(a.get(), fill, a.size() * sizeof(*a.get()), m->stream) : cudaSuccess;
+  };
+  NVB_CUDA(eachSlotArray(refill));
+  prune_ok_ = prune_default_;
+  return NVB_OK;
+}
+
+int EsdfState::blocksWritten(NvbMapper* m) {
+  prune_ok_ = false;
+  NVB_CUDA(cudaMemsetAsync(nbr_.get(), kUnlinked, nbr_.size() * sizeof(int), m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  return NVB_OK;
+}
+
+int EsdfState::reserveSliceColumns(NvbMapper* m, size_t columns) {
+  const size_t keys = (size_t)nextPow2(2ll * columns);
+  NVB_CUDA(colset_.grow(m, keys, keys));
+  NVB_CUDA(cols_.grow(m, 2 * columns, 2 * columns));
+  return NVB_OK;
+}
+
+int EsdfState::reserveDeadCleared(NvbMapper* m) {
+  const size_t n = 3 * (size_t)m->esdf.capacity();
+  NVB_CUDA(dead_cleared_xyz_.grow(m, n, n, kNoFill, kKeepContents));
+  return NVB_OK;
+}
+
+EsdfCtx EsdfState::ctx(DeviceCounters* ctr) const {
+  EsdfCtx c{};
+  c.work = work_.get(), c.work_count = &ctr->work_count;
+  c.upd_list = upd_list_.get(), c.upd_count = &ctr->upd_count;
+  c.clr_list = clr_list_.get(), c.clr_count = &ctr->clr_count;
+  c.clr_aabb = ctr->clr_aabb;
+  c.cleared_list = cleared_list_.get(), c.cleared_count = &ctr->cleared_count;
+  c.ring_a = ring_a_.get(), c.ring_b = ring_b_.get();
+  c.ring_count = ctr->ring_count;
+  c.tail_state = ctr->tail_state;
+  c.stamp_a = stamp_a_.get(), c.stamp_b = stamp_b_.get();
+  c.ring_id = &ctr->ring_id;
+  c.nbr = nbr_.get(), c.seed_upd = seed_upd_.get(), c.seed_clr = seed_clr_.get();
+  c.clr_bits = clr_bits_.get();
+  c.psum = psum_.get(), c.prune = (prune_ok_ && driver_ == 3) ? 1 : 0;
+  c.nbr27 = nbr27_.get(), c.shadow = shadow_.get(), c.cand_stamp = cand_stamp_.get();
+  c.xslab = xslab_.get(), c.xrec = xrec_.get(), c.xtail = ctr->xtail, c.xseg = xseg_, c.xcounts = xcounts_.get();
+  c.xsplit_min_k = split_min_k_;
+  c.ges_counts = ctr->ges_counts;
+  c.cand_a = cand_a_.get(), c.cand_b = cand_b_.get(), c.ges_switch = ges_switch_;
+  c.colset_keys = colset_.get(), c.colset_mask = colset_.size() ? (unsigned int)(colset_.size() - 1) : 0u;
+  c.cols = cols_.get(), c.cols_count = &ctr->cols_count;
+  c.dead_cleared_xyz = dead_cleared_xyz_.get();
+  c.dead_cleared_count = dead_cleared_xyz_.get() ? &ctr->dead_cleared_count : nullptr;
+  c.cleared_seq = &ctr->cleared_seq;
+  c.update_seq = update_seq_;
+  c.barrier = barrier_.get();
+  c.phase_max = phase_max_.get();
+  c.stats = stats_.get();
+  return c;
 }
 
 constexpr int kHostListCap = 1 << 15;  // entries of the pinned frame-list buffer (512 KiB)
-
-// esdf_ints layout
-enum { kWorkCount = 0, kUpdCount = 1, kClrCount = 2, kClrAabb = 3, kClearedCount = 9, kRingCount = 10, kRingId = 14,
-       kTodoCount = 15, kFrameCount = 16, kError = 17, kClearedSeq = 18, kTailState = 20, kDeadCount = 22, kDeadClearedCount = 23, kGesCounts = 24, kTodoFsCount = 28, kFsWorkCount = 29, kColsCount = 30, kColorWorkCount = 31, kXTail = 32, kTodoMeshCount = 36, kNumInts = 40 };
 
 // ---- The block-update tracker: which consumers are told when a block changes, and how each one is refilled and reset.
 
@@ -731,14 +893,15 @@ enum { kWorkCount = 0, kUpdCount = 1, kClrCount = 2, kClrAabb = 3, kClearedCount
 // layer exists. Their arrays follow the projective slab's capacity and keep their contents.
 int growTracker(NvbMapper* m, int cap) {
   const bool has[kNumBlocksToUpdateTypes] = {true, m->freespace.exists(), m->mesh.exists()};
-  const int count_at[kNumBlocksToUpdateTypes] = {kTodoCount, kTodoFsCount, kTodoMeshCount};
+  DeviceCounters* ctr = m->counters.get();
+  int* const count[kNumBlocksToUpdateTypes] = {&ctr->todo_count, &ctr->todo_fs_count, &ctr->todo_mesh_count};
   const size_t n = cap;
   for (int k = 0; k < kNumBlocksToUpdateTypes; k++) {
     if (!has[k]) continue;
     TrackedBlocks& t = m->tracker[k];
     NVB_CUDA(t.dirty.grow(m, n, n, 0, kKeepContents));
     NVB_CUDA(t.slots.grow(m, n, n, 0, kKeepContents));
-    t.count = m->esdf_ints.get() + count_at[k];
+    t.count = count[k];
   }
   return NVB_OK;
 }
@@ -790,38 +953,10 @@ int resetTracker(NvbMapper* m) {
 float logOddsFromProbability(float p);
 
 EsdfCtx makeEsdfCtx(NvbMapper* m) {
-  EsdfCtx c{};
+  EsdfCtx c = m->esdf_state.ctx(m->counters.get());
   c.tsdf = m->tsdf.dev(), c.esdf = m->esdf.dev();
   c.freespace = m->freespace.dev();
   c.use_freespace = m->projective_layer_type == NVB_PROJECTIVE_TSDF_WITH_FREESPACE ? 1 : 0;
-  c.work = m->work.get();
-  c.work_count = m->esdf_ints.get() + kWorkCount;
-  c.upd_list = m->upd_list.get(), c.upd_count = m->esdf_ints.get() + kUpdCount;
-  c.clr_list = m->clr_list.get(), c.clr_count = m->esdf_ints.get() + kClrCount;
-  c.clr_aabb = m->esdf_ints.get() + kClrAabb;
-  c.cleared_list = m->cleared_list.get(), c.cleared_count = m->esdf_ints.get() + kClearedCount;
-  c.ring_a = m->ring_a.get(), c.ring_b = m->ring_b.get();
-  c.ring_count = m->esdf_ints.get() + kRingCount;
-  c.tail_state = m->esdf_ints.get() + kTailState;
-  c.stamp_a = m->stamp_a.get(), c.stamp_b = m->stamp_b.get();
-  c.ring_id = m->esdf_ints.get() + kRingId;
-  c.nbr = m->nbr.get(), c.seed_upd = m->seed_upd.get(), c.seed_clr = m->seed_clr.get();
-  c.clr_bits = m->clr_bits.get();
-  c.psum = m->psum.get(), c.prune = (m->prune_ok && m->esdf_persistent == 3) ? 1 : 0;
-  c.nbr27 = m->nbr27.get(), c.shadow = m->shadow.get(), c.cand_stamp = m->cand_stamp.get();
-  c.xslab = m->xslab.get(), c.xrec = m->xrec.get(), c.xtail = m->esdf_ints.get() + kXTail, c.xseg = m->xseg, c.xcounts = m->xcounts.get();
-  c.xsplit_min_k = m->esdf_split_min_k;
-  c.ges_counts = m->esdf_ints.get() + kGesCounts;
-  c.cand_a = m->cand_a.get(), c.cand_b = m->cand_b.get(), c.ges_switch = m->ges_switch;
-  c.colset_keys = m->colset.get(), c.colset_mask = m->colset.size() ? (unsigned int)(m->colset.size() - 1) : 0u;
-  c.cols = m->cols.get(), c.cols_count = m->esdf_ints.get() + kColsCount;
-  c.dead_cleared_xyz = m->dead_cleared_xyz.get();
-  c.dead_cleared_count = m->dead_cleared_xyz.get() ? m->esdf_ints.get() + kDeadClearedCount : nullptr;
-  c.cleared_seq = m->esdf_ints.get() + kClearedSeq;
-  c.update_seq = m->update_seq;
-  c.barrier = m->barrier.get();
-  c.phase_max = m->phase_max.get();
-  c.stats = m->stats.get();
   c.error = m->error_dev;
   // esdf_integrator.cu:693-696, 672-676
   const float max_esdf_distance_vox = m->ep.max_esdf_distance_m / m->voxel_size;
@@ -968,7 +1103,7 @@ int ensureEsdfCapacity(NvbMapper* m, long long need) {
   if (need <= m->esdf.capacity()) return NVB_OK;
   if ((rc = grownCapacity(m->esdf.capacity(), need, "ESDF layer", &cap))) return rc;
   NVB_CUDA(m->esdf.grow(m, cap));
-  return allocEsdfScratch(m, cap);
+  return m->esdf_state.grow(m, cap);
 }
 
 // Every call that adds blocks reserves room through its slab's kind. The projective slab (TSDF or occupancy) counts them in
@@ -1328,14 +1463,9 @@ int enqueueEsdf(NvbMapper* m, const int* in_xyz_dev, int n_explicit, bool from_t
   m->esdf_mode = want_mode;
   const int upper = std::max(1, from_tracker ? m->bounds.projectiveUpper(m->tsdf.capacity()) : n_explicit);
   if ((rc = reserveEsdf(m, from_tracker ? 0 : n_explicit))) return rc;
-  if (slice) {
-    // column set + column list sized to the projective layer
-    const size_t columns = std::max(m->tsdf.capacity(), upper);
-    const size_t want = (size_t)nextPow2(2ll * columns);
-    NVB_CUDA(m->colset.grow(m, want, want));
-    NVB_CUDA(m->cols.grow(m, 2 * columns, 2 * columns));
-  }
-  m->update_seq++;
+  // the slice's columns: at most one per block of the projective layer
+  if (slice && (rc = m->esdf_state.reserveSliceColumns(m, std::max(m->tsdf.capacity(), upper)))) return rc;
+  m->esdf_state.beginUpdate();
   EsdfCtx c = makeEsdfCtx(m);
   const TrackerList todo = from_tracker ? m->tracker[kEsdfBlocks].list() : TrackerList{};
   c.tracker_dirty = todo.dirty;
@@ -1373,7 +1503,8 @@ int enqueueEsdf(NvbMapper* m, const int* in_xyz_dev, int n_explicit, bool from_t
       m->launches += 2;
     }
   };
-  if (m->esdf_persistent) {
+  const int driver = m->esdf_state.driver();
+  if (driver) {
     // The whole ESDF chain (allocate, mark, clear, wavefront) runs back to back on the side stream; the frame's
     // critical path has no cross-stream hand-over. `stream` only waits for the mark kernel: after it nothing on
     // the side stream reads the projective layer or the tracker, so the next frame's raycast / compaction /
@@ -1392,9 +1523,9 @@ int enqueueEsdf(NvbMapper* m, const int* in_xyz_dev, int n_explicit, bool from_t
     m->launches++;
     endStageOn(m, es);
     beginStageOn(m, 5, es);
-    e = m->esdf_persistent == 3   ? launchEsdfComputeX(c, m->num_sms, m->esdf_reserved_sms, es, &launches)
-        : m->esdf_persistent == 2 ? launchEsdfComputeGes(c, m->num_sms, es, &launches)
-                                  : launchEsdfComputePersistent(c, m->num_sms, es, &launches);
+    e = driver == 3   ? launchEsdfComputeX(c, m->num_sms, m->esdf_state.reservedSms(), es, &launches)
+        : driver == 2 ? launchEsdfComputeGes(c, m->num_sms, es, &launches)
+                      : launchEsdfComputePersistent(c, m->num_sms, es, &launches);
     endStageOn(m, es);
     if (e == cudaSuccess) {
       NVB_CUDA(cudaEventRecord(m->esdf_done, es));
@@ -1494,14 +1625,6 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   nvb_default_ground_plane_params(&m->gp);
   m->projective_layer_type = opts->projective_layer_type;
   m->keep_last_view = opts->keep_last_view ? 1 : 0;
-  m->esdf_persistent = opts->esdf_persistent;
-  m->esdf_split_min_k = esdfWaveXSplitMinK();
-  if (const char* e = getenv("NVB_GES_SWITCH")) m->ges_switch = atoi(e);
-  {
-    const char* e = getenv("NVB_CLEAR_PRUNE");
-    m->prune_default = m->esdf_persistent == 3 && !(e && atoi(e) == 0);
-    m->prune_ok = m->prune_default;
-  }
   NVB_CUDA(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
   NVB_CUDA(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
   {
@@ -1530,17 +1653,11 @@ static int createMapperResources(const NvbMapperOptions* opts, NvbMapper* m) {
   NVB_CUDA(m->esdf.create(m, ecap, kEsdfBlockBytes));
   if (m->projective_layer_type == NVB_PROJECTIVE_TSDF_WITH_FREESPACE)
     NVB_CUDA(m->freespace.create(m, tcap, kFreespaceBlockBytes));
-  NVB_CUDA(m->esdf_ints.grow(m, kNumInts, kNumInts, 0));
+  NVB_CUDA(m->counters.grow(m, 1, 1, 0));
   if ((rc = growTracker(m, tcap))) return rc;
-  if ((rc = allocEsdfScratch(m, ecap))) return rc;
-  const int one = 1;
-  NVB_CUDA(cudaMemcpyAsync(m->esdf_ints.get() + kRingId, &one, sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  m->frame_count = m->esdf_ints.get() + kFrameCount;
-  m->error_dev = m->esdf_ints.get() + kError;
-  NVB_CUDA(m->clr_bits.grow(m, 2048, 2048));
-  NVB_CUDA(m->stats.grow(m, 16, 16, 0));
-  NVB_CUDA(m->phase_max.grow(m, 4000, 4000, 0));
-  NVB_CUDA(m->barrier.grow(m, 16, 16, 0));  // 64 bytes
+  if ((rc = m->esdf_state.create(m, ecap, opts->esdf_persistent))) return rc;
+  m->frame_count = &m->counters.get()->frame_count;
+  m->error_dev = &m->counters.get()->error;
   NVB_CUDA(m->ticket.grow(m, 16, 16, 0));   // 64 bytes
   NVB_CUDA(allocPinned(&m->h_ints, 64));
   memset(m->h_ints.get(), 0, 64 * sizeof(int));
@@ -1609,15 +1726,7 @@ static int resetLayers(NvbMapper* m) {
     if (L->exists()) NVB_CUDA(L->empty(m->stream));
   int rc;
   if ((rc = resetTracker(m))) return rc;
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kClearedCount, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kClearedSeq, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->esdf_ints.get() + kDeadClearedCount, 0, sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->seed_upd.get(), 0, (size_t)m->esdf.capacity() * sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->seed_clr.get(), 0, (size_t)m->esdf.capacity() * sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->psum.get(), 0, 2 * (size_t)m->esdf.capacity() * sizeof(int), m->stream));
-  m->prune_ok = m->prune_default;  // an empty layer: every summary is exact again
-  NVB_CUDA(cudaMemsetAsync(m->nbr.get(), 0xFE, (size_t)m->esdf.capacity() * 6 * sizeof(int), m->stream));
-  NVB_CUDA(cudaMemsetAsync(m->nbr27.get(), 0xFE, (size_t)m->esdf.capacity() * 27 * sizeof(int), m->stream));
+  if ((rc = m->esdf_state.reset(m))) return rc;
   NVB_CUDA(cudaMemsetAsync(m->error_dev, 0, sizeof(int), m->stream));
   if (m->mesh.exists()) NVB_CUDA(cudaMemsetAsync(m->mesh_state.get(), 0, kArenaInts * sizeof(int), m->stream));
   m->bounds.reset(0, 0, 0);
@@ -1738,9 +1847,7 @@ namespace {
 int ensureRemovalScratch(NvbMapper* m) {
   const size_t dead = m->tsdf.capacity();
   NVB_CUDA(m->dead.grow(m, dead, dead));
-  const size_t cleared = 3 * (size_t)m->esdf.capacity();
-  NVB_CUDA(m->dead_cleared_xyz.grow(m, cleared, cleared, kNoFill, kKeepContents));
-  return NVB_OK;
+  return m->esdf_state.reserveDeadCleared(m);
 }
 
 // Mapper::clearBlocksInLayers (src/mapper/mapper.cpp:546-634) for the n_dead {slot, x, y, z} of m->dead, whose projective
@@ -1748,7 +1855,7 @@ int ensureRemovalScratch(NvbMapper* m) {
 // the freespace, colour and mesh twins go, every touched hash is rebuilt without them, and the indices join
 // cleared_blocks_. `removed` receives the dead list. The tracker is the caller's.
 int removeDeadBlocks(NvbMapper* m, int n_dead, std::vector<int4>* removed) {
-  const int* dead_count = m->esdf_ints.get() + kDeadCount;
+  const int* dead_count = &m->counters.get()->dead_count;
   EsdfCtx c = makeEsdfCtx(m);
   if (m->esdf_mode == 2) {
     c.slice_mode = 1;
@@ -1758,9 +1865,7 @@ int removeDeadBlocks(NvbMapper* m, int n_dead, std::vector<int4>* removed) {
     c.slice_out_bz = (int)std::floor(m->sp.slice_height_m / m->block_size);
   }
   launchEsdfRemoveBlocks(c, m->dead.get(), dead_count, n_dead, m->stream);
-  // Voxels of other blocks may keep parents inside the removed blocks: the reference clears them when they happen to be
-  // candidates of a later clear pass, which the per-block parent boxes cannot tell. No pruning from here on.
-  m->prune_ok = false;
+  m->esdf_state.forgetParentBoxes();
   std::vector<LayerSlab*> touched = {&m->tsdf, &m->esdf};
   if (m->freespace.exists()) {
     launchRemoveBlocks(m->freespace.dev(), m->dead.get(), dead_count, n_dead, m->stream);
@@ -1856,7 +1961,7 @@ int32_t nvb_mapper_decay(NvbMapper* m, const NvbDecayExclusion* exclusion, const
     a.cam = *cam;
   }
   a.dead = m->dead.get();
-  a.dead_count = m->esdf_ints.get() + kDeadCount;
+  a.dead_count = &m->counters.get()->dead_count;
   NVB_CUDA(cudaMemsetAsync(a.dead_count, 0, sizeof(int), m->stream));
   launchDecay(a, m->num_sms, m->stream);
   m->launches++;
@@ -1908,7 +2013,7 @@ int freespaceUpdateImpl(NvbMapper* m, const int* in_xyz_dev, int n_explicit, lon
   a.tsdf = m->tsdf.dev(), a.fs = m->freespace.dev();
   if (in_xyz_dev) a.in_xyz = in_xyz_dev, a.n_explicit = n_explicit;
   else a.todo = m->tracker[kFreespaceBlocks].list();
-  a.work = m->fs_work.get(), a.work_count = m->esdf_ints.get() + kFsWorkCount, a.error = m->error_dev;
+  a.work = m->fs_work.get(), a.work_count = &m->counters.get()->fs_work_count, a.error = m->error_dev;
   a.max_tsdf_distance_for_occupancy_m = m->fp.max_tsdf_distance_for_occupancy_m;
   a.max_unobserved_ms = m->fp.max_unobserved_to_keep_consecutive_occupancy_ms;
   a.min_free_ms = m->fp.min_duration_since_occupied_for_freespace_ms;
@@ -1994,7 +2099,7 @@ int32_t nvb_mapper_clear_outside_radius(NvbMapper* m, const float center[3], flo
   int rc = ensureRemovalScratch(m);
   if (rc) return rc;
   // getBlocksOutsideRadius over the projective layer's blocks (TSDF for kTsdf / kTsdfWithFreespace, occupancy for kOccupancy)
-  int* dead_count = m->esdf_ints.get() + kDeadCount;
+  int* dead_count = &m->counters.get()->dead_count;
   NVB_CUDA(cudaMemsetAsync(dead_count, 0, sizeof(int), m->stream));
   launchSelectOutsideRadius(m->tsdf.dev(), center, radius, m->block_size, m->dead.get(), dead_count, m->stream);
   m->launches++;
@@ -2326,7 +2431,7 @@ int32_t nvb_mapper_integrate_color(NvbMapper* m, const uint8_t* color, const uin
     a.w_old_h = roundThroughHalf(w_old), a.w_new_h = roundThroughHalf(w_new);
   }
   a.work = m->color_work.get();
-  a.work_count = m->esdf_ints.get() + kColorWorkCount;
+  a.work_count = &m->counters.get()->color_work_count;
   a.error = m->error_dev;
   a.rows = rows, a.cols = cols;
   a.depth_subsample = rows / a.drows;  // projective_integrator_impl.cuh:320
@@ -2354,7 +2459,7 @@ int32_t nvb_mapper_last_color_blocks(NvbMapper* m, int32_t* out_xyz_host, int32_
   if (out_count) *out_count = 0;
   if (!m->color.exists() || !m->color_work.get()) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
-  return readBlockList(m, m->esdf_ints.get() + kColorWorkCount, m->color_work.get(), Record::kXyzFirst, false, out_xyz_host,
+  return readBlockList(m, &m->counters.get()->color_work_count, m->color_work.get(), Record::kXyzFirst, false, out_xyz_host,
                        cap, out_count);
 }
 
@@ -2887,14 +2992,13 @@ int32_t nvb_esdf_slice_aabb(NvbMapper* m, float slice_height_m, float aabb_out[6
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   const int zb = (int)std::floor(slice_height_m / m->block_size);
-  int* box_dev = m->esdf_ints.get() + kGesCounts;  // four scratch ints (the wavefront is idle)
+  int* box_dev = m->counters.get()->slice_box;
   const int init[4] = {INT32_MAX, INT32_MAX, INT32_MIN, INT32_MIN};
   NVB_CUDA(cudaMemcpyAsync(box_dev, init, sizeof(init), cudaMemcpyHostToDevice, m->stream));
   launchSliceAabb(m->esdf.dev(), zb, box_dev, m->stream);
   int box[4];
   NVB_CUDA(cudaMemcpyAsync(box, box_dev, sizeof(box), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  NVB_CUDA(cudaMemsetAsync(box_dev, 0, sizeof(box), m->stream));
   m->launches++;
   if (box[0] > box[2]) return NVB_OK;  // no block at that height: empty AABB (:166-168)
   // getAABBOfBlock: [index * block_size, (index + 1) * block_size]
@@ -3111,11 +3215,9 @@ int32_t nvb_mapper_get_cache_last_viewpoint(const NvbMapper* m) { return m ? m->
 int32_t nvb_mapper_set_esdf_reserved_sms(NvbMapper* m, int32_t reserved_sms) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
   if (reserved_sms < 0 || reserved_sms > 64) return fail(NVB_ERR_INVALID_ARGUMENT, "reserved_sms must be in [0, 64]");
-  m->esdf_reserved_sms = reserved_sms;
-  if (m->xrec.get() && esdfWaveXGrid(m->num_sms, reserved_sms) != m->xseg_grid) return allocWaveXRecords(m, m->esdf.capacity());
-  return NVB_OK;
+  return m->esdf_state.setReservedSms(m, reserved_sms);
 }
-int32_t nvb_mapper_get_esdf_reserved_sms(const NvbMapper* m) { return m ? m->esdf_reserved_sms : 0; }
+int32_t nvb_mapper_get_esdf_reserved_sms(const NvbMapper* m) { return m ? m->esdf_state.reservedSms() : 0; }
 
 int32_t nvb_mapper_set_depth_preprocessing(NvbMapper* m, int32_t enable, int32_t num_dilations) {
   if (!m) return fail(NVB_ERR_INVALID_ARGUMENT, "null mapper");
@@ -3268,17 +3370,13 @@ int32_t nvb_layer_set_blocks(NvbMapper* m, int32_t layer, const int32_t* xyz_hos
   NVB_CUDA(host.in(static_cast<const unsigned char*>(in_host), (size_t)n * L->dev().block_bytes, &in_dev));
   launchScatterBlocks(L->dev(), esdf, xyz_dev, n, in_dev, m->error_dev, m->stream);
   m->launches++;
-  if (esdf) m->prune_ok = false;  // voxels written from outside: the parent boxes are no longer bounds
   NVB_CUDA(syncAll(m));
   if (projective) {
     // a later updateEsdf must see these blocks: the ESDF consumer's next update covers every block. Only the ESDF is
     // told; the freespace and mesh consumers keep their lists.
     m->tracker[kEsdfBlocks].initialized = false;
   } else if (esdf) {
-    // blocks created outside the ESDF update path are not linked: forget the neighbour table,
-    // it is re-resolved lazily through the hash
-    NVB_CUDA(cudaMemsetAsync(m->nbr.get(), 0xFE, (size_t)m->esdf.capacity() * 6 * sizeof(int), m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
+    if (int rc = m->esdf_state.blocksWritten(m)) return rc;
   }
   return checkDeviceError(m);
 }
@@ -3404,8 +3502,7 @@ int32_t nvb_mapper_load_map(NvbMapper* m, const char* path, int32_t loaded_block
     LayerSlab* L = want[k] ? savedLayerOf(m, k) : nullptr;
     if (L && (rc = uploadLoadedLayer(m, L, in[k]))) return rc;
   }
-  // the clear pass's parent boxes of the loaded ESDF blocks: pruning stays exact
-  launchEsdfParentBoxes(m->esdf.dev(), n_esdf, m->psum.get(), m->stream);
+  m->esdf_state.buildParentBoxes(m->esdf.dev(), n_esdf, m->stream);
   m->launches++;
   // the fill-level bounds from the real counts (tightenEsdfBound)
   m->bounds.reset(n_proj, std::max(0, n_esdf - n_proj), 0);
@@ -3467,9 +3564,9 @@ int32_t nvb_mapper_last_esdf_stats(NvbMapper* m, int64_t out[8]) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
-  long long tmp[8];
-  NVB_CUDA(cudaMemcpy(tmp, m->stats.get(), sizeof(tmp), cudaMemcpyDeviceToHost));
-  for (int i = 0; i < 8; i++) out[i] = tmp[i];
+  long long s[kNumEsdfStats];
+  NVB_CUDA(m->esdf_state.readStats(s));
+  std::copy(s + kStatWork, s + kStatRings + 1, out);
   return NVB_OK;
 }
 
@@ -3477,13 +3574,9 @@ int32_t nvb_mapper_esdf_time_split(NvbMapper* m, int64_t out[4]) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
-  long long tmp[5];
-  NVB_CUDA(cudaMemcpy(tmp, m->stats.get() + 8, sizeof(tmp), cudaMemcpyDeviceToHost));
-  for (int i = 0; i < 4; i++) out[i] = tmp[i];
-  out[0] = tmp[0];
-  // [1]+[2] are CTA 0's own work; tmp[4] is the sum over phases of the slowest CTA's work: report it in [1]
-  // of a second call convention: keep the API at 4 entries, fold it in as out[2] = slowest-CTA work total.
-  out[2] = tmp[4];
+  long long s[kNumEsdfStats];
+  NVB_CUDA(m->esdf_state.readStats(s));
+  out[0] = s[kStatBarrierNs], out[1] = s[kStatAxisNs], out[2] = s[kStatSlowestCtaWorkNs], out[3] = s[kStatBarriers];
   return NVB_OK;
 }
 
@@ -3491,9 +3584,9 @@ int32_t nvb_mapper_esdf_clear_blocks_read(NvbMapper* m, int64_t* out) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
-  long long v = 0;
-  NVB_CUDA(cudaMemcpy(&v, m->stats.get() + 13, sizeof(v), cudaMemcpyDeviceToHost));
-  *out = v;
+  long long s[kNumEsdfStats];
+  NVB_CUDA(m->esdf_state.readStats(s));
+  *out = s[kStatClearBlocksRead];
   return NVB_OK;
 }
 
@@ -3501,9 +3594,9 @@ int32_t nvb_mapper_esdf_split_stats(NvbMapper* m, int64_t out[2]) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
-  long long tmp[2];
-  NVB_CUDA(cudaMemcpy(tmp, m->stats.get() + 14, sizeof(tmp), cudaMemcpyDeviceToHost));
-  out[0] = tmp[0], out[1] = tmp[1];
+  long long s[kNumEsdfStats];
+  NVB_CUDA(m->esdf_state.readStats(s));
+  out[0] = s[kStatSplitCandidates], out[1] = s[kStatRestFetches];
   return NVB_OK;
 }
 
@@ -3511,8 +3604,7 @@ int32_t nvb_mapper_debug_phase_max(NvbMapper* m, int64_t* out, int32_t cap) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
-  if (cap > 4000) cap = 4000;
-  NVB_CUDA(cudaMemcpy(out, m->phase_max.get(), (size_t)cap * sizeof(long long), cudaMemcpyDeviceToHost));
+  NVB_CUDA(m->esdf_state.readPhaseMax(out, std::min(cap, (int32_t)kPhaseMaxEntries)));
   return NVB_OK;
 }
 

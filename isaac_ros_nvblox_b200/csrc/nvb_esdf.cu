@@ -51,10 +51,10 @@ __device__ __forceinline__ void resetEsdfUpdate(const EsdfCtx& c, int n) {
     c.ring_count[2] = 0;  // mark-kernel "CTAs done" counter
     c.ges_counts[0] = c.ges_counts[1] = c.ges_counts[2] = c.ges_counts[3] = 0;
     *c.barrier = 0;
-    for (int k = 0; k < 16; k++) c.stats[k] = 0;
-    c.stats[0] = n;
+    for (int k = 0; k < kNumEsdfStats; k++) c.stats[k] = 0;
+    c.stats[kStatWork] = n;
   }
-  for (int q = i; q < 4000; q += gridDim.x * blockDim.x) c.phase_max[q] = 0ull;
+  for (int q = i; q < kPhaseMaxEntries; q += gridDim.x * blockDim.x) c.phase_max[q] = 0ull;
   if (c.clr_bits)
     for (int q = i; q < kClearBitWords; q += gridDim.x * blockDim.x) c.clr_bits[q] = 0u;
 }
@@ -180,7 +180,7 @@ __device__ __forceinline__ void markFinish(const EsdfCtx& c, MarkLocal& ml) {
     const int nclr = *(volatile int*)c.clr_count;
     const int nupd = *(volatile int*)c.upd_count;
     updatePersistentClearedList(c, nclr);
-    c.stats[1] = nupd, c.stats[2] = nclr;
+    c.stats[kStatWithSites] = nupd, c.stats[kStatToClear] = nclr;
   }
 }
 
@@ -648,8 +648,8 @@ __global__ void __launch_bounds__(kThreads, 5) esdfClearKernel(EsdfCtx c) {
     }
     __syncthreads();
   }
-  if (lane == 0 && ncand_total) atomicAdd((unsigned long long*)&c.stats[3], (unsigned long long)ncand_total);
-  if (tid == 0 && nread_total) atomicAdd((unsigned long long*)&c.stats[13], (unsigned long long)nread_total);
+  if (lane == 0 && ncand_total) atomicAdd((unsigned long long*)&c.stats[kStatClearCandidates], (unsigned long long)ncand_total);
+  if (tid == 0 && nread_total) atomicAdd((unsigned long long*)&c.stats[kStatClearBlocksRead], (unsigned long long)nread_total);
 }
 
 // ---------------------------------------------------------------------------
@@ -1168,8 +1168,8 @@ cudaError_t runEsdfComputeHostLoop(const EsdfCtx& c, int num_sms, cudaStream_t s
     return e;
   if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
   long long h_cl = h_cleared;
-  cudaMemcpyAsync(c.stats + 4, &h_cl, sizeof(long long), cudaMemcpyHostToDevice, stream);
-  cudaMemcpyAsync(c.stats + 5, h_stats, 3 * sizeof(long long), cudaMemcpyHostToDevice, stream);
+  cudaMemcpyAsync(c.stats + kStatCleared, &h_cl, sizeof(long long), cudaMemcpyHostToDevice, stream);
+  cudaMemcpyAsync(c.stats + kStatSwept, h_stats, 3 * sizeof(long long), cudaMemcpyHostToDevice, stream);
   cudaMemcpyAsync(c.ring_id, &ring, sizeof(int), cudaMemcpyHostToDevice, stream);
   return cudaStreamSynchronize(stream);
 }

@@ -183,12 +183,12 @@ __global__ void __maxnreg__(NVB_WAVE_MAXREG) esdfWaveKernel(EsdfCtx c) {
 #undef NVB_TICK
   if (cta == 0 && threadIdx.x == 0) {
     *c.ring_id = ring + 1;
-    c.stats[4] = *(volatile int*)c.cleared_count;
-    c.stats[5] = swept, c.stats[6] = faces, c.stats[7] = rings;
-    c.stats[8] = t_bar, c.stats[9] = t_axis, c.stats[10] = t_sweep, c.stats[11] = n_bar;
+    c.stats[kStatCleared] = *(volatile int*)c.cleared_count;
+    c.stats[kStatSwept] = swept, c.stats[kStatFaces] = faces, c.stats[kStatRings] = rings;
+    c.stats[kStatBarrierNs] = t_bar, c.stats[kStatAxisNs] = t_axis, c.stats[kStatSweepNs] = t_sweep, c.stats[kStatBarriers] = n_bar;
     long long sum_max = 0;
     for (int q = 0; q < n_bar && q < 1000; q++) sum_max += (long long)c.phase_max[q];
-    c.stats[12] = sum_max;  // sum over phases of the slowest CTA's work time
+    c.stats[kStatSlowestCtaWorkNs] = sum_max;
   }
 }
 
@@ -444,12 +444,12 @@ __global__ void __maxnreg__(NVB_WAVE_MAXREG) esdfWaveGesKernel(EsdfCtx c) {
 #undef GES_BARRIER
   if (cta == 0 && tid == 0) {
     *c.ring_id = ring + 1;
-    c.stats[4] = *(volatile int*)c.cleared_count;
-    c.stats[5] = swept, c.stats[6] = faces, c.stats[7] = rings;
-    c.stats[8] = t_bar, c.stats[9] = t_work, c.stats[10] = 0, c.stats[11] = n_bar;
+    c.stats[kStatCleared] = *(volatile int*)c.cleared_count;
+    c.stats[kStatSwept] = swept, c.stats[kStatFaces] = faces, c.stats[kStatRings] = rings;
+    c.stats[kStatBarrierNs] = t_bar, c.stats[kStatWorkNs] = t_work, c.stats[kStatSweepNs] = 0, c.stats[kStatBarriers] = n_bar;
     long long sum_max = 0;
     for (int q = 0; q < n_bar && q < 1000; q++) sum_max += (long long)c.phase_max[q];
-    c.stats[12] = sum_max;
+    c.stats[kStatSlowestCtaWorkNs] = sum_max;
     c.phase_max[3990] = tg, c.phase_max[3991] = te, c.phase_max[3992] = ts, c.phase_max[3993] = ncand, c.phase_max[3994] = nchg;
   }
 }

@@ -112,7 +112,7 @@ constexpr int kXFlagOff = kXFaceCells * 16;           // byte offset of the flag
 constexpr int kXSlotBytes = kXFaceCells * (16 + 4);  // 7 680
 #if NVB_WAVEX_PROF
 constexpr int kXProfWords = 24;  // counters per group, copied to phase_max[kXProfBase ..] (tools/wavex_profile.py)
-constexpr int kXProfBase = 4000 - kXProfWords;
+constexpr int kXProfBase = kPhaseMaxEntries - kXProfWords;
 #endif
 
 struct XTables {
@@ -939,19 +939,19 @@ __global__ void __maxnreg__(NVB_WAVEX_MAXREG) esdfWaveXKernel(EsdfCtx c) {
 #undef X_TIME_BARRIER
 #undef X_DBG
   if (tid == 0 && xs.n_split) {  // (the counts are final: the last ring ended with a CTA barrier)
-    atomicAdd((unsigned long long*)&c.stats[14], (unsigned long long)xs.n_split);
-    atomicAdd((unsigned long long*)&c.stats[15], (unsigned long long)xs.n_rest);
+    atomicAdd((unsigned long long*)&c.stats[kStatSplitCandidates], (unsigned long long)xs.n_split);
+    atomicAdd((unsigned long long*)&c.stats[kStatRestFetches], (unsigned long long)xs.n_rest);
   }
   if (cta == 0 && tid == 0) {
     *c.ring_id = xs.ring + 1;
-    c.stats[4] = *(volatile int*)c.cleared_count;
-    c.stats[5] = xs.swept, c.stats[6] = xs.faces, c.stats[7] = xs.rings;
-    c.stats[10] = xs.n_tail, c.stats[11] = xs.n_bar;
+    c.stats[kStatCleared] = *(volatile int*)c.cleared_count;
+    c.stats[kStatSwept] = xs.swept, c.stats[kStatFaces] = xs.faces, c.stats[kStatRings] = xs.rings;
+    c.stats[kStatTailRings] = xs.n_tail, c.stats[kStatBarriers] = xs.n_bar;
 #if NVB_WAVEX_PROF
-    c.stats[8] = t_bar, c.stats[9] = t_work;
+    c.stats[kStatBarrierNs] = t_bar, c.stats[kStatWorkNs] = t_work;
     long long sum_max = 0;
     for (int q = 0; q < xs.n_bar && q < 1000; q++) sum_max += (long long)c.phase_max[q];
-    c.stats[12] = sum_max;
+    c.stats[kStatSlowestCtaWorkNs] = sum_max;
     for (int q = 0; q < kXProfWords; q++) c.phase_max[kXProfBase + q] = xs.prof[0][q];
 #endif
   }

@@ -454,8 +454,8 @@ struct EsdfCtx {
   int* tracker_dirty;
   int* tracker_todo_count;
   unsigned int* barrier;  // grid barrier counter
-  unsigned long long* phase_max;  // debug: per-phase max-over-CTAs work time (1000 entries)
-  long long* stats;    // 16 counters ([14], [15]: the exchange-slab wavefront's split candidates and rest-of-block fetches)
+  unsigned long long* phase_max;  // debug, kPhaseMaxEntries: per-phase max-over-CTAs work time in the first 1000
+  long long* stats;    // kNumEsdfStats counters, by EsdfStat
   int* error;
   float max_sq;
   float max_esdf_distance_m;
@@ -869,5 +869,32 @@ struct ExportPointsArgs {
 };
 void launchExportCount(const ExportPointsArgs& a, cudaStream_t stream);  // counts + scan + totals
 void launchExportEmit(const ExportPointsArgs& a, cudaStream_t stream);
+
+// nvb_esdf*.cu: the slots of EsdfCtx::stats, the last update's statistics, by what the kernels store in them. Two slots
+// depend on the wavefront driver: slot 9 is CTA 0's axis-pass time in the persistent wavefront and its work time in the
+// gather-replay and exchange-slab ones; slot 10 is the persistent wavefront's sweep time, 0 in the gather-replay one, and
+// the exchange-slab one's single-CTA tail rings.
+enum EsdfStat {
+  kStatWork,                 // the update's work items
+  kStatWithSites,            // blocks with sites
+  kStatToClear,              // to-clear blocks
+  kStatClearCandidates,      // the clear pass's candidate blocks
+  kStatCleared,              // blocks on the cleared list
+  kStatSwept,                // ring members swept
+  kStatFaces,                // face passes
+  kStatRings,
+  kStatBarrierNs,            // CTA 0's wait in grid barriers
+  kStatAxisNs = 9,           // persistent wavefront
+  kStatWorkNs = 9,           // gather-replay and exchange-slab wavefronts
+  kStatSweepNs = 10,         // persistent wavefront
+  kStatTailRings = 10,       // exchange-slab wavefront
+  kStatBarriers,
+  kStatSlowestCtaWorkNs,     // sum over barrier phases of the slowest CTA's work time
+  kStatClearBlocksRead,      // blocks the clear pass read
+  kStatSplitCandidates,      // exchange-slab wavefront: candidates that fetched their own block split ...
+  kStatRestFetches,          // ... and those that then fetched the rest of it
+  kNumEsdfStats
+};
+constexpr int kPhaseMaxEntries = 4000;  // EsdfCtx::phase_max: the wavefront's per-phase debug words
 
 }  // namespace nvb
