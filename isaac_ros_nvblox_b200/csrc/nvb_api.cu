@@ -77,6 +77,8 @@ class DeviceArray {
   // front. An existing allocation is replaced only once both of the mapper's streams are idle, and freed once the fill
   // and the copy are done; the new pointer is published last, so after a failure the array still owns the old one.
   cudaError_t grow(NvbMapper* m, size_t need, size_t count, int fill = kNoFill, bool keep = false);
+  // Doubling growth: room for `need` elements in an allocation of max(need, 2 x size()), unfilled, keeping nothing.
+  cudaError_t growDoubling(NvbMapper* m, size_t need) { return grow(m, need, 2 * n_); }
 
  private:
   T* p_ = nullptr;
@@ -588,6 +590,195 @@ class FrameList {
   int last_n_ = 0;  // the count of the last read
 };
 
+// The mesh layer's arena (nvb_mesh.cu): the segments of every mesh block's vertices, normals, triangle indices and colours
+// in one set of four arrays, and a spare set that a repack moves the live segments into before the two swap. Beside them
+// the kArena* state words, an update's per-entry counts and offsets, and the device copy of an explicit block list.
+class MeshArena {
+ public:
+  // The state words, zeroed; nothing happens once they exist.
+  int create(NvbMapper* m);
+  size_t capacity() const { return live_.t.size(); }  // entries
+  bool hasGeometry() const { return live_.v.get() != nullptr; }
+  // The arrays, the state words, the counts and the offsets into `c`.
+  void fill(MeshCtx* c) const;
+  // The counts and offsets of an update over `list` entries.
+  int reserveList(NvbMapper* m, size_t list);
+  // After an update's count pass on m->stream (one synchronisation): when the update does not fit behind the fill level,
+  // the arena is repacked with room for it, `c` is pointed at the new arrays and the offsets are scanned again.
+  int fitUpdate(NvbMapper* m, MeshCtx* c);
+  // The n block indices `xyz` (host) copied to the device on m->stream and waited for; valid until the next upload.
+  int upload(NvbMapper* m, const int32_t* xyz, int n, const int** dev);
+  // No segments: the state words are zeroed on `st`.
+  cudaError_t empty(cudaStream_t st) { return cudaMemsetAsync(state_.get(), 0, kArenaInts * sizeof(int), st); }
+  // The state words, a blocking copy.
+  cudaError_t readState(int out[kArenaInts]) const {
+    return cudaMemcpy(out, state_.get(), kArenaInts * sizeof(int), cudaMemcpyDeviceToHost);
+  }
+
+ private:
+  // One arena of `entries` entries: 3 floats per entry in v and n, 1 int in t and 4 bytes in c.
+  struct Geometry {
+    DeviceArray<float> v, n;
+    DeviceArray<int> t;
+    DeviceArray<unsigned char> c;
+    cudaError_t grow(NvbMapper* m, size_t entries) {
+      cudaError_t e = v.grow(m, 3 * entries, 3 * entries);
+      if (e == cudaSuccess) e = n.grow(m, 3 * entries, 3 * entries);
+      if (e == cudaSuccess) e = t.grow(m, entries, entries);
+      if (e == cudaSuccess) e = c.grow(m, 4 * entries, 4 * entries);
+      return e;
+    }
+  };
+  // Moves the live segments into the spare arrays with at least `need` free entries behind them, then swaps the two.
+  int repack(NvbMapper* m, long long need, const MeshCtx& c);
+
+  Geometry live_, spare_;
+  DeviceArray<int> state_;
+  DeviceArray<int> counts_, offsets_;
+  DeviceArray<int> xyz_;
+};
+
+// The slots [0, hw) of a layer in (x, y, z) block-index order, sorted on the device: their packIndex keys and the slots,
+// each followed by its sorted copy, and the radix sort's scratch. Free slots sort last.
+class SlotOrder {
+ public:
+  // Sorts the slots of [0, hw) of `layer` on m->stream (two launches); *sorted is the list of hw sorted slots.
+  int sort(NvbMapper* m, const DevLayer& layer, int hw, const int** sorted);
+
+ private:
+  DeviceArray<unsigned long long> keys_;  // 2 x hw
+  DeviceArray<int> slots_;                // 2 x hw
+  DeviceArray<unsigned char> temp_;
+};
+
+// The ground-plane estimator (GroundPlaneEstimator, experimental/ground_plane/): the TSDF slots' order, the zero crossings'
+// counts and totals, the crossings and candidates of the last computation (its optionals), the RANSAC fit's generator
+// states, costs, planes and result word, nvb_ransac_fit_plane's copy of its points, and the last plane.
+class GroundPlaneEstimator {
+ public:
+  // GroundPlaneEstimator::computeGroundPlane on the TSDF layer with m->gp. The state is reset first, and again when the
+  // fit fails or returns an error.
+  int compute(NvbMapper* m, float plane[4], int32_t* found);
+  void lastPlane(float plane[4], int32_t* found) const {
+    *found = found_ ? 1 : 0;
+    if (found_ && plane) std::memcpy(plane, plane_, sizeof(plane_));
+  }
+  // The first min(n, cap) crossings or candidates of the last computation, as xyz triples.
+  int points(NvbMapper* m, int32_t which, float* xyz, int32_t cap, int32_t* n, int32_t* valid) const;
+  // RansacPlaneFitter::fit on n >= 3 points (xyz triples in `memory`).
+  int fitPoints(NvbMapper* m, const float* xyz, int32_t memory, int n, int iterations, float threshold, float plane[4],
+                int32_t* found);
+
+ private:
+  int ransacFit(NvbMapper* m, const float4* pts, int n, int iterations, float threshold, float plane[4], int* found);
+  void reset() {  // GroundPlaneEstimator::resetInternal
+    valid_ = found_ = false;
+    num_crossings_ = num_candidates_ = 0;
+  }
+
+  SlotOrder order_;
+  DeviceArray<int2> counts_;
+  DeviceArray<int> totals_;
+  DeviceArray<float3> crossings_;
+  DeviceArray<float4> candidates_;
+  DeviceArray<float4> fit_points_;
+  DeviceArray<unsigned char> states_;  // curand_init(1234, i, 0) for each state of ransacStateBytes() bytes
+  DeviceArray<float> costs_;           // per iteration
+  DeviceArray<float4> planes_;
+  DeviceArray<float> result_;  // {nx, ny, nz, d, found}
+  bool valid_ = false;         // crossings and candidates of the last computation are kept
+  int num_crossings_ = 0, num_candidates_ = 0;
+  bool found_ = false;
+  float plane_[4] = {0, 0, 0, 0};
+};
+
+// A published output's device buffer and its size in bytes.
+struct DeviceBytes {
+  const void* p;
+  size_t bytes;
+};
+
+// Dynamics detection's outputs of the last frame (DynamicsDetection, dynamics/dynamics_detection.h), sized by pixels: the
+// staged depth, the mask, the filtered mask, the overlay and the points, with the tile counts, the point total and the
+// published rows and cols. Also the scratch of the connected-component filter (MaskPreprocessor).
+class DynamicsOutputs {
+ public:
+  // DynamicsDetection::computeDynamics on m->stream: the caller's depth image of a.rows x a.cols pixels (in `memory`) is
+  // staged, `a` gets the output buffers and the size is published. The other fields of `a` are the caller's.
+  int compute(NvbMapper* m, const float* depth, int32_t memory, DynamicsArgs a);
+  // The filter's labels and sizes for a->drows x a->dcols pixels (at least one), into `a`.
+  int reserveComponents(NvbMapper* m, CcArgs* a);
+  int rows() const { return rows_; }
+  int cols() const { return cols_; }
+  DeviceBytes mask() const { return {mask_.get(), (size_t)rows_ * cols_}; }
+  DeviceBytes overlay() const { return {overlay_.get(), (size_t)rows_ * cols_ * 3}; }
+  DeviceBytes points(int k) const { return {points_.get(), (size_t)k * 3 * sizeof(float)}; }
+  // The number of points of the last detection, read on `st` and waited for; 0 before the first.
+  int pointCount(int* n, cudaStream_t st) const;
+  void deviceBuffers(NvbDynamicsBuffers* out) const {
+    out->depth = depth_.get(), out->mask = mask_.get(), out->cleaned_mask = clean_.get(), out->overlay = overlay_.get();
+    out->points = points_.get(), out->num_points = totals_.get();
+    out->rows = rows_, out->cols = cols_;
+  }
+
+ private:
+  // Grows the per-pixel buffers (nothing is kept: the next call rewrites them). Growing synchronises first, so that no
+  // pending kernel, and no consumer ordered behind this mapper's streams, still reads the old buffers.
+  int reserve(NvbMapper* m, int pixels);
+
+  DeviceArray<float> depth_;
+  DeviceArray<unsigned char> mask_, clean_, overlay_;
+  DeviceArray<float> points_;
+  DeviceArray<int2> counts_;
+  DeviceArray<int> totals_;  // {points, 0}
+  int rows_ = 0, cols_ = 0;
+  DeviceArray<int> cc_labels_, cc_sizes_;
+};
+
+// The image masker's outputs of the last split (ImageMasker, semantics/image_masker.h): background, foreground and overlay,
+// sized by depth pixels, the min-depth scratch, sized by mask pixels, and the published rows, cols and overlay flag.
+class MaskerOutputs {
+ public:
+  // ImageMasker::splitImageOnGPU on m->stream, without a synchronisation: the caller's depth image and mask (sizes in `a`,
+  // in `memory`) are staged, `a` gets the outputs (the overlay only `with_overlay`) and the sizes are published. The other
+  // fields of `a` are the caller's.
+  int split(NvbMapper* m, const float* depth, const uint8_t* mask, int32_t memory, MaskerArgs a, bool with_overlay);
+  // The buffer and byte count that `which` (NvbSplitOutput) names, and its size; an overlay that was not made has none.
+  int output(int32_t which, DeviceBytes* out, int32_t* rows, int32_t* cols) const;
+  void deviceBuffers(NvbSplitBuffers* out) const {
+    out->background = background_.get(), out->foreground = foreground_.get();
+    out->overlay = has_overlay_ ? overlay_.get() : nullptr;
+    out->rows = rows_, out->cols = cols_;
+  }
+
+ private:
+  DeviceArray<float> min_depth_;
+  DeviceArray<float> background_, foreground_;
+  DeviceArray<unsigned char> overlay_;
+  int rows_ = 0, cols_ = 0;
+  bool has_overlay_ = false;
+};
+
+// Unions of block lists: nvb_blocks_union's own list and count (so the last frame's block list survives a union), and
+// the bitset and state words of the device-resident merge of segments, usable on any stream.
+class BlockUnion {
+ public:
+  // The n device block indices `xyz` marked in the view bitset of the AABB grid `g` and compacted into the own list in
+  // linear cell order; the first cap go to `out_xyz`, the count to `out_count` (one synchronisation). Four launches.
+  int merge(NvbMapper* m, const int32_t* xyz, int n, const ViewGrid& g, int32_t* out_xyz, int32_t cap, int32_t* out_count);
+  // The union of `num` segments (launchUnionSegments) on `st`, without a synchronisation. Five launches.
+  int mergeSegments(NvbMapper* m, const int32_t* segments, int32_t num, int32_t stride, int32_t cap_entries,
+                    int32_t* out_xyz, int32_t out_cap, int32_t* out_count, cudaStream_t st);
+  // The error word of the last merge of segments, once the device is idle; 0 before the first.
+  int readError(int32_t* error) const;
+
+ private:
+  DeviceArray<int4> list_;
+  DeviceArray<int> count_;
+  DeviceArray<unsigned int> bits_;
+  DeviceArray<UnionState> state_;  // one
+};
+
 }  // namespace
 
 struct NvbMapper {
@@ -624,26 +815,13 @@ struct NvbMapper {
   DeviceArray<int4> fs_work;
   SlabBounds bounds;
 
-  DeviceArray<int4> union_list;  // nvb_blocks_union's own output list
-  DeviceArray<int> union_list_count;
+  BlockUnion block_union;
 
-  // Mesh layer (nvb_mesh.cu): header slab + one arena for vertices / normals / triangle indices / colours. An arena of
-  // mesh_t.size() entries holds 3 floats per entry in mesh_v and mesh_n and 4 bytes per entry in mesh_c.
+  // Mesh layer (nvb_mesh.cu): the header slab and the arena its headers point into
   LayerSlab mesh;
   // every layer of the mapper, the absent ones included
   std::array<LayerSlab*, 5> layers() { return {&tsdf, &esdf, &freespace, &color, &mesh}; }
-  DeviceArray<float> mesh_v;
-  DeviceArray<float> mesh_n;
-  DeviceArray<int> mesh_t;
-  DeviceArray<unsigned char> mesh_c;
-  DeviceArray<float> mesh_alt_v;  // the spare arena a repack moves the live segments into (then the two swap)
-  DeviceArray<float> mesh_alt_n;
-  DeviceArray<int> mesh_alt_t;
-  DeviceArray<unsigned char> mesh_alt_c;
-  DeviceArray<int> mesh_state;  // kArena* ints
-  DeviceArray<int> mesh_counts;
-  DeviceArray<int> mesh_offsets;
-  DeviceArray<int> mesh_xyz_dev;
+  MeshArena mesh_arena;
   NvbMeshParams mp{1e-4f, 1, 5.0f};
   int cache_last_viewpoint = 1;
   // Mapper::do_depth_preprocessing / depth_preprocessing_num_dilations (mapper_params.h:33-42; mapper.cpp:335-352)
@@ -669,42 +847,11 @@ struct NvbMapper {
   std::set<std::array<int, 3>> cleared_blocks;
   DeviceArray<int4> shape_sel;
   DeviceArray<NvbBoundingShape> shapes_dev;
-  // ground-plane estimator (nvb_ground.cu): parameters, device scratch, the last result (GroundPlaneEstimator's optionals)
+  // ground-plane estimator (nvb_ground.cu)
   NvbGroundPlaneParams gp{};
-  DeviceArray<unsigned long long> gp_keys;  // 2 x gp_counts.size(): packIndex keys of the TSDF slots, then the sorted keys
-  DeviceArray<int> gp_slots;                // 2 x gp_counts.size(): the slots, then the slots in (x, y, z) block-index order
-  DeviceArray<int2> gp_counts;
-  DeviceArray<unsigned char> gp_sort_temp;  // the radix sort's scratch
-  DeviceArray<int> gp_totals;
-  DeviceArray<float3> gp_crossings;
-  DeviceArray<float4> gp_candidates;
-  DeviceArray<float4> gp_fit_points;  // nvb_ransac_fit_plane's own copy of its points
-  DeviceArray<unsigned char> gp_states;  // curand_init(1234, i, 0) for each state of ransacStateBytes() bytes
-  DeviceArray<float> gp_costs;  // per iteration
-  DeviceArray<float4> gp_planes;
-  DeviceArray<float> gp_result;     // {nx, ny, nz, d, found}
-  bool gp_valid = false;            // crossings and candidates of the last computation are kept
-  int gp_num_crossings = 0, gp_num_candidates = 0;
-  bool gp_found = false;
-  float gp_plane[4] = {0, 0, 0, 0};
-  // dynamics detection (nvb_dynamics.cu): the last frame's outputs, sized by pixels; the filter's scratch
-  DeviceArray<float> dyn_depth;    // staged depth
-  DeviceArray<unsigned char> dyn_mask;
-  DeviceArray<unsigned char> dyn_clean;
-  DeviceArray<unsigned char> dyn_overlay;
-  DeviceArray<float> dyn_points;
-  DeviceArray<int2> dyn_counts;
-  DeviceArray<int> dyn_totals;     // {points, 0}
-  int dyn_rows = 0, dyn_cols = 0;
-  DeviceArray<int> cc_labels;
-  DeviceArray<int> cc_sizes;
-  // image masker (nvb_masker.cu): the last split's outputs, sized by pixels, and the min-depth scratch
-  DeviceArray<float> msk_min_depth;      // mask-sized
-  DeviceArray<float> msk_background;
-  DeviceArray<float> msk_foreground;
-  DeviceArray<unsigned char> msk_overlay;
-  int msk_rows = 0, msk_cols = 0;
-  bool msk_has_overlay = false;
+  GroundPlaneEstimator ground;
+  DynamicsOutputs dynamics;  // nvb_dynamics.cu
+  MaskerOutputs masker;      // nvb_masker.cu
   cudaEvent_t dyn_event = nullptr;    // nvb_mapper_wait_for: recorded on this mapper's stream
   // CallerBuffers' staging of host buffers. Unlike the device's default pool, it keeps freed memory across synchronisations,
   // so a call does not map its staging anew each time.
@@ -712,9 +859,6 @@ struct NvbMapper {
   cudaEvent_t query_event = nullptr;  // point queries (nvb_query_*): the hand-over between this mapper and the query's stream
   int keep_last_view = 0;
   LastView last_view;
-  // device-resident merge of block lists (nvb_blocks_union_segments): own scratch, usable on any stream
-  DeviceArray<unsigned int> union_bits;
-  DeviceArray<int> union_state;           // AABB, error flag, words in use
   DeviceArray<int> xyz_upload;
 
   std::unique_ptr<HostWords, PinnedFree> host_words;
@@ -1831,7 +1975,7 @@ static int resetLayers(NvbMapper* m) {
   if ((rc = resetTracker(m))) return rc;
   if ((rc = m->esdf_state.reset(m))) return rc;
   NVB_CUDA(cudaMemsetAsync(m->error_dev, 0, sizeof(int), m->stream));
-  if (m->mesh.exists()) NVB_CUDA(cudaMemsetAsync(m->mesh_state.get(), 0, kArenaInts * sizeof(int), m->stream));
+  if (m->mesh.exists()) NVB_CUDA(m->mesh_arena.empty(m->stream));
   m->bounds.reset(0, 0, 0);
   NVB_CUDA(syncAll(m));
   return NVB_OK;
@@ -2694,28 +2838,128 @@ int32_t nvb_mapper_get_ground_plane_params(const NvbMapper* m, NvbGroundPlanePar
 }  // extern "C"
 
 namespace {
+int SlotOrder::sort(NvbMapper* m, const DevLayer& layer, int hw, const int** sorted) {
+  const size_t n = hw, temp_bytes = groundSortTempBytes(hw);
+  NVB_CUDA(keys_.growDoubling(m, 2 * n));
+  NVB_CUDA(slots_.growDoubling(m, 2 * n));
+  NVB_CUDA(temp_.grow(m, std::max<size_t>(temp_bytes, 1), std::max<size_t>(temp_bytes, 1)));
+  NVB_CUDA(launchGroundSortBlocks(layer, hw, keys_.get(), slots_.get(), temp_.get(), temp_bytes, m->stream));
+  *sorted = slots_.get() + hw;
+  return NVB_OK;
+}
+
+int GroundPlaneEstimator::compute(NvbMapper* m, float plane[4], int32_t* found) {
+  *found = 0;
+  reset();
+  // an occupancy mapper's TsdfLayer is empty: no blocks, no plane
+  if (m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY) return NVB_OK;
+  NVB_CUDA(cudaSetDevice(m->device));
+  // The TSDF layer is written on `stream` only; the ESDF stream does not touch it.
+  int hw = 0;
+  NVB_CUDA(m->tsdf.fillLevel(&hw, m->stream));
+  if (hw == 0) return NVB_OK;  // "tsdf_layer.numBlocks() == 0"
+  NVB_CUDA(counts_.growDoubling(m, hw));
+  NVB_CUDA(totals_.grow(m, 2, 2));
+  // The slots below the high-water mark in (x, y, z) block-index order; free slots sort last and count nothing (a layer
+  // whose slots are all free gives no crossings, hence no plane, like an empty one).
+  GroundExtractArgs a{};
+  int rc;
+  if ((rc = order_.sort(m, m->tsdf.dev(), hw, &a.slots))) return rc;
+  m->launches += 2;
+  a.tsdf = m->tsdf.dev();
+  a.num_blocks = hw;
+  a.counts = counts_.get(), a.totals = totals_.get();
+  a.block_size = m->block_size, a.voxel_size = m->voxel_size;
+  a.min_tsdf_weight = m->gp.min_tsdf_weight;
+  a.min_z = m->gp.ground_points_candidates_min_z_m, a.max_z = m->gp.ground_points_candidates_max_z_m;
+  launchGroundCount(a, m->stream);
+  m->launches += 2;
+  int totals[2];
+  NVB_CUDA(cudaMemcpyAsync(totals, totals_.get(), sizeof(totals), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  // "Maximum number of crossings reached." (tsdf_zero_crossings_extractor.cu:126-131)
+  if (totals[0] >= m->gp.max_crossings) return checkDeviceError(m);
+  NVB_CUDA(crossings_.growDoubling(m, std::max(totals[0], 1)));
+  NVB_CUDA(candidates_.growDoubling(m, std::max(totals[1], 1)));
+  a.crossings = crossings_.get(), a.candidates = candidates_.get();
+  launchGroundEmit(a, m->stream);
+  m->launches++;
+  valid_ = true;
+  num_crossings_ = totals[0], num_candidates_ = totals[1];
+  int f = 0;
+  float pl[4];
+  if ((rc = ransacFit(m, candidates_.get(), totals[1], m->gp.num_ransac_iterations, m->gp.ransac_distance_threshold_m, pl, &f))) {
+    reset();
+    return rc;
+  }
+  if (!f) {
+    reset();
+    return checkDeviceError(m);
+  }
+  found_ = true;
+  std::memcpy(plane_, pl, sizeof(pl));
+  if (plane) std::memcpy(plane, pl, sizeof(pl));
+  *found = 1;
+  return checkDeviceError(m);
+}
+
+int GroundPlaneEstimator::points(NvbMapper* m, int32_t which, float* xyz, int32_t cap, int32_t* n, int32_t* valid) const {
+  *valid = valid_ ? 1 : 0;
+  *n = 0;
+  if (!valid_) return NVB_OK;
+  *n = which == NVB_GROUND_POINTS_CROSSINGS ? num_crossings_ : num_candidates_;
+  const int k = std::min(*n, std::max(cap, 0));
+  if (!xyz || k == 0) return NVB_OK;
+  NVB_CUDA(cudaSetDevice(m->device));
+  if (which == NVB_GROUND_POINTS_CROSSINGS) {
+    NVB_CUDA(cudaMemcpyAsync(xyz, crossings_.get(), (size_t)k * sizeof(float3), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+  } else {
+    std::vector<float4> c((size_t)k);
+    NVB_CUDA(cudaMemcpyAsync(c.data(), candidates_.get(), (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+    for (int i = 0; i < k; i++) xyz[3 * i] = c[i].x, xyz[3 * i + 1] = c[i].y, xyz[3 * i + 2] = c[i].z;
+  }
+  return NVB_OK;
+}
+
+int GroundPlaneEstimator::fitPoints(NvbMapper* m, const float* xyz, int32_t memory, int n, int iterations, float threshold,
+                                    float plane[4], int32_t* found) {
+  NVB_CUDA(cudaSetDevice(m->device));
+  const size_t points_n = n;
+  NVB_CUDA(fit_points_.growDoubling(m, points_n));
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);
+  const float* src;
+  NVB_CUDA(bufs.in(xyz, points_n * 3 * sizeof(float), &src));
+  launchPackPoints(src, n, fit_points_.get(), m->stream);
+  m->launches++;
+  int rc, f = 0;
+  if ((rc = ransacFit(m, fit_points_.get(), n, iterations, threshold, plane, &f))) return rc;
+  *found = f;
+  return checkDeviceError(m);
+}
+
 // RansacPlaneFitter::fit on n points already on the device (float4); the generator states of new iterations are made
 // once and kept.
-int ransacFit(NvbMapper* m, const float4* pts, int n, int iterations, float threshold, float plane[4], int* found) {
+int GroundPlaneEstimator::ransacFit(NvbMapper* m, const float4* pts, int n, int iterations, float threshold, float plane[4],
+                                    int* found) {
   *found = 0;
   if (n < 3) return NVB_OK;  // "We need at least three points to form a plane"
-  const size_t have = m->gp_states.size() / ransacStateBytes();
+  const size_t have = states_.size() / ransacStateBytes();
   if ((size_t)iterations > have) {
     const size_t bytes = (size_t)iterations * ransacStateBytes();
-    NVB_CUDA(m->gp_states.grow(m, bytes, bytes, kNoFill, kKeepContents));
-    launchRansacInit(m->gp_states.get(), (int)have, iterations, m->stream);
+    NVB_CUDA(states_.grow(m, bytes, bytes, kNoFill, kKeepContents));
+    launchRansacInit(states_.get(), (int)have, iterations, m->stream);
     m->launches++;
     NVB_CUDA(cudaStreamSynchronize(m->stream));
   }
-  const size_t it = iterations;
-  NVB_CUDA(m->gp_costs.grow(m, it, std::max(it, 2 * m->gp_costs.size())));
-  NVB_CUDA(m->gp_planes.grow(m, it, std::max(it, 2 * m->gp_planes.size())));
-  NVB_CUDA(m->gp_result.grow(m, 5, 5));
-  launchRansacFit(pts, n, iterations, threshold, m->gp_states.get(), m->gp_costs.get(), m->gp_planes.get(), m->gp_result.get(),
-                  m->stream);
+  NVB_CUDA(costs_.growDoubling(m, iterations));
+  NVB_CUDA(planes_.growDoubling(m, iterations));
+  NVB_CUDA(result_.grow(m, 5, 5));
+  launchRansacFit(pts, n, iterations, threshold, states_.get(), costs_.get(), planes_.get(), result_.get(), m->stream);
   m->launches += 2;
   float out[5];
-  NVB_CUDA(cudaMemcpyAsync(out, m->gp_result.get(), sizeof(out), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(out, result_.get(), sizeof(out), cudaMemcpyDeviceToHost, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   int f = 0;
   std::memcpy(&f, &out[4], sizeof(int));
@@ -2725,83 +2969,18 @@ int ransacFit(NvbMapper* m, const float4* pts, int n, int iterations, float thre
   }
   return NVB_OK;
 }
-
-void groundReset(NvbMapper* m) {  // GroundPlaneEstimator::resetInternal
-  m->gp_valid = false, m->gp_found = false;
-  m->gp_num_crossings = m->gp_num_candidates = 0;
-}
 }  // namespace
 
 extern "C" {
 
 int32_t nvb_mapper_compute_ground_plane(NvbMapper* m, float plane[4], int32_t* found) {
   if (!m || !found) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  *found = 0;
-  groundReset(m);
-  // an occupancy mapper's TsdfLayer is empty: no blocks, no plane
-  if (m->projective_layer_type == NVB_PROJECTIVE_OCCUPANCY) return NVB_OK;
-  NVB_CUDA(cudaSetDevice(m->device));
-  // The TSDF layer is written on `stream` only; the ESDF stream does not touch it.
-  int hw = 0;
-  NVB_CUDA(m->tsdf.fillLevel(&hw, m->stream));
-  if (hw == 0) return NVB_OK;  // "tsdf_layer.numBlocks() == 0"
-  // The slots below the high-water mark in (x, y, z) block-index order, sorted on the device; free slots sort last and
-  // count nothing (a layer whose slots are all free gives no crossings, hence no plane, like an empty one).
-  const size_t blocks = hw;
-  const size_t cap = std::max(blocks, 2 * m->gp_counts.size());
-  NVB_CUDA(m->gp_keys.grow(m, 2 * blocks, 2 * cap));
-  NVB_CUDA(m->gp_slots.grow(m, 2 * blocks, 2 * cap));
-  NVB_CUDA(m->gp_counts.grow(m, blocks, cap));
-  const size_t temp_bytes = groundSortTempBytes(hw);
-  NVB_CUDA(m->gp_sort_temp.grow(m, temp_bytes, temp_bytes));
-  int rc = NVB_OK;
-  NVB_CUDA(m->gp_totals.grow(m, 2, 2));
-  NVB_CUDA(launchGroundSortBlocks(m->tsdf.dev(), hw, m->gp_keys.get(), m->gp_slots.get(), m->gp_sort_temp.get(), m->gp_sort_temp.size(),
-                                  m->stream));
-  m->launches += 2;
-  GroundExtractArgs a{};
-  a.tsdf = m->tsdf.dev();
-  a.slots = m->gp_slots.get() + hw, a.num_blocks = hw;
-  a.counts = m->gp_counts.get(), a.totals = m->gp_totals.get();
-  a.block_size = m->block_size, a.voxel_size = m->voxel_size;
-  a.min_tsdf_weight = m->gp.min_tsdf_weight;
-  a.min_z = m->gp.ground_points_candidates_min_z_m, a.max_z = m->gp.ground_points_candidates_max_z_m;
-  launchGroundCount(a, m->stream);
-  m->launches += 2;
-  int totals[2];
-  NVB_CUDA(cudaMemcpyAsync(totals, m->gp_totals.get(), sizeof(totals), cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
-  // "Maximum number of crossings reached." (tsdf_zero_crossings_extractor.cu:126-131)
-  if (totals[0] >= m->gp.max_crossings) return checkDeviceError(m);
-  const size_t crossings = std::max(totals[0], 1), candidates = std::max(totals[1], 1);
-  NVB_CUDA(m->gp_crossings.grow(m, crossings, std::max(crossings, 2 * m->gp_crossings.size())));
-  NVB_CUDA(m->gp_candidates.grow(m, candidates, std::max(candidates, 2 * m->gp_candidates.size())));
-  a.crossings = m->gp_crossings.get(), a.candidates = m->gp_candidates.get();
-  launchGroundEmit(a, m->stream);
-  m->launches++;
-  m->gp_valid = true;
-  m->gp_num_crossings = totals[0], m->gp_num_candidates = totals[1];
-  int f = 0;
-  float pl[4];
-  if ((rc = ransacFit(m, m->gp_candidates.get(), totals[1], m->gp.num_ransac_iterations, m->gp.ransac_distance_threshold_m, pl, &f))) {
-    groundReset(m);
-    return rc;
-  }
-  if (!f) {
-    groundReset(m);
-    return checkDeviceError(m);
-  }
-  m->gp_found = true;
-  std::memcpy(m->gp_plane, pl, sizeof(pl));
-  if (plane) std::memcpy(plane, pl, sizeof(pl));
-  *found = 1;
-  return checkDeviceError(m);
+  return m->ground.compute(m, plane, found);
 }
 
 int32_t nvb_mapper_ground_plane(NvbMapper* m, float plane[4], int32_t* found) {
   if (!m || !found) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  *found = m->gp_found ? 1 : 0;
-  if (m->gp_found && plane) std::memcpy(plane, m->gp_plane, sizeof(m->gp_plane));
+  m->ground.lastPlane(plane, found);
   return NVB_OK;
 }
 
@@ -2809,46 +2988,18 @@ int32_t nvb_mapper_ground_plane_points(NvbMapper* m, int32_t which, float* xyz, 
   if (!m || !n || !valid) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (which != NVB_GROUND_POINTS_CROSSINGS && which != NVB_GROUND_POINTS_CANDIDATES)
     return fail(NVB_ERR_INVALID_ARGUMENT, "which must be NVB_GROUND_POINTS_CROSSINGS or NVB_GROUND_POINTS_CANDIDATES");
-  *valid = m->gp_valid ? 1 : 0;
-  *n = 0;
-  if (!m->gp_valid) return NVB_OK;
-  *n = which == NVB_GROUND_POINTS_CROSSINGS ? m->gp_num_crossings : m->gp_num_candidates;
-  const int k = std::min(*n, std::max(cap, 0));
-  if (!xyz || k == 0) return NVB_OK;
-  NVB_CUDA(cudaSetDevice(m->device));
-  if (which == NVB_GROUND_POINTS_CROSSINGS) {
-    NVB_CUDA(cudaMemcpyAsync(xyz, m->gp_crossings.get(), (size_t)k * sizeof(float3), cudaMemcpyDeviceToHost, m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-  } else {
-    std::vector<float4> c((size_t)k);
-    NVB_CUDA(cudaMemcpyAsync(c.data(), m->gp_candidates.get(), (size_t)k * sizeof(float4), cudaMemcpyDeviceToHost, m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    for (int i = 0; i < k; i++) xyz[3 * i] = c[i].x, xyz[3 * i + 1] = c[i].y, xyz[3 * i + 2] = c[i].z;
-  }
-  return NVB_OK;
+  return m->ground.points(m, which, xyz, cap, n, valid);
 }
 
 int32_t nvb_ransac_fit_plane(NvbMapper* m, const float* points, int32_t memory, int32_t n, int32_t num_ransac_iterations,
                              float ransac_distance_threshold_m, float plane[4], int32_t* found) {
   if (!m || !plane || !found) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (n < 0 || (n > 0 && !points)) return fail(NVB_ERR_INVALID_ARGUMENT, "bad point list");
-  int rc;
-  if ((rc = checkMemoryKind(memory))) return rc;
+  if (int rc = checkMemoryKind(memory)) return rc;
   if (num_ransac_iterations < 1) return fail(NVB_ERR_INVALID_ARGUMENT, "num_ransac_iterations must be >= 1");
   *found = 0;
   if (n < 3) return NVB_OK;
-  NVB_CUDA(cudaSetDevice(m->device));
-  const size_t points_n = n;
-  NVB_CUDA(m->gp_fit_points.grow(m, points_n, std::max(points_n, 2 * m->gp_fit_points.size())));
-  CallerBuffers bufs(memory, m->stream, m->stage_pool);
-  const float* src;
-  NVB_CUDA(bufs.in(points, points_n * 3 * sizeof(float), &src));
-  launchPackPoints(src, n, m->gp_fit_points.get(), m->stream);
-  m->launches++;
-  int f = 0;
-  if ((rc = ransacFit(m, m->gp_fit_points.get(), n, num_ransac_iterations, ransac_distance_threshold_m, plane, &f))) return rc;
-  *found = f;
-  return checkDeviceError(m);
+  return m->ground.fitPoints(m, points, memory, n, num_ransac_iterations, ransac_distance_threshold_m, plane, found);
 }
 
 }  // extern "C"
@@ -2856,29 +3007,88 @@ int32_t nvb_ransac_fit_plane(NvbMapper* m, const float* points, int32_t memory, 
 namespace {
 constexpr long long kMaxDynamicsPixels = 1ll << 28;  // 3-byte overlay and 12-byte points per pixel stay below 2^32
 
-// Grows the detector's per-pixel buffers (nothing is kept: the next call rewrites them). Growing synchronises first, so
-// that no pending kernel, and no consumer ordered behind this mapper's streams, still reads the old buffers.
-int ensureDynamicsBuffers(NvbMapper* m, int pixels) {
+int DynamicsOutputs::reserve(NvbMapper* m, int pixels) {
   const size_t n = pixels;
-  NVB_CUDA(m->dyn_depth.grow(m, n, n));
-  NVB_CUDA(m->dyn_mask.grow(m, n, n));
-  NVB_CUDA(m->dyn_clean.grow(m, n, n));
-  NVB_CUDA(m->dyn_overlay.grow(m, 3 * n, 3 * n));
-  NVB_CUDA(m->dyn_points.grow(m, 3 * n, 3 * n));
+  NVB_CUDA(depth_.grow(m, n, n));
+  NVB_CUDA(mask_.grow(m, n, n));
+  NVB_CUDA(clean_.grow(m, n, n));
+  NVB_CUDA(overlay_.grow(m, 3 * n, 3 * n));
+  NVB_CUDA(points_.grow(m, 3 * n, 3 * n));
   const size_t tiles = dynamicsNumTiles(pixels);
-  NVB_CUDA(m->dyn_counts.grow(m, tiles, tiles));
-  NVB_CUDA(m->dyn_totals.grow(m, 2, 2, 0));
+  NVB_CUDA(counts_.grow(m, tiles, tiles));
+  NVB_CUDA(totals_.grow(m, 2, 2, 0));
   return NVB_OK;
 }
 
-// Copies `bytes` of one of the mapper's published outputs to the caller's `out` (in `memory`) on the mapper's stream; a
-// host copy waits for it.
-int copyToCaller(NvbMapper* m, void* out, const void* src, size_t bytes, int32_t memory) {
-  if (!out || bytes == 0 || !src) return NVB_OK;
+int DynamicsOutputs::compute(NvbMapper* m, const float* depth, int32_t memory, DynamicsArgs a) {
+  const int pixels = a.rows * a.cols;
+  if (int rc = reserve(m, pixels)) return rc;
+  // The freespace layer is written on `stream` only (nvb_mapper_update_freespace); the detection follows it there.
+  NVB_CUDA(cudaMemcpyAsync(depth_.get(), depth, (size_t)pixels * sizeof(float),
+                           memory == NVB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, m->stream));
+  a.depth = depth_.get();
+  a.mask = mask_.get(), a.overlay = overlay_.get(), a.counts = counts_.get(), a.points = points_.get();
+  launchDynamicsDetect(a, totals_.get(), m->stream);
+  m->launches += 3;
+  rows_ = a.rows, cols_ = a.cols;
+  return NVB_OK;
+}
+
+int DynamicsOutputs::reserveComponents(NvbMapper* m, CcArgs* a) {
+  const size_t down = std::max(a->drows * a->dcols, 1);
+  NVB_CUDA(cc_labels_.growDoubling(m, down));
+  NVB_CUDA(cc_sizes_.growDoubling(m, down));
+  a->labels = cc_labels_.get(), a->sizes = cc_sizes_.get();
+  return NVB_OK;
+}
+
+int DynamicsOutputs::pointCount(int* n, cudaStream_t st) const {
+  *n = 0;
+  if (!totals_.get()) return NVB_OK;  // never computed
+  NVB_CUDA(cudaMemcpyAsync(n, totals_.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
+  NVB_CUDA(cudaStreamSynchronize(st));
+  return NVB_OK;
+}
+
+int MaskerOutputs::split(NvbMapper* m, const float* depth, const uint8_t* mask, int32_t memory, MaskerArgs a,
+                         bool with_overlay) {
+  const size_t n = (size_t)a.rows * a.cols, mn = (size_t)a.mrows * a.mcols;
+  // Growing synchronises the mapper's streams first, so no pending split still uses the old buffers.
+  NVB_CUDA(background_.grow(m, n, n));
+  NVB_CUDA(foreground_.grow(m, n, n));
+  if (with_overlay) NVB_CUDA(overlay_.grow(m, 3 * n, 3 * n));
+  NVB_CUDA(min_depth_.grow(m, mn, mn));
+  CallerBuffers bufs(memory, m->stream, m->stage_pool);  // released behind the split: the call does not synchronise
+  NVB_CUDA(bufs.in(depth, n * sizeof(float), &a.depth));
+  NVB_CUDA(bufs.in(mask, mn, &a.mask));
+  a.min_depth = min_depth_.get();
+  a.unmasked = background_.get(), a.masked = foreground_.get();
+  a.overlay = with_overlay ? overlay_.get() : nullptr;
+  launchSplitDepth(a, m->num_sms, m->stream);
+  NVB_CUDA(cudaGetLastError());
+  m->launches += 3;
+  rows_ = a.rows, cols_ = a.cols, has_overlay_ = with_overlay;
+  return NVB_OK;
+}
+
+int MaskerOutputs::output(int32_t which, DeviceBytes* out, int32_t* rows, int32_t* cols) const {
+  const size_t n = (size_t)rows_ * cols_;
+  if (which == NVB_SPLIT_BACKGROUND) *out = {background_.get(), n * sizeof(float)};
+  else if (which == NVB_SPLIT_FOREGROUND) *out = {foreground_.get(), n * sizeof(float)};
+  else if (which == NVB_SPLIT_OVERLAY) *out = {overlay_.get(), has_overlay_ ? 3 * n : 0};
+  else return fail(NVB_ERR_INVALID_ARGUMENT, "bad split output");
+  *rows = out->bytes ? rows_ : 0, *cols = out->bytes ? cols_ : 0;
+  return NVB_OK;
+}
+
+// Copies one of the mapper's published outputs to the caller's `out` (in `memory`) on the mapper's stream; a host copy
+// waits for it.
+int copyToCaller(NvbMapper* m, void* out, DeviceBytes src, int32_t memory) {
+  if (!out || src.bytes == 0 || !src.p) return NVB_OK;
   CallerBuffers bufs(memory, m->stream, m->stage_pool);
   void* dev;
-  NVB_CUDA(bufs.out(out, bytes, &dev));
-  NVB_CUDA(cudaMemcpyAsync(dev, src, bytes, cudaMemcpyDeviceToDevice, m->stream));
+  NVB_CUDA(bufs.out(out, src.bytes, &dev));
+  NVB_CUDA(cudaMemcpyAsync(dev, src.p, src.bytes, cudaMemcpyDeviceToDevice, m->stream));
   NVB_CUDA(bufs.finish());
   return NVB_OK;
 }
@@ -2894,23 +3104,14 @@ int32_t nvb_mapper_compute_dynamics(NvbMapper* m, const float* depth, int32_t me
     return fail(NVB_ERR_INVALID_ARGUMENT, "the mapper has no freespace layer");
   if ((long long)rows * cols > kMaxDynamicsPixels) return fail(NVB_ERR_INVALID_ARGUMENT, "depth image too large");
   NVB_CUDA(cudaSetDevice(m->device));
-  const int pixels = rows * cols;
-  if ((rc = ensureDynamicsBuffers(m, pixels))) return rc;
-  // The freespace layer is written on `stream` only (nvb_mapper_update_freespace); the detection follows it there.
-  NVB_CUDA(cudaMemcpyAsync(m->dyn_depth.get(), depth, (size_t)pixels * sizeof(float),
-                           memory == NVB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, m->stream));
   DynamicsArgs a{};
-  a.depth = m->dyn_depth.get(), a.rows = rows, a.cols = cols;
+  a.rows = rows, a.cols = cols;
   a.T_L_C = rigidFromColMajor(T_L_C);
   a.cam = *cam;
   a.fs = m->freespace.dev();
   a.block_size = m->block_size;
   a.voxel_size_inv = (float)(1.0 / (double)(m->block_size * (1.0f / kVps)));  // 1.0 / blockSizeToVoxelSize(block_size)
-  a.mask = m->dyn_mask.get(), a.overlay = m->dyn_overlay.get(), a.counts = m->dyn_counts.get(), a.points = m->dyn_points.get();
-  launchDynamicsDetect(a, m->dyn_totals.get(), m->stream);
-  m->launches += 3;
-  m->dyn_rows = rows, m->dyn_cols = cols;
-  return NVB_OK;
+  return m->dynamics.compute(m, depth, memory, a);
 }
 
 int32_t nvb_mapper_remove_small_components(NvbMapper* m, const uint8_t* mask_in, uint8_t* mask_out, int32_t memory,
@@ -2934,10 +3135,7 @@ int32_t nvb_mapper_remove_small_components(NvbMapper* m, const uint8_t* mask_in,
   CcArgs a{};
   a.rows = rows, a.cols = cols, a.drows = rows / 2, a.dcols = cols / 2;
   a.min_size = threshold / 4;  // size_threshold / (kDownScaleFactor * kDownScaleFactor)
-  const size_t down = std::max(a.drows * a.dcols, 1);
-  NVB_CUDA(m->cc_labels.grow(m, down, std::max(down, 2 * m->cc_labels.size())));
-  NVB_CUDA(m->cc_sizes.grow(m, down, std::max(down, 2 * m->cc_sizes.size())));
-  a.labels = m->cc_labels.get(), a.sizes = m->cc_sizes.get();
+  if (int rc = m->dynamics.reserveComponents(m, &a)) return rc;
   CallerBuffers bufs(memory, m->stream, m->stage_pool);
   NVB_CUDA(bufs.in(mask_in, (size_t)pixels, &a.in));
   NVB_CUDA(bufs.out(mask_out, (size_t)pixels, &a.out));
@@ -2950,38 +3148,34 @@ int32_t nvb_mapper_remove_small_components(NvbMapper* m, const uint8_t* mask_in,
 int32_t nvb_mapper_dynamic_mask(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols) {
   if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (int rc = checkMemoryKind(memory)) return rc;
-  *rows = m->dyn_rows, *cols = m->dyn_cols;
+  *rows = m->dynamics.rows(), *cols = m->dynamics.cols();
   NVB_CUDA(cudaSetDevice(m->device));
-  return copyToCaller(m, out, m->dyn_mask.get(), (size_t)m->dyn_rows * m->dyn_cols, memory);
+  return copyToCaller(m, out, m->dynamics.mask(), memory);
 }
 
 int32_t nvb_mapper_dynamic_overlay(NvbMapper* m, uint8_t* out, int32_t memory, int32_t* rows, int32_t* cols) {
   if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (int rc = checkMemoryKind(memory)) return rc;
-  *rows = m->dyn_rows, *cols = m->dyn_cols;
+  *rows = m->dynamics.rows(), *cols = m->dynamics.cols();
   NVB_CUDA(cudaSetDevice(m->device));
-  return copyToCaller(m, out, m->dyn_overlay.get(), (size_t)m->dyn_rows * m->dyn_cols * 3, memory);
+  return copyToCaller(m, out, m->dynamics.overlay(), memory);
 }
 
 int32_t nvb_mapper_dynamic_points(NvbMapper* m, float* xyz, int32_t memory, int32_t cap, int32_t* out_count) {
   if (!m || !out_count) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (int rc = checkMemoryKind(memory)) return rc;
   *out_count = 0;
-  if (!m->dyn_totals.get()) return NVB_OK;  // never computed
   NVB_CUDA(cudaSetDevice(m->device));
   int n = 0;
-  NVB_CUDA(cudaMemcpyAsync(&n, m->dyn_totals.get(), sizeof(int), cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  if (int rc = m->dynamics.pointCount(&n, m->stream)) return rc;
   *out_count = n;
   const int k = std::min(n, std::max(cap, 0));
-  return copyToCaller(m, xyz, m->dyn_points.get(), (size_t)k * 3 * sizeof(float), memory);
+  return copyToCaller(m, xyz, m->dynamics.points(k), memory);
 }
 
 int32_t nvb_mapper_dynamics_device_buffers(NvbMapper* m, NvbDynamicsBuffers* out) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  out->depth = m->dyn_depth.get(), out->mask = m->dyn_mask.get(), out->cleaned_mask = m->dyn_clean.get(), out->overlay = m->dyn_overlay.get();
-  out->points = m->dyn_points.get(), out->num_points = m->dyn_totals.get();
-  out->rows = m->dyn_rows, out->cols = m->dyn_cols;
+  m->dynamics.deviceBuffers(out);
   return NVB_OK;
 }
 
@@ -3018,52 +3212,28 @@ int32_t nvb_mapper_split_depth_image(NvbMapper* m, const float* depth, int32_t d
   if ((long long)depth_rows * depth_cols > kMaxDynamicsPixels || (long long)mask_rows * mask_cols > kMaxDynamicsPixels)
     return fail(NVB_ERR_INVALID_ARGUMENT, "image too large");
   NVB_CUDA(cudaSetDevice(m->device));
-  const size_t n = (size_t)depth_rows * depth_cols, mn = (size_t)mask_rows * mask_cols;
-  // Growing synchronises the mapper's streams first, so no pending split still uses the old buffers.
-  NVB_CUDA(m->msk_background.grow(m, n, n));
-  NVB_CUDA(m->msk_foreground.grow(m, n, n));
-  if (with_overlay) NVB_CUDA(m->msk_overlay.grow(m, 3 * n, 3 * n));
-  NVB_CUDA(m->msk_min_depth.grow(m, mn, mn));
   MaskerArgs a{};
-  CallerBuffers bufs(memory, m->stream, m->stage_pool);  // released behind the split: the call does not synchronise
-  NVB_CUDA(bufs.in(depth, n * sizeof(float), &a.depth));
-  NVB_CUDA(bufs.in(mask, mn, &a.mask));
   a.rows = depth_rows, a.cols = depth_cols, a.mrows = mask_rows, a.mcols = mask_cols;
   a.T_CM_CD = rigidFromColMajor(T_CM_CD);
   a.depth_cam = *depth_cam, a.mask_cam = *mask_cam;
   a.occlusion_threshold_m = params->occlusion_threshold_m;
   a.masked_invalid = params->depth_masked_image_invalid_pixel;
   a.unmasked_invalid = params->depth_unmasked_image_invalid_pixel;
-  a.min_depth = m->msk_min_depth.get();
-  a.unmasked = m->msk_background.get(), a.masked = m->msk_foreground.get();
-  a.overlay = with_overlay ? m->msk_overlay.get() : nullptr;
-  launchSplitDepth(a, m->num_sms, m->stream);
-  NVB_CUDA(cudaGetLastError());
-  m->launches += 3;
-  m->msk_rows = depth_rows, m->msk_cols = depth_cols, m->msk_has_overlay = with_overlay != 0;
-  return NVB_OK;
+  return m->masker.split(m, depth, mask, memory, a, with_overlay != 0);
 }
 
 int32_t nvb_mapper_split_output(NvbMapper* m, int32_t which, void* out, int32_t memory, int32_t* rows, int32_t* cols) {
   if (!m || !rows || !cols) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   if (int rc = checkMemoryKind(memory)) return rc;
-  const size_t n = (size_t)m->msk_rows * m->msk_cols;
-  const void* src;
-  size_t bytes;
-  if (which == NVB_SPLIT_BACKGROUND) src = m->msk_background.get(), bytes = n * sizeof(float);
-  else if (which == NVB_SPLIT_FOREGROUND) src = m->msk_foreground.get(), bytes = n * sizeof(float);
-  else if (which == NVB_SPLIT_OVERLAY) src = m->msk_overlay.get(), bytes = m->msk_has_overlay ? 3 * n : 0;
-  else return fail(NVB_ERR_INVALID_ARGUMENT, "bad split output");
-  *rows = bytes ? m->msk_rows : 0, *cols = bytes ? m->msk_cols : 0;
+  DeviceBytes src;
+  if (int rc = m->masker.output(which, &src, rows, cols)) return rc;
   NVB_CUDA(cudaSetDevice(m->device));
-  return copyToCaller(m, out, src, bytes, memory);
+  return copyToCaller(m, out, src, memory);
 }
 
 int32_t nvb_mapper_split_device_buffers(NvbMapper* m, NvbSplitBuffers* out) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  out->background = m->msk_background.get(), out->foreground = m->msk_foreground.get();
-  out->overlay = m->msk_has_overlay ? m->msk_overlay.get() : nullptr;
-  out->rows = m->msk_rows, out->cols = m->msk_cols;
+  m->masker.deviceBuffers(out);
   return NVB_OK;
 }
 
@@ -3220,6 +3390,53 @@ int32_t nvb_mapper_last_frame_blocks(NvbMapper* m, int32_t* out_xyz_host, int32_
   return m->frame_list.read(m, out_xyz_host, cap, out_count);
 }
 
+}  // extern "C"
+
+namespace {
+int BlockUnion::merge(NvbMapper* m, const int32_t* xyz, int n, const ViewGrid& g, int32_t* out_xyz, int32_t cap,
+                      int32_t* out_count) {
+  int rc;
+  if ((rc = m->view.reserve(m, g))) return rc;
+  const int need = std::min(n, g.linear_size);
+  NVB_CUDA(list_.grow(m, need, (size_t)std::min<long long>((long long)(1.5 * need) + 64, 0x7fffffff)));
+  NVB_CUDA(count_.grow(m, 1, 1));
+  launchMarkList(xyz, n, g, m->view.bits(), m->stream);
+  m->view.compact(g, list_.get(), count_.get(), false, m->tsdf.dev(), TrackerLists{}, m->error_dev, true, m->stream);
+  if (out_xyz && cap > 0) launchUnpackList(list_.get(), count_.get(), out_xyz, cap, m->stream);
+  m->launches += 4;
+  if (out_count) {
+    NVB_CUDA(cudaMemcpyAsync(&m->host_words->union_count, count_.get(), sizeof(int), cudaMemcpyDeviceToHost, m->stream));
+    NVB_CUDA(cudaStreamSynchronize(m->stream));
+    *out_count = m->host_words->union_count;
+  }
+  return NVB_OK;
+}
+
+int BlockUnion::mergeSegments(NvbMapper* m, const int32_t* segments, int32_t num, int32_t stride, int32_t cap_entries,
+                              int32_t* out_xyz, int32_t out_cap, int32_t* out_count, cudaStream_t st) {
+  // 2^28 cells = 32 MiB of bits: a union AABB of e.g. 1024 x 1024 x 256 blocks (410 m x 410 m x 102 m at 5 cm voxels)
+  constexpr long long kUnionCells = 1ll << 28;
+  NVB_CUDA(bits_.grow(m, kUnionCells / 32, kUnionCells / 32, 0));
+  NVB_CUDA(state_.grow(m, 1, 1, 0));
+  launchUnionSegments(segments, num, stride, cap_entries, reinterpret_cast<int*>(state_.get()), bits_.get(), kUnionCells, out_xyz,
+                      out_cap, out_count, st);
+  m->launches += 5;
+  return NVB_OK;
+}
+
+int BlockUnion::readError(int32_t* error) const {
+  *error = 0;
+  if (!state_.get()) return NVB_OK;
+  NVB_CUDA(cudaDeviceSynchronize());
+  UnionState s;
+  NVB_CUDA(cudaMemcpy(&s, state_.get(), sizeof(s), cudaMemcpyDeviceToHost));
+  *error = s.error;
+  return NVB_OK;
+}
+}  // namespace
+
+extern "C" {
+
 int32_t nvb_blocks_union(NvbMapper* m, const int32_t* xyz_dev, int32_t n, const int32_t aabb_min[3],
                          const int32_t aabb_max[3], int32_t* out_xyz_dev, int32_t cap, int32_t* out_count_host) {
   if (!m || !aabb_min || !aabb_max || (n > 0 && !xyz_dev)) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
@@ -3236,24 +3453,7 @@ int32_t nvb_blocks_union(NvbMapper* m, const int32_t* xyz_dev, int32_t n, const 
   g.size = make_int3((int)sx, (int)sy, (int)sz);
   g.linear_size = (int)(sx * sy * sz);
   g.num_words = (g.linear_size + 31) / 32;
-  int rc;
-  if ((rc = m->view.reserve(m, g))) return rc;
-  const int need = std::min(n, g.linear_size);
-  NVB_CUDA(m->union_list.grow(m, need, (size_t)std::min<long long>((long long)(1.5 * need) + 64, 0x7fffffff)));
-  NVB_CUDA(m->union_list_count.grow(m, 1, 1));
-  launchMarkList(xyz_dev, n, g, m->view.bits(), m->stream);
-  // the union has its own list: the last frame's block list (nvb_mapper_last_frame_blocks) survives a merge
-  m->view.compact(g, m->union_list.get(), m->union_list_count.get(), false, m->tsdf.dev(), TrackerLists{}, m->error_dev, true,
-                  m->stream);
-  if (out_xyz_dev && cap > 0) launchUnpackList(m->union_list.get(), m->union_list_count.get(), out_xyz_dev, cap, m->stream);
-  m->launches += 4;
-  if (out_count_host) {
-    NVB_CUDA(cudaMemcpyAsync(&m->host_words->union_count, m->union_list_count.get(), sizeof(int), cudaMemcpyDeviceToHost,
-                             m->stream));
-    NVB_CUDA(cudaStreamSynchronize(m->stream));
-    *out_count_host = m->host_words->union_count;
-  }
-  return NVB_OK;
+  return m->block_union.merge(m, xyz_dev, n, g, out_xyz_dev, cap, out_count_host);
 }
 
 int32_t nvb_mapper_append_frame_blocks(NvbMapper* m, int32_t* segment_dev, int32_t cap_entries) {
@@ -3271,27 +3471,14 @@ int32_t nvb_blocks_union_segments(NvbMapper* m, const int32_t* segments_dev, int
       segment_stride_ints < 1 + 3 * cap_entries)
     return fail(NVB_ERR_INVALID_ARGUMENT, "bad argument");
   NVB_CUDA(cudaSetDevice(m->device));
-  // 2^28 cells = 32 MiB of bits: a union AABB of e.g. 1024 x 1024 x 256 blocks (410 m x 410 m x 102 m at 5 cm voxels)
-  constexpr long long kUnionCells = 1ll << 28;
-  NVB_CUDA(m->union_bits.grow(m, kUnionCells / 32, kUnionCells / 32, 0));
-  NVB_CUDA(m->union_state.grow(m, 8, 8, 0));
-  launchUnionSegments(segments_dev, num_segments, segment_stride_ints, cap_entries, m->union_state.get(), m->union_bits.get(),
-                      kUnionCells, out_xyz_dev, out_cap, out_count_dev, stream ? (cudaStream_t)stream : m->stream);
-  m->launches += 5;
-  return NVB_OK;
+  return m->block_union.mergeSegments(m, segments_dev, num_segments, segment_stride_ints, cap_entries, out_xyz_dev, out_cap,
+                                      out_count_dev, stream ? (cudaStream_t)stream : m->stream);
 }
 
 int32_t nvb_blocks_union_status(NvbMapper* m, int32_t* out_error) {
   if (!m || !out_error) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
   NVB_CUDA(cudaSetDevice(m->device));
-  *out_error = 0;
-  if (m->union_state.get()) {
-    NVB_CUDA(cudaDeviceSynchronize());
-    int st[8];
-    NVB_CUDA(cudaMemcpy(st, m->union_state.get(), sizeof(st), cudaMemcpyDeviceToHost));
-    *out_error = st[6];
-  }
-  return NVB_OK;
+  return m->block_union.readError(out_error);
 }
 
 int32_t nvb_mapper_set_cache_last_viewpoint(NvbMapper* m, int32_t enable) {
@@ -3619,19 +3806,14 @@ int32_t nvb_layer_export_points(NvbMapper* m, int32_t layer, int32_t memory, flo
   *n = 0;
   if (hw == 0) return NVB_OK;
   if ((long long)hw * kVpb > 0x7fffffffll) return fail(NVB_ERR_CAPACITY, "more than 2^31 voxels to export");
-  DeviceArray<unsigned long long> keys;
-  DeviceArray<int> slots, totals;
+  SlotOrder order;
+  DeviceArray<int> totals;
   DeviceArray<int2> counts;
-  DeviceArray<unsigned char> temp;
-  const size_t temp_bytes = groundSortTempBytes(hw);
-  NVB_CUDA(keys.grow(m, 2 * (size_t)hw, 2 * (size_t)hw));
-  NVB_CUDA(slots.grow(m, 2 * (size_t)hw, 2 * (size_t)hw));
   NVB_CUDA(counts.grow(m, hw, hw));
   NVB_CUDA(totals.grow(m, 2, 2));
-  NVB_CUDA(temp.grow(m, std::max<size_t>(temp_bytes, 1), std::max<size_t>(temp_bytes, 1)));
-  NVB_CUDA(launchGroundSortBlocks(L->dev(), hw, keys.get(), slots.get(), temp.get(), temp_bytes, m->stream));
   ExportPointsArgs a{};
-  a.layer = L->dev(), a.layer_id = layer, a.slots = slots.get() + hw, a.num_blocks = hw;
+  if (int rc = order.sort(m, L->dev(), hw, &a.slots)) return rc;
+  a.layer = L->dev(), a.layer_id = layer, a.num_blocks = hw;
   a.counts = counts.get(), a.totals = totals.get();
   a.block_size = m->block_size, a.voxel_size = m->voxel_size;
   launchExportCount(a, m->stream);
@@ -3729,38 +3911,45 @@ int64_t nvb_mapper_kernel_launches(const NvbMapper* m) { return m ? m->launches 
 // ---------------------------------------------------------------------------
 namespace {
 
-int ensureMeshLayer(NvbMapper* m) {
-  NVB_CUDA(followProjectiveSlab(m, &m->mesh, kMeshHeaderBytes));
-  // The arena state and the mesh consumer's tracker arrays: allocated with the layer, or by the next call when that failed
-  // part-way. Once they exist, both calls return at once.
-  NVB_CUDA(m->mesh_state.grow(m, kArenaInts, kArenaInts, 0));
-  return growTracker(m, m->tsdf.capacity());
+int MeshArena::create(NvbMapper* m) {
+  NVB_CUDA(state_.grow(m, kArenaInts, kArenaInts, 0));
+  return NVB_OK;
 }
 
-MeshCtx makeMeshCtx(NvbMapper* m) {
-  MeshCtx c{};
-  c.tsdf = m->tsdf.dev(), c.color = m->color.dev(), c.mesh = m->mesh.dev();
-  c.vertices = m->mesh_v.get(), c.normals = m->mesh_n.get(), c.triangles = m->mesh_t.get(), c.colors_raw = m->mesh_c.get();
-  c.colors = reinterpret_cast<uchar4*>(m->mesh_c.get());
-  c.arena_state = m->mesh_state.get();
-  c.counts = m->mesh_counts.get(), c.offsets = m->mesh_offsets.get();
-  c.block_size = m->block_size, c.voxel_size = m->voxel_size;
-  c.min_weight = m->mp.min_weight, c.cutoff_distance_m = m->mp.cutoff_distance_vox * m->voxel_size;
-  c.weld = m->mp.weld_vertices ? 1 : 0;
-  c.error = m->error_dev;
-  return c;
+void MeshArena::fill(MeshCtx* c) const {
+  c->vertices = live_.v.get(), c->normals = live_.n.get(), c->triangles = live_.t.get(), c->colors_raw = live_.c.get();
+  c->colors = reinterpret_cast<uchar4*>(live_.c.get());
+  c->arena_state = state_.get();
+  c->counts = counts_.get(), c->offsets = offsets_.get();
 }
 
-// Moves the live segments into a fresh arena of at least `need` free entries behind them (growth and garbage collection
-// are the same operation: a segment is live while a header points at it).
-int repackMeshArena(NvbMapper* m, long long need) {
+int MeshArena::reserveList(NvbMapper* m, size_t list) {
+  NVB_CUDA(counts_.growDoubling(m, list));
+  NVB_CUDA(offsets_.growDoubling(m, list));
+  return NVB_OK;
+}
+
+int MeshArena::fitUpdate(NvbMapper* m, MeshCtx* c) {
+  // the one number the host needs: does the update fit behind the arena's fill level?
+  int state[kArenaInts];
+  NVB_CUDA(cudaMemcpyAsync(state, state_.get(), sizeof(state), cudaMemcpyDeviceToHost, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  if ((long long)state[kArenaLastBase] + state[kArenaLastTotal] <= (long long)capacity()) return NVB_OK;
+  if (int rc = repack(m, state[kArenaLastTotal], *c)) return rc;
+  fill(c);
+  launchMeshScan(*c, m->stream);  // the offsets move with the fill level
+  m->launches++;
+  return NVB_OK;
+}
+
+// Growth and garbage collection are the same operation: a segment is live while a header points at it.
+int MeshArena::repack(NvbMapper* m, long long need, const MeshCtx& c) {
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   int nslots = 0;
   NVB_CUDA(m->mesh.fillLevel(&nslots));
   DeviceArray<int> sizes, new_off;
   NVB_CUDA(sizes.grow(m, (size_t)nslots + 1, (size_t)nslots + 1));
   NVB_CUDA(new_off.grow(m, (size_t)nslots + 1, (size_t)nslots + 1));
-  MeshCtx c = makeMeshCtx(m);
   launchMeshCompactSizes(c, nslots, sizes.get(), m->stream);
   std::vector<int> h((size_t)nslots + 1, 0), o((size_t)nslots + 1, 0);
   NVB_CUDA(cudaMemcpyAsync(h.data(), sizes.get(), (size_t)nslots * sizeof(int), cudaMemcpyDeviceToHost, m->stream));
@@ -3769,50 +3958,63 @@ int repackMeshArena(NvbMapper* m, long long need) {
   for (int i = 0; i < nslots; i++) o[i] = (int)live, live += h[i];
   // at least half of the arena is free behind the live data after a repack: with an update re-emitting ~1/5 of the live
   // vertices, that is several updates between repacks
-  long long cap = std::max<long long>(m->mesh_t.size(), 1 << 20);
+  long long cap = std::max<long long>(capacity(), 1 << 20);
   while (cap < 2 * (live + need)) cap *= 2;
   if (cap > 0x7fffffffll) return fail(NVB_ERR_CAPACITY, "mesh arena beyond 2^31 vertices");
   // The spare arena is the one the previous repack moved out of, never larger than `cap`: when it has the right size it
   // is reused (no cudaMalloc in the steady state).
-  NVB_CUDA(m->mesh_alt_v.grow(m, 3 * cap, 3 * cap));
-  NVB_CUDA(m->mesh_alt_n.grow(m, 3 * cap, 3 * cap));
-  NVB_CUDA(m->mesh_alt_t.grow(m, cap, cap));
-  NVB_CUDA(m->mesh_alt_c.grow(m, 4 * cap, 4 * cap));
+  NVB_CUDA(spare_.grow(m, cap));
   NVB_CUDA(cudaMemcpyAsync(new_off.get(), o.data(), (size_t)nslots * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  if (m->mesh_v.get())
-    launchMeshCompactMove(c, nslots, new_off.get(), m->mesh_alt_v.get(), m->mesh_alt_n.get(), m->mesh_alt_t.get(),
-                          m->mesh_alt_c.get(), m->num_sms, m->stream);
+  if (hasGeometry())
+    launchMeshCompactMove(c, nslots, new_off.get(), spare_.v.get(), spare_.n.get(), spare_.t.get(), spare_.c.get(), m->num_sms,
+                          m->stream);
   const int state[kArenaInts] = {(int)live, 0, (int)live, 0};
-  NVB_CUDA(cudaMemcpyAsync(m->mesh_state.get(), state, sizeof(state), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaMemcpyAsync(state_.get(), state, sizeof(state), cudaMemcpyHostToDevice, m->stream));
   NVB_CUDA(cudaStreamSynchronize(m->stream));
-  std::swap(m->mesh_v, m->mesh_alt_v), std::swap(m->mesh_n, m->mesh_alt_n), std::swap(m->mesh_t, m->mesh_alt_t);
-  std::swap(m->mesh_c, m->mesh_alt_c);
+  std::swap(live_, spare_);
   m->launches += 2;
   return NVB_OK;
+}
+
+int MeshArena::upload(NvbMapper* m, const int32_t* xyz, int n, const int** dev) {
+  const size_t ints = 3 * (size_t)n;
+  NVB_CUDA(xyz_.growDoubling(m, ints));
+  NVB_CUDA(cudaMemcpyAsync(xyz_.get(), xyz, ints * sizeof(int), cudaMemcpyHostToDevice, m->stream));
+  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  *dev = xyz_.get();
+  return NVB_OK;
+}
+
+int ensureMeshLayer(NvbMapper* m) {
+  NVB_CUDA(followProjectiveSlab(m, &m->mesh, kMeshHeaderBytes));
+  // The arena state and the mesh consumer's tracker arrays: allocated with the layer, or by the next call when that failed
+  // part-way. Once they exist, both calls return at once.
+  int rc;
+  if ((rc = m->mesh_arena.create(m))) return rc;
+  return growTracker(m, m->tsdf.capacity());
+}
+
+MeshCtx makeMeshCtx(NvbMapper* m) {
+  MeshCtx c{};
+  c.tsdf = m->tsdf.dev(), c.color = m->color.dev(), c.mesh = m->mesh.dev();
+  m->mesh_arena.fill(&c);
+  c.block_size = m->block_size, c.voxel_size = m->voxel_size;
+  c.min_weight = m->mp.min_weight, c.cutoff_distance_m = m->mp.cutoff_distance_vox * m->voxel_size;
+  c.weld = m->mp.weld_vertices ? 1 : 0;
+  c.error = m->error_dev;
+  return c;
 }
 
 // One mesh update over a device list (explicit indices, or TSDF slots from the tracker).
 int meshUpdateImpl(NvbMapper* m, const int* xyz_dev, const TrackerList& todo, int upper, bool color) {
   int rc;
   if (upper <= 0) return NVB_OK;
-  const size_t list = upper;
-  NVB_CUDA(m->mesh_counts.grow(m, list, std::max(list, 2 * m->mesh_counts.size())));
-  NVB_CUDA(m->mesh_offsets.grow(m, list, std::max(list, 2 * m->mesh_offsets.size())));
+  if ((rc = m->mesh_arena.reserveList(m, upper))) return rc;
   MeshCtx c = makeMeshCtx(m);
   c.in_xyz = xyz_dev, c.todo = todo, c.in_count_host = upper;
   launchMeshCount(c, upper, m->num_sms, m->stream);
   m->launches += 2;
-  // the one number the host needs: does the update fit behind the arena's fill level?
-  int state[kArenaInts];
-  NVB_CUDA(cudaMemcpyAsync(state, m->mesh_state.get(), sizeof(state), cudaMemcpyDeviceToHost, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
-  if ((long long)state[kArenaLastBase] + state[kArenaLastTotal] > (long long)m->mesh_t.size()) {
-    if ((rc = repackMeshArena(m, state[kArenaLastTotal]))) return rc;
-    c = makeMeshCtx(m);
-    c.in_xyz = xyz_dev, c.todo = todo, c.in_count_host = upper;
-    launchMeshScan(c, m->stream);  // the offsets move with the fill level
-    m->launches++;
-  }
+  if ((rc = m->mesh_arena.fitUpdate(m, &c))) return rc;
   launchMeshEmit(c, upper, m->num_sms, m->stream);
   m->launches += c.weld ? 2 : 1;
   if (color) {
@@ -3870,11 +4072,9 @@ int32_t nvb_mesh_integrate_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, 
   NVB_CUDA(cudaSetDevice(m->device));
   if ((rc = ensureMeshLayer(m))) return rc;
   if (num_blocks == 0) return NVB_OK;  // (:73-75)
-  const size_t ints = 3 * (size_t)num_blocks;
-  NVB_CUDA(m->mesh_xyz_dev.grow(m, ints, std::max(ints, 2 * m->mesh_xyz_dev.size())));
-  NVB_CUDA(cudaMemcpyAsync(m->mesh_xyz_dev.get(), blocks_xyz_host, ints * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
-  if ((rc = meshUpdateImpl(m, m->mesh_xyz_dev.get(), TrackerList{}, num_blocks, update_color != 0))) return rc;
+  const int* xyz_dev;
+  if ((rc = m->mesh_arena.upload(m, blocks_xyz_host, num_blocks, &xyz_dev))) return rc;
+  if ((rc = meshUpdateImpl(m, xyz_dev, TrackerList{}, num_blocks, update_color != 0))) return rc;
   NVB_CUDA(cudaStreamSynchronize(m->stream));
   return checkDeviceError(m);
 }
@@ -3886,13 +4086,10 @@ int32_t nvb_mesh_update_color(NvbMapper* m, const int32_t* blocks_xyz_host, int3
   if (rc) return rc;
   NVB_CUDA(cudaSetDevice(m->device));
   if ((rc = ensureMeshLayer(m))) return rc;
-  if (num_blocks == 0 || !m->mesh_v.get()) return NVB_OK;
-  const size_t ints = 3 * (size_t)num_blocks;
-  NVB_CUDA(m->mesh_xyz_dev.grow(m, ints, std::max(ints, 2 * m->mesh_xyz_dev.size())));
-  NVB_CUDA(cudaMemcpyAsync(m->mesh_xyz_dev.get(), blocks_xyz_host, ints * sizeof(int), cudaMemcpyHostToDevice, m->stream));
-  NVB_CUDA(cudaStreamSynchronize(m->stream));
+  if (num_blocks == 0 || !m->mesh_arena.hasGeometry()) return NVB_OK;
   MeshCtx c = makeMeshCtx(m);
-  c.in_xyz = m->mesh_xyz_dev.get(), c.in_count_host = num_blocks;
+  if ((rc = m->mesh_arena.upload(m, blocks_xyz_host, num_blocks, &c.in_xyz))) return rc;
+  c.in_count_host = num_blocks;
   launchMeshColor(c, num_blocks, m->num_sms, m->stream);
   m->launches++;
   NVB_CUDA(cudaStreamSynchronize(m->stream));
@@ -3966,12 +4163,12 @@ int32_t nvb_mesh_get_blocks(NvbMapper* m, const int32_t* blocks_xyz_host, int32_
 
 int32_t nvb_mesh_arena_stats(NvbMapper* m, int64_t out[4]) {
   if (!m || !out) return fail(NVB_ERR_INVALID_ARGUMENT, "null argument");
-  out[0] = (int64_t)m->mesh_t.size(), out[1] = out[2] = out[3] = 0;
+  out[0] = (int64_t)m->mesh_arena.capacity(), out[1] = out[2] = out[3] = 0;
   if (!m->mesh.exists()) return NVB_OK;
   NVB_CUDA(cudaSetDevice(m->device));
   NVB_CUDA(syncAll(m));
   int state[kArenaInts];
-  NVB_CUDA(cudaMemcpy(state, m->mesh_state.get(), sizeof(state), cudaMemcpyDeviceToHost));
+  NVB_CUDA(m->mesh_arena.readState(state));
   out[1] = state[kArenaUsed], out[2] = state[kArenaLastTotal], out[3] = state[kArenaGarbage];
   return NVB_OK;
 }

@@ -897,4 +897,13 @@ enum EsdfStat {
 };
 constexpr int kPhaseMaxEntries = 4000;  // EsdfCtx::phase_max: the wavefront's per-phase debug words
 
+// nvb_merge.cu: the state words of a merge of segments. launchUnionSegments takes them as `int* state`: declared with this
+// type, nvcc's code for an unrelated ESDF kernel (nvb_esdf_wave.cu) was no longer the same from one build to the next.
+struct UnionState {
+  int aabb_min[3], aabb_max[3];  // the union's AABB; INT32_MAX / INT32_MIN while it is empty
+  int error;                     // 1: the AABB does not fit the bitset
+  int words;                     // bitset words in use
+};
+static_assert(sizeof(UnionState) == 8 * sizeof(int), "UnionState layout");
+
 }  // namespace nvb

@@ -17,11 +17,11 @@ namespace {
 constexpr int kMergeThreads = 256;
 constexpr int kMergeTileWords = 64;
 
-// state: [0..2] min, [3..5] max, [6] error (1: the AABB does not fit the bitset), [7] number of bitset words in use
-__global__ void unionInitKernel(int* state) {
-  if (threadIdx.x < 3) state[threadIdx.x] = INT32_MAX;
-  else if (threadIdx.x < 6) state[threadIdx.x] = INT32_MIN;
-  else if (threadIdx.x < 8) state[threadIdx.x] = 0;
+__global__ void unionInitKernel(UnionState* state) {
+  if (threadIdx.x < 3) state->aabb_min[threadIdx.x] = INT32_MAX;
+  else if (threadIdx.x < 6) state->aabb_max[threadIdx.x - 3] = INT32_MIN;
+  else if (threadIdx.x == 6) state->error = 0;
+  else if (threadIdx.x == 7) state->words = 0;
 }
 
 __device__ __forceinline__ bool segmentEntry(const int* segs, int num_segments, int stride, int cap, long long i, int* x, int* y, int* z) {
@@ -35,7 +35,7 @@ __device__ __forceinline__ bool segmentEntry(const int* segs, int num_segments, 
   return true;
 }
 
-__global__ void unionAabbKernel(const int* __restrict__ segs, int num_segments, int stride, int cap, int* state) {
+__global__ void unionAabbKernel(const int* __restrict__ segs, int num_segments, int stride, int cap, UnionState* state) {
   int lo[3] = {INT32_MAX, INT32_MAX, INT32_MAX}, hi[3] = {INT32_MIN, INT32_MIN, INT32_MIN};
   const long long total = (long long)num_segments * cap;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -52,33 +52,37 @@ __global__ void unionAabbKernel(const int* __restrict__ segs, int num_segments, 
   }
   if ((threadIdx.x & 31) == 0 && lo[0] <= hi[0]) {
 #pragma unroll
-    for (int a = 0; a < 3; a++) atomicMin(state + a, lo[a]), atomicMax(state + 3 + a, hi[a]);
+    for (int a = 0; a < 3; a++) atomicMin(&state->aabb_min[a], lo[a]), atomicMax(&state->aabb_max[a], hi[a]);
   }
 }
 
-__device__ __forceinline__ bool unionGrid(const int* state, long long cap_bits, int* sx, int* sxy, long long* cells) {
-  if (state[0] > state[3]) return false;  // no entries
-  const long long dx = (long long)state[3] - state[0] + 1, dy = (long long)state[4] - state[1] + 1, dz = (long long)state[5] - state[2] + 1;
+__device__ __forceinline__ bool unionGrid(const UnionState* state, long long cap_bits, int* sx, int* sxy, long long* cells) {
+  const int* lo = state->aabb_min;
+  const int* hi = state->aabb_max;
+  if (lo[0] > hi[0]) return false;  // no entries
+  const long long dx = (long long)hi[0] - lo[0] + 1, dy = (long long)hi[1] - lo[1] + 1, dz = (long long)hi[2] - lo[2] + 1;
   *cells = dx * dy * dz;
   if (*cells > cap_bits) return false;
   *sx = (int)dx, *sxy = (int)(dx * dy);
   return true;
 }
 
-__global__ void unionMarkKernel(const int* __restrict__ segs, int num_segments, int stride, int cap, int* state, unsigned int* bits,
-                                long long cap_bits) {
+__global__ void unionMarkKernel(const int* __restrict__ segs, int num_segments, int stride, int cap, UnionState* state,
+                                unsigned int* bits, long long cap_bits) {
   int sx, sxy;
   long long cells;
   if (!unionGrid(state, cap_bits, &sx, &sxy, &cells)) {
-    if (blockIdx.x == 0 && threadIdx.x == 0 && state[0] <= state[3]) state[6] = 1;  // entries, but the AABB does not fit
+    // entries, but the AABB does not fit
+    if (blockIdx.x == 0 && threadIdx.x == 0 && state->aabb_min[0] <= state->aabb_max[0]) state->error = 1;
     return;
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) state[7] = (int)((cells + 31) / 32);
+  if (blockIdx.x == 0 && threadIdx.x == 0) state->words = (int)((cells + 31) / 32);
   const long long total = (long long)num_segments * cap;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     int x, y, z;
     if (segmentEntry(segs, num_segments, stride, cap, i, &x, &y, &z)) {
-      const long long lin = (long long)(x - state[0]) + (long long)(y - state[1]) * sx + (long long)(z - state[2]) * sxy;
+      const int* lo = state->aabb_min;
+      const long long lin = (long long)(x - lo[0]) + (long long)(y - lo[1]) * sx + (long long)(z - lo[2]) * sxy;
       atomicOr(bits + (lin >> 5), 1u << (lin & 31));
     }
   }
@@ -86,7 +90,7 @@ __global__ void unionMarkKernel(const int* __restrict__ segs, int num_segments, 
 
 // Ordered compaction: tile t owns 64 bitset words; its output offset is the popcount of all preceding words, which every tile
 // recomputes for itself (the bitset is a few KB in L2), so tiles are independent (the scheme of compactAllocateKernel).
-__global__ void __launch_bounds__(kMergeThreads) unionCompactKernel(const int* state, const unsigned int* bits, long long cap_bits,
+__global__ void __launch_bounds__(kMergeThreads) unionCompactKernel(const UnionState* state, const unsigned int* bits, long long cap_bits,
                                                                     int* out_xyz, int out_cap, int* out_count) {
   __shared__ int s_incl[kMergeTileWords];
   __shared__ unsigned int s_word[kMergeTileWords];
@@ -139,17 +143,17 @@ __global__ void __launch_bounds__(kMergeThreads) unionCompactKernel(const int* s
       const long long lin = (long long)(w0 + lo) * 32 + bit;
       const int o = prefix + j;
       if (o < out_cap) {
-        out_xyz[3 * o] = (int)(lin % sx) + state[0];
-        out_xyz[3 * o + 1] = (int)((lin / sx) % (sxy / sx)) + state[1];
-        out_xyz[3 * o + 2] = (int)(lin / sxy) + state[2];
+        out_xyz[3 * o] = (int)(lin % sx) + state->aabb_min[0];
+        out_xyz[3 * o + 1] = (int)((lin / sx) % (sxy / sx)) + state->aabb_min[1];
+        out_xyz[3 * o + 2] = (int)(lin / sxy) + state->aabb_min[2];
       }
     }
     __syncthreads();
   }
 }
 
-__global__ void unionClearKernel(const int* state, unsigned int* bits) {
-  const int n = state[7];
+__global__ void unionClearKernel(const UnionState* state, unsigned int* bits) {
+  const int n = state->words;
   for (int w = blockIdx.x * blockDim.x + threadIdx.x; w < n; w += gridDim.x * blockDim.x) bits[w] = 0u;
 }
 
@@ -181,8 +185,9 @@ void launchAppendFrame(const int4* frame, const int* frame_count, int* seg, int 
   appendFrameKernel<<<1, 1024, 0, stream>>>(frame, frame_count, seg, cap, error);
 }
 
-void launchUnionSegments(const int* segs, int num_segments, int stride, int cap, int* state, unsigned int* bits, long long cap_bits,
-                         int* out_xyz, int out_cap, int* out_count, cudaStream_t stream) {
+void launchUnionSegments(const int* segs, int num_segments, int stride, int cap, int* state_words, unsigned int* bits,
+                         long long cap_bits, int* out_xyz, int out_cap, int* out_count, cudaStream_t stream) {
+  UnionState* state = reinterpret_cast<UnionState*>(state_words);
   const long long total = (long long)num_segments * cap;
   int grid = (int)((total + kMergeThreads - 1) / kMergeThreads);
   grid = grid < 1 ? 1 : (grid > 592 ? 592 : grid);

@@ -214,7 +214,7 @@ TSDF_WIPE = dict(decay_factor=1e-6, decayed_weight_threshold=1e-3)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# Mesh arena (nvb_api.cu repackMeshArena): at least 2^20 entries, and after a repack at least twice the live data plus the
+# Mesh arena (nvb_api.cu MeshArena::repack): at least 2^20 entries, and after a repack at least twice the live data plus the
 # update. MESH_ARENA_TARGET: a 2 cm full-layer update grows it past 2^22 entries.
 # Freespace (nvb_api.cu updateFreespaceImpl): freespaceUpdateKernel runs on 4 CTAs per SM; H100 SXM has 132 SMs.
 # ---------------------------------------------------------------------------------------------------------------------
